@@ -1,15 +1,16 @@
 #!/usr/bin/env python
-"""hsbench-style block-mode throughput of the B200 scan runtime.
+"""hsbench-style block-mode throughput of the H100 scan runtime.
 
   python bench.py --gpus N --steps K --warmup W            (ours)
   python bench.py --impl reference --gpus N --steps K ...  (reference CPU arm)
+  python bench.py ... --dump-outputs DIR                   (also write the last timed pass's matches)
 
 Workload = BASELINE.json configs[1]: 1 000 short literals, 1 GiB synthetic corpus
-as 2^20 blocks x 1 KiB, block mode, one B200 (per rank; blocks shard by rank).
+as 2^20 blocks x 1 KiB, block mode, one H100 (per rank; blocks shard by rank).
 One "step" = one hsbench repeat GROUP: --passes-per-step (default 40) passes of the
 literal scan path over the whole resident corpus (hsbench's inner loop: every block
 through hs_scan once per repeat, -n repeats, tools/hsbench/main.cpp:503-527); the
-default --steps 10 therefore times 400 passes (~146 ms per GPU), so that a barrier
+default --steps 10 therefore times 400 passes, so that a barrier
 is < 0.5 % of the region and nvidia-smi gets its samples.  The region is timed with
 CUDA events on the launching stream, max over ranks (the wall clock with the closing
 barrier is printed beside it).  Metric: Gbit/s = 8 * corpus bytes * passes / seconds /
@@ -24,13 +25,19 @@ Prints ONE JSON line (rank 0):
              recorded by the library around it on its stream
   secondary  (N = 1) the other literal configurations of BASELINE.json, each with
              kernel-event roofline and a bit-exact check against the reference
-             runtime: config 1 through the stock hs_scan, Teddy 48, fat Teddy 96,
+             runtime (the C restatement oracle/hs_oracle.c where the reference is not
+             built): config 1 through the stock hs_scan, Teddy 48, fat Teddy 96,
              config-5 shape (50 000 literals), config-4 shape (stream set), the DFA
              engines (McClellan 8 / 16, Sheng) against the reference engines
              (N > 1) the config-5 shape sharded at 8 GiB per GPU
+
+--dump-outputs DIR writes, after the timed steps, the match list of the last timed
+pass as the caller receives it from hs_b200_fetch_matches, ordered by (block, to, id):
+DIR/matches_{id,block,to}.npy (float64) and DIR/match_count.npy.  Above DUMP_BYTES a
+fixed seeded sample of the rows is written.  The inputs are seeded, so runs with the
+same arguments can be compared output for output.
 """
 import argparse
-import hashlib
 import json
 import os
 import subprocess
@@ -44,7 +51,8 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 METRIC = "hsbench block-mode scan throughput (Gbit/s scanned), match set bit-exact vs CPU ref"
-KERNEL_SRC = os.path.join(ROOT, "hyperscan_b200", "csrc", "device", "scan_kernels.cu")
+DUMP_BYTES = 64 << 20
+H100_HBM_GBS = 3350.0   # NVIDIA H100 SXM data sheet, HBM3
 
 
 def parse():
@@ -69,6 +77,8 @@ def parse():
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "nccl"],
                     help="N>1: p2p = records stored into every rank's buffer by the confirm kernel itself over "
                          "NVLink peer memory; nccl = one all-gather per pass")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed pass's matches to DIR/*.npy (float64)")
     return ap.parse_args()
 
 
@@ -86,7 +96,7 @@ def config_of(args, n, info=None):
                      "%d blocks x %d B per GPU, block mode" % (args.lits, args.blocks, args.block_len),
          "corpus_bytes_per_gpu": args.blocks * args.block_len,
          "passes_per_step": args.passes_per_step,
-         "l2": "inputs larger than L2 (corpus >> 126 MB), no flush needed",
+         "l2": "inputs larger than L2 (corpus >> 50 MB), no flush needed",
          "sharding": "blocks sharded by rank, database replicated" if n > 1 else "single GPU"}
     if args.blocks * args.block_len <= 256 << 20:
         c["l2"] = "WARNING: corpus not much larger than L2"
@@ -141,6 +151,7 @@ class ClockSampler:
     def close(self):
         if self.proc:
             self.proc.terminate()
+            self.proc.wait()
             self.proc = None
 
     def window(self, t0, t1):
@@ -166,6 +177,16 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": mx or None, "reasons": [], "samples": 0}
         return {"sm_mhz": float(np.median(sm)), "sm_max_mhz": mx, "reasons": sorted(reasons),
                 "samples": len(sm)}
+
+
+def oracle_module():
+    """The reference runtime (oracle/_ref) where it is built, else the C restatement
+    (oracle/hs_oracle.c, built by build()): same scan_sorted / stream_collect calls."""
+    import oracle.ref as ref
+    if ref.available():
+        return ref
+    import oracle.port as port
+    return port
 
 
 def pinned_threads():
@@ -344,7 +365,7 @@ def replant(base, nblocks, block_len, lits, per_kb, seed):
     return data
 
 
-def secondary_block(capi, ref, name, lits, flags, ids, base, nblocks, block_len, peak, platform=None, passes=7):
+def secondary_block(capi, oracle, name, lits, flags, ids, base, nblocks, block_len, peak, platform=None, passes=7):
     """Kernel-event roofline + bit-exact check of one more literal configuration."""
     db = capi.compile_lit_multi(lits, flags, ids, platform=platform)
     data = replant(base, nblocks, block_len, lits, 0.01, 99)
@@ -364,7 +385,7 @@ def secondary_block(capi, ref, name, lits, flags, ids, base, nblocks, block_len,
             ms.append(sc.last_kernel_ms())
     got = capi.fetch_matches(db, sc)
     vb = min(4096, nblocks)
-    want = ref.scan_sorted(db.ptr, data, off[:vb], ln[:vb])
+    want = oracle.scan_sorted(db.ptr, data, off[:vb], ln[:vb])
     exact = bool(np.array_equal(np.sort(got[got["block"] < vb], order=["block", "to", "id"]), want))
     c = sc.counters()
     kms = float(np.median(ms))
@@ -384,13 +405,14 @@ def secondary_single_gpu(args, capi, torch, base, peak):
     import ctypes as C
     import oracle.ref as ref
     from hyperscan_b200 import synth
-    sec = {}
+    oracle = oracle_module()
+    sec = {"oracle": oracle.__name__}
     bl = args.block_len
     nb = min(args.blocks, (args.secondary_mb << 20) // bl)
 
     # configs[0]: simplegrep -- 1 literal, 1 MiB buffer, through the STOCK hs_scan (per-call latency)
     lits, flags, ids = synth.literal_set(1, min_len=6, max_len=6, seed=1)
-    out, db, data = secondary_block(capi, ref, "noodle", lits, flags, ids, base, nb, bl, peak)
+    out, db, data = secondary_block(capi, oracle, "noodle", lits, flags, ids, base, nb, bl, peak)
     one = data[: 1 << 20].tobytes()
     sc = capi.Scratch(db)
     lat = []
@@ -398,8 +420,8 @@ def secondary_single_gpu(args, capi, torch, base, peak):
         t0 = time.perf_counter()
         rc, m = capi.scan(db, one, sc)
         lat.append(time.perf_counter() - t0)
-    want = ref.scan_sorted(db.ptr, np.frombuffer(one, dtype=np.uint8), np.array([0], np.uint64),
-                           np.array([len(one)], np.uint32))
+    want = oracle.scan_sorted(db.ptr, np.frombuffer(one, dtype=np.uint8), np.array([0], np.uint64),
+                              np.array([len(one)], np.uint32))
     out.update({"hs_scan_1mib_call_ms_median": float(np.median(lat[10:]) * 1e3),
                 "hs_scan_1mib_gbit_s": len(one) * 8 / float(np.median(lat[10:])) / 1e9,
                 "hs_scan_bit_exact": sorted(m) == sorted((int(r["id"]), int(r["to"])) for r in want),
@@ -408,16 +430,16 @@ def secondary_single_gpu(args, capi, torch, base, peak):
     sec["config1_noodle_1lit"] = out
 
     lits, flags, ids = synth.literal_set(48, min_len=4, max_len=8, seed=48)
-    sec["teddy_48lits"], _, _ = secondary_block(capi, ref, "teddy48", lits, flags, ids, base, nb, bl, peak)
+    sec["teddy_48lits"], _, _ = secondary_block(capi, oracle, "teddy48", lits, flags, ids, base, nb, bl, peak)
 
     if ref.best_isa() != "corei7":
         lits, flags, ids = synth.literal_set(96, min_len=4, max_len=8, seed=96)
         plat = C.byref(capi.PlatformInfo(0, capi.HS_CPU_FEATURES_AVX2, 0, 0))
-        sec["fat_teddy_96lits"], _, _ = secondary_block(capi, ref, "fat96", lits, flags, ids, base, nb, bl, peak,
+        sec["fat_teddy_96lits"], _, _ = secondary_block(capi, oracle, "fat96", lits, flags, ids, base, nb, bl, peak,
                                                         platform=plat)
 
     lits, flags, ids = synth.literal_set(50000, min_len=4, max_len=16, caseless_frac=0.1, seed=5)
-    sec["config5_shape_50k_lits"], _, _ = secondary_block(capi, ref, "50k", lits, flags, ids, base, nb, bl, peak)
+    sec["config5_shape_50k_lits"], _, _ = secondary_block(capi, oracle, "50k", lits, flags, ids, base, nb, bl, peak)
 
     # configs[3] shape: stream set, state resident in HBM, writes from pinned host memory
     lits, flags, ids = synth.literal_set(5000, min_len=4, max_len=8, caseless_frac=0.1, seed=4)
@@ -441,7 +463,7 @@ def secondary_single_gpu(args, capi, torch, base, peak):
     ok = True
     for s in (0, ns // 2, ns - 1):                                 # 5 writes of the same 1 KiB per stream
         cat = np.tile(data[s * bl:(s + 1) * bl], rounds + 1)
-        want, err = ref.stream_collect(db.ptr, cat, np.full(rounds + 1, bl, dtype=np.uint32))
+        want, err = oracle.stream_collect(db.ptr, cat, np.full(rounds + 1, bl, dtype=np.uint32))
         exp = sorted((int(r["block"]) - 1, int(r["id"]), int(r["to"])) for r in want if int(r["block"]) >= 1)
         mine = sorted((r_, int(x["id"]), int(x["to"])) for r_, recs in enumerate(got) for x in recs[recs["block"] == s])
         ok = ok and err == 0 and mine == exp
@@ -474,11 +496,13 @@ def secondary_single_gpu(args, capi, torch, base, peak):
             if i >= 2:
                 ms.append(kms)
         vb = min(2048, ndfa)
-        want = ref.nfa_exec_blocks(eng, data, off[:vb], ln[:vb])
         def triples(r):
             t = np.stack([r["block"].astype(np.int64), r["to"].astype(np.int64), r["id"].astype(np.int64)], axis=1)
             return t[np.lexsort((t[:, 2], t[:, 1], t[:, 0]))]
-        exact = bool(np.array_equal(triples(got[got["block"] < vb]), triples(want)))
+        exact = None     # the reference engines alone run raw engine tables
+        if ref.available():
+            want = ref.nfa_exec_blocks(eng, data, off[:vb], ln[:vb])
+            exact = bool(np.array_equal(triples(got[got["block"] < vb]), triples(want)))
         kms = float(np.median(ms))
         ach = (ndfa * bl + 16 * got.size) / (kms * 1e-3) / 1e9
         sec["dfa_" + name] = {"engine_bytes": len(eng), "blocks": ndfa, "block_len": bl, "kernel_ms": kms,
@@ -507,8 +531,10 @@ def secondary_single_gpu(args, capi, torch, base, peak):
             ms.append(sc.last_kernel_ms())
     got = capi.fetch_matches(db, sc)
     vb = min(2048, ndfa)
-    want = ref.scan_sorted(db.ptr, data, off[:vb], ln[:vb])
-    exact = bool(np.array_equal(np.sort(got[got["block"] < vb], order=["block", "to", "id"]), want))
+    exact = None     # the C restatement has no automata: only the reference runtime checks this database
+    if ref.available():
+        want = ref.scan_sorted(db.ptr, data, off[:vb], ln[:vb])
+        exact = bool(np.array_equal(np.sort(got[got["block"] < vb], order=["block", "to", "id"]), want))
     kms = float(np.median(ms))
     ach = (ndfa * bl + 16 * int(got.size)) / (kms * 1e-3) / 1e9
     info = db.info()
@@ -525,21 +551,16 @@ def secondary_single_gpu(args, capi, torch, base, peak):
     return sec
 
 
-def traffic_record():
-    """dram bytes per launch from the committed ncu capture, valid only for the kernel
-    source it was taken from (profiles/traffic.json carries the source hash)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            t = json.load(f)
-        with open(KERNEL_SRC, "rb") as f:
-            sha = hashlib.sha256(f.read()).hexdigest()[:16]
-        if t.get("kernel_source_sha16") != sha:
-            return None, "profiles/traffic.json was captured from another build of scan_kernels.cu (%s != %s)" % (
-                t.get("kernel_source_sha16"), sha)
-        return t.get("dram_bytes_per_launch"), "ncu dram__bytes_read.sum + dram__bytes_write.sum of %s over %s" % (
-            t.get("kernel"), t.get("command"))
-    except (OSError, ValueError) as e:
-        return None, "no capture: %s" % e
+def dump_matches(out_dir, matches):
+    """The last timed pass's matches, ordered by (block, to, id), as float64 columns."""
+    m = np.sort(matches, order=["block", "to", "id"])
+    rows = (DUMP_BYTES - 4096) // (3 * 8)       # the .npy headers and the count fit in the rest
+    if m.size > rows:
+        m = m[np.sort(np.random.default_rng(0).choice(m.size, size=rows, replace=False))]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "match_count.npy"), np.array([matches.size], dtype=np.float64))
+    for col in ("id", "block", "to"):
+        np.save(os.path.join(out_dir, "matches_%s.npy" % col), m[col].astype(np.float64))
 
 
 def main():
@@ -590,6 +611,9 @@ def main():
     barrier()
     dt = time.perf_counter() - t0
     t1w = time.time()
+    matches = capi.fetch_matches(db, passes.last_scratch(K * P))
+    if args.dump_outputs and rank == 0:
+        dump_matches(args.dump_outputs, matches)
     wall = dt
     dt = passes.device_ms * 1e-3          # CUDA events on the launching stream; the wall clock is printed beside it
     print("[bench rank %d] %d passes: device %.3f ms (events), host run %.3f ms, with barrier %.3f ms, kernel sum %.3f ms"
@@ -624,13 +648,13 @@ def main():
 
     # ---- parity spot-check on this run's data (not timed) ----------------------
     verify = {}
-    matches = capi.fetch_matches(db, passes.last_scratch(K * P))
     verify["matches_per_pass_rank0"] = int(matches.size)
     if rank == 0 and args.verify_blocks and not args.no_cpu:
-        import oracle.ref as ref
+        oracle = oracle_module()
         vb = min(args.verify_blocks, len(off))
-        want = ref.scan_sorted(db.ptr, data, off[:vb], ln[:vb])
+        want = oracle.scan_sorted(db.ptr, data, off[:vb], ln[:vb])
         got = matches[matches["block"] < vb]
+        verify["oracle"] = oracle.__name__
         verify["verified_blocks"] = vb
         verify["bit_exact_vs_reference"] = bool(np.array_equal(np.sort(got, order=["block", "to", "id"]), want))
     if world > 1:
@@ -682,8 +706,7 @@ def main():
                "matches_delivered_per_step": int(nm), "delivered_in_block_order": ordered,
                "api": "hs_b200_scan_blocks_collect(host pinned buffer): H2D, scan + confirm kernels, D2H of the "
                       "records, report rules and (block, to, id) ordering on the host -> match array on host",
-               "bound": "one PCIe Gen5 x16 link per GPU: the H2D copy of the corpus is ~95 % of the call "
-                        "(tools/h2d_ceiling.py); the scan itself needs < 3 % of that time"}
+               "bound": "one PCIe Gen5 x16 link per GPU: the H2D copy of the corpus (tools/h2d_ceiling.py)"}
         # the same call path with the corpus ALREADY in device memory (a framework that produces its
         # input on the GPU): wrap the device buffer, scan, fetch the ordered matches to the host
         dcorp = torch.from_numpy(data).to(dev)
@@ -715,7 +738,7 @@ def main():
             peaks = json.load(f)
     except OSError:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     secondary = None
     if not args.no_secondary:
         try:
@@ -728,13 +751,12 @@ def main():
     passes.close()
 
     if rank == 0:
-        peak_src = "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+        peak_src = "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
         kms = float(np.mean(kernel_ms))
         alg_bytes = corpus_bytes + 16 * int(n)
         achieved = alg_bytes / (kms * 1e-3) / 1e9
-        traffic, traffic_src = traffic_record()
         roof = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                "peak_source": peak_src,
                 "kernel": "scanKernelPair (class-pair first stage, prefilter) + confirmKernel, CUDA events on "
                           "the launching stream around both",
                 "kernel_ms": kms, "algorithmic_bytes_per_launch": alg_bytes}
@@ -796,10 +818,10 @@ def secondary_sharded(args, capi, hdist, torch, dist, dev, world, rank, local, b
         dist.all_reduce(cnt, op=dist.ReduceOp.SUM)
     out = None
     if rank == 0:
-        import oracle.ref as ref
+        oracle = oracle_module()
         got = capi.fetch_matches(db, passes.last_scratch(T))
         vb = 2048
-        want = ref.scan_sorted(db.ptr, one, off[:vb], ln[:vb])
+        want = oracle.scan_sorted(db.ptr, one, off[:vb], ln[:vb])
         exact = bool(np.array_equal(np.sort(got[got["block"] < vb], order=["block", "to", "id"]), want))
         kmean = float(np.mean(kms))
         out = {"config5_shape_sharded": {
@@ -810,7 +832,7 @@ def secondary_sharded(args, capi, hdist, torch, dist, dev, world, rank, local, b
             "rank0_kernel_ms": kmean, "rank0_roofline_frac": (big.numel() + 16 * int(n)) / (kmean * 1e-3) / 1e9 / peak,
             "exchange": ("p2p peer stores" if passes.peerx is not None else "nccl all-gather per pass")
             if world > 1 else "none (one GPU)",
-            "rank0_verified_blocks": vb, "rank0_bit_exact_vs_reference": exact,
+            "rank0_verified_blocks": vb, "rank0_bit_exact_vs_reference": exact, "oracle": oracle.__name__,
             "note": "weak scaling: every --gpus N run prints this shape; the ratio of value_gbit_s at N=8 and "
                     "N=1 is the scaling of BASELINE configs[4]"}}
     passes.close()

@@ -73,7 +73,7 @@ int main(int argc, char *argv[]) {
         hs_free_database(database);
         return -1;
     }
-    printf("Scanning %u bytes with Hyperscan (B200 runtime %s)\n", length, hs_version());
+    printf("Scanning %u bytes with Hyperscan (H100 runtime %s)\n", length, hs_version());
     if (hs_scan(database, inputData, length, 0, scratch, eventHandler, pattern) != HS_SUCCESS) {
         fprintf(stderr, "ERROR: Unable to scan input buffer. Exiting.\n");
         hs_free_scratch(scratch);

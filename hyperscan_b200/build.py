@@ -1,11 +1,15 @@
 """Build the native libraries in-tree.
 
   hyperscan_b200/lib/libhs_b200.so   the product: C ABI (include/hs_b200.h) +
-                                     sm_100a kernels (nvcc, -gencode
-                                     arch=compute_100a,code=sm_100a)
+                                     sm_90a kernels (nvcc, -gencode
+                                     arch=compute_90a,code=sm_90a)
   oracle/_build/liboracle.so         the CPU restatement (test infrastructure)
-  oracle/_ref/libhsref_<isa>.so      the unmodified reference runtime, only when
-                                     /root/reference is present (oracle/ref/Makefile)
+  oracle/_ref/libhsref_<isa>.so      the unmodified reference runtime, only where a
+                                     checkout of intel/hyperscan 5.4.2 is found
+                                     (HS_REFERENCE overrides the default location in
+                                     build_oracle; oracle/ref/Makefile); without it the
+                                     tests use the answers recorded in
+                                     tests/golden/ref_answers
 
 Everything is rebuilt only when a source is newer than the output.
 """
@@ -18,7 +22,7 @@ CSRC = os.path.join(ROOT, "hyperscan_b200", "csrc")
 LIBDIR = os.path.join(ROOT, "hyperscan_b200", "lib")
 OBJDIR = os.path.join(LIBDIR, "obj")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 HOST_SRCS = ["host/api_host.cpp", "host/rose_build.cpp", "host/hwlm_build.cpp", "host/db_walk.cpp",
              "host/pair_table.cpp", "host/dfa_build.cpp", "host/limex_build.cpp", "host/regex_nfa.cpp"]

@@ -1,7 +1,7 @@
 /*
  * accel_kernels.cu -- the "skip to the next interesting byte" primitives of the
  * reference (src/nfa/accel.h:46-121, run_accel src/nfa/accel.c:35) as one
- * sm_100a kernel: first position in [0, len) whose byte (pair) is in the class.
+ * sm_90a kernel: first position in [0, len) whose byte (pair) is in the class.
  *
  *   vermicelli        src/nfa/vermicelli.h:43-110    byte == c  (nocase: & 0xdf)
  *   double vermicelli src/nfa/vermicelli.h:172-246   c1 at p, c2 at p+1; a
@@ -197,7 +197,7 @@ cudaError_t launchAccelFind(int type, const u8 *params, const u8 *d_buf, u64 len
     if (len == 0) {
         return cudaSuccess;
     }
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const u64 chunks = (len + 15) / 16;

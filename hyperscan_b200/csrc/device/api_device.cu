@@ -1,7 +1,7 @@
 /*
  * api_device.cu -- device half of the C ABI: scratch, corpus handles and the
  * scan entry points (include/hs_b200.h).  The thin host shim around the
- * sm_100a kernels in scan_kernels.cu:
+ * sm_90a kernels in scan_kernels.cu:
  *
  *   hs_alloc_scratch / hs_clone_scratch / hs_scratch_size / hs_free_scratch
  *        src/scratch.c:244-460 -- here a scratch owns a CUDA stream, the
@@ -45,8 +45,8 @@ std::atomic<unsigned long long> g_launches{0};
 
 /* runtime tunables (hs_b200_set_runtime_option / HSB200_* environment) */
 struct RuntimeOpts {
-    int warps = 0;           /* per CTA; 0 = what measured best for the kernel (28 in direct mode: 896
-                              * threads x 72 registers; 32 with TMA staging) */
+    int warps = 0;           /* per CTA; 0 = the kernel's default (28 in direct mode: 896 threads x 72
+                              * registers; 32 with TMA staging) */
     int tileBytes = 1024;
     int stages = 2;
     int wideFdr = 0;         /* 1: use all 8 FDR slots (u64 entries) when they fit */
@@ -55,15 +55,17 @@ struct RuntimeOpts {
     int rebuild = 1;         /* rebuild the FDR first-stage table over slots 1..4 from the literals */
     int domain = 0;          /* rebuilt table: hash domain bits (0 = as compiled) */
     int direct = 1;          /* 1: corpus straight into registers; 0: TMA-staged tiles */
-    int pfDist = 8;          /* direct mode: L2 prefetch distance in 512-byte steps */
+    int pfDist = 4;          /* direct mode: L2 prefetch distance in 512-byte steps.  On an H100 SXM (700 W)
+                              * 4 against 8 took 17 % off the Teddy-48 and noodle kernels and 3 % off FDR with
+                              * 1 000 literals, and left 5 000 / 50 000 literals unchanged (1 GiB, tools/sweep.py);
+                              * on a card limited to 400 W, whose clock is power-bound, 4 and 8 are level */
     int replicas = 1;        /* rebuilt table: copies per entry (0 = fill up to 128 KB, max 16);
-                              * measured: no gain, and a small footprint lets NCCL CTAs co-reside */
+                              * a small footprint lets NCCL CTAs co-reside */
     int queue = 2;           /* candidates go through the per-warp shared-memory queue: 0 never, 1 always,
-                              * 2 for the per-byte tables (Teddy, noodle: measured +15 %) but not for the
+                              * 2 for the per-byte tables (Teddy, noodle) but not for the
                               * FDR hash table, whose kernel is shared-memory bound either way */
-    int wide = 1;            /* 1: wide-step kernel (32-byte lanes, always queued) for FK_BYTE32 / FK_HASH32.
-                              * Measured with split=1 and 28 warps: Teddy-48 4.14 TB/s against 3.08 for the
-                              * 16-byte queued kernel, noodle 4.43 against 3.19 (profiles/r02_*) */
+    int wide = 1;            /* 1: wide-step kernel (32-byte lanes, always queued) for FK_BYTE32 / FK_HASH32,
+                              * 0: the 16-byte queued kernel */
     int split = 1;           /* 1 (with wide): scan kernel stops at the prefilter, confirmKernel finishes the
                               * candidates from a list in HBM (second half of the record ring) */
     int firstStage = 3;      /* FDR databases: 3 = class-pair tables (FK_PAIR32: two conflict-free lookups per
@@ -79,9 +81,9 @@ struct RuntimeOpts {
                               * pass many candidates), 1 = by the modelled first-stage rate */
     int bigSetClasses = 4;   /* ... classes left to the second byte (pair table = 4 KiB each) */
     int dfaIlp = 1;          /* DFA kernels: blocks walked by one lane at a time; 2 = two interleaved state chains
-                              * per lane, measured SLOWER (half the warps per block count: profiles/r02_dfa.log) */
+                              * per lane (half the warps for the same block count) */
     int fatPair = 1;         /* fat Teddy (16 buckets): 1 = class-pair first stage with the buckets folded onto
-                              * 8 bits (3.0 TB/s), 0 = 64-bit per-byte entries (FK_BYTE64, 1.75 TB/s) */
+                              * 8 bits, 0 = 64-bit per-byte entries (FK_BYTE64) */
     int chunkMB = 128;       /* host->device pipeline granularity */
     int initialRing = 1 << 20;
 };
@@ -885,7 +887,7 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
             }
             programsOk = walkConfirm(bc, h->length, im->confOff, 8 * oct, &im->exhaustible, &tails);
             if (oct == 2 && g_opts.fatPair && g_opts.split && !tails.empty()) {
-                /* 49..96 literals: the class-pair kernel filters them at 3 TB/s where the 64-bit
+                /* 49..96 literals: the class-pair kernel filters them faster than the 64-bit
                  * per-byte entries cost two shared-memory wavefronts a byte; its 8 bucket bits
                  * carry buckets i and i + 8 (confirmKernel unfolds them) */
                 table.clear();
@@ -1199,9 +1201,8 @@ hs_error_t planScan(const hs_scratch *s, const DevImage *im, ScanPlan *pl) {
         pl->cfg.stride = 1;
         /* candidate path: per-lane queue entries while candidates are rare; one entry per
          * word with candidates for sets that saturate the first stage (heavy=2 forces it).
-         * The modelled rate assumes independent slots and is ~30x below what is measured:
-         * 0.0015 modelled is ~40 candidates per KiB, where the per-word path starts to win
-         * (profiles/r02_sweep_candidate_paths.log) */
+         * The modelled rate assumes independent slots and is ~30x below the observed one:
+         * 0.0015 modelled is ~40 candidates per KiB, where the per-word path starts to win */
         pl->cfg.queued = g_opts.heavy == 2 || (g_opts.heavy == 1 && im->pairRate > 0.0015) ? 2 : 1;
         pl->cfg.wide = 0;
         pl->cfg.split = 1;
@@ -1524,9 +1525,11 @@ hs_error_t hs_valid_platform(void) {
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
         return HS_ARCH_ERROR;
     }
-    int major = 0;
+    /* the library carries sm_90a code only, which loads on compute capability 9.0 alone */
+    int major = 0, minor = 0;
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, 0);
-    return major >= 10 ? HS_SUCCESS : HS_ARCH_ERROR;
+    cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, 0);
+    return major == 9 && minor == 0 ? HS_SUCCESS : HS_ARCH_ERROR;
 }
 
 unsigned long long hs_b200_launch_count(void) { return g_launches.load(); }

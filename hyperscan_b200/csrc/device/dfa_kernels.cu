@@ -1,5 +1,5 @@
 /*
- * dfa_kernels.cu -- the reference's DFA engines in block mode on sm_100a:
+ * dfa_kernels.cu -- the reference's DFA engines in block mode on sm_90a:
  * McClellan with 8- and 16-bit states (incl. Sherman states) and Sheng, run
  * over every block of a corpus, straight from the engines' own bytes.
  *
@@ -323,7 +323,7 @@ __device__ u32 shermanNext(const u8 *nfa, u32 shermanOffset, u32 shermanLimit, u
  *
  * One thread per block means 32 lanes reading 32 different blocks, and a dependent lookup
  * per byte.  Two things decide the speed: how a warp's corpus bytes arrive and how many
- * instructions a byte costs (the first version: 29 per byte, issue bound at 0.5-1.0 TB/s).
+ * instructions a byte costs (the first version: 29 per byte, issue bound).
  *
  *  - A warp stages its 32 blocks through shared memory: CH bytes of every block per
  *    refill, loaded coalesced (8 lanes x 16 B = 128 contiguous bytes of one block, four

@@ -1,6 +1,6 @@
 /*
  * kernels.h -- launch interface between the C-ABI shim (api_device.cu) and the
- * sm_100a scan kernels (scan_kernels.cu).  Plain PODs only.
+ * sm_90a scan kernels (scan_kernels.cu).  Plain PODs only.
  */
 #ifndef HSB200_KERNELS_H
 #define HSB200_KERNELS_H

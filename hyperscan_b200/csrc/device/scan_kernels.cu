@@ -1,5 +1,5 @@
 /*
- * scan_kernels.cu -- sm_100a scan kernels for the floating literal matcher:
+ * scan_kernels.cu -- sm_90a scan kernels for the floating literal matcher:
  * first-stage shift-OR filter (FDR / Teddy / noodle tables), hash confirm and
  * the pure-literal rose program, all on the device.
  *
@@ -1944,7 +1944,7 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelPair(const HSB_GRID_CONSTAN
  * c[e-3] | c[e-2] << 5 | c[e-1] << 10: the bank of a lookup is then (c[e-3] + c[e-2] +
  * c[e-1]) mod 32, not c[e-3] alone -- with the plain fields every lane whose byte e-3 is
  * no letter (class 0: half of printable text) hits bank 0 at a different address, 11
- * wavefronts per lookup measured (profiles/r02_ncu_gram_plain_fields.csv) against ~3.5 now. */
+ * wavefronts per lookup against ~3.5 now. */
 struct GramQueue {
     static constexpr u32 SLOTS = 64;                      /* < 32 pending + <= 32 appended per round */
     static constexpr u32 RUN_START = 16 * SLOTS;          /* entry = {word offset in the run, 4-bit candidate map,

@@ -197,7 +197,7 @@ hs_error_t hs_serialize_database(const hs_database_t *db, char **bytes,
 }
 
 /* Any combination of the three NO* feature bits is a database some reference
- * build could have produced; the B200 engines consume every table variant, so
+ * build could have produced; the H100 engines consume every table variant, so
  * (unlike src/database.c:115-124) none of them is a platform mismatch. */
 static hs_error_t checkPlatform(u64 p) {
     const u64 known = PLATFORM_NOAVX2 | PLATFORM_NOAVX512 | PLATFORM_NOAVX512VBMI;
@@ -889,7 +889,7 @@ static hs_error_t compileCommon(const char *const *expressions,
                                        (int)i};
                 }
                 if (f & HS_FLAG_SOM_LEFTMOST) {
-                    throw CompileError{"HS_FLAG_SOM_LEFTMOST is not supported by the B200 "
+                    throw CompileError{"HS_FLAG_SOM_LEFTMOST is not supported by the H100 "
                                        "literal compiler yet.", (int)i};
                 }
                 {
@@ -938,7 +938,7 @@ static hs_error_t compileCommon(const char *const *expressions,
                 continue;
             }
             if (f & HS_FLAG_SOM_LEFTMOST) {
-                throw CompileError{"HS_FLAG_SOM_LEFTMOST is not supported by the B200 "
+                throw CompileError{"HS_FLAG_SOM_LEFTMOST is not supported by the H100 "
                                    "literal compiler yet.", (int)i};
             }
             pats.push_back(p);

@@ -2,7 +2,7 @@
  * hwlm_build.h -- host-side literal-matcher table builder (interface).
  *
  * Emits HWLM tables (noodle / Teddy / FDR + hash confirm + flood control) in
- * the reference's byte layouts, so the same bytes can be consumed by the B200
+ * the reference's byte layouts, so the same bytes can be consumed by the H100
  * kernels and by the unmodified reference runtime (used as the parity oracle).
  * Mirrors the role of hwlmBuildProto()/hwlmBuild() (reference:
  * src/hwlm/hwlm_build.cpp:107-212).
@@ -35,7 +35,7 @@ struct HwlmBuildOpts {
     int forceEngine = -1;       /* -1 auto; 0 FDR; 3..18 Teddy id (tests) */
     int forceDomain = 0;        /* FDR: 9..15, 0 = auto */
     int forceStride = 0;        /* FDR: 1,2,4, 0 = auto */
-    int maxDomain = 15;         /* cap for the auto choice (B200: smem-resident table) */
+    int maxDomain = 15;         /* cap for the auto choice (H100: smem-resident table) */
     bool allowFlood = true;
 };
 

@@ -1,6 +1,6 @@
 /*
  * ref_layout.h -- byte layouts of the Hyperscan 5.4.2 database ("bytecode")
- * structures that the B200 runtime consumes and the host literal compiler
+ * structures that the H100 runtime consumes and the host literal compiler
  * emits.  The serialised database format is the drop-in boundary
  * (BASELINE.json north_star: "serialised database format stays"), so these
  * are restated here field-for-field; every struct cites the reference header

@@ -1,5 +1,5 @@
 /*
- * hs_b200.h -- C ABI of libhs_b200.so, the B200-native block-mode scan runtime
+ * hs_b200.h -- C ABI of libhs_b200.so, the H100-native block-mode scan runtime
  * for Hyperscan databases.
  *
  * Part 1 re-declares, with identical names, argument meaning and error
@@ -256,7 +256,7 @@ hs_error_t hs_scan_vector(const hs_database_t *db, const char *const *data,
                           match_event_handler onEvent, void *context);
 
 /* ------------------------------------------------------------------------
- * Part 2: B200 batch / device-resident extension
+ * Part 2: H100 batch / device-resident extension
  * ---------------------------------------------------------------------- */
 
 /* One match record as the device writes it (16 bytes; SURVEY.md section 8d). */

@@ -7,7 +7,7 @@ oracle/ holds the CPU side of every parity check:
                 compiled where they lie by oracle/ref/Makefile) + ref_driver.c.
                 Because our host compiler emits reference-format databases, the
                 reference's own hs_scan()/hwlmExec() consume the very same bytes
-                the B200 kernels consume.  This is the strongest oracle ("kind":
+                the H100 kernels consume.  This is the strongest oracle ("kind":
                 "reference" in bench.py's cpu_baseline).
   hs_oracle.c   plain-C restatement of the block-mode literal path (FDR / Teddy
                 / noodle first stage, hash confirm, pure-literal rose program,

@@ -1,15 +1,29 @@
 """ctypes binding of the unmodified reference runtime built into oracle/_ref/
-(see oracle/ref/Makefile, oracle/ref/ref_driver.c).  TEST INFRASTRUCTURE ONLY."""
+(see oracle/ref/Makefile, oracle/ref/ref_driver.c).  TEST INFRASTRUCTURE ONLY.
+
+Where the reference runtime is not built, the calls below that tests use answer
+from tests/golden/ref_answers/: what the reference returned to the same call of
+the same test on the same inputs, recorded by running the suite with the
+reference built and HS_REF_RECORD=1.  (A compiled database is not part of the
+key: its bytes are not reproducible from run to run, while what it must match
+is.)  A question that was never recorded is an error, not a skip.
+HS_REF_REPLAY=1 uses the recordings even where the reference is built."""
+import atexit
 import ctypes as C
+import hashlib
 import os
 
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 REF_DIR = os.path.join(_HERE, "_ref")
+ANSWERS_DIR = os.path.join(os.path.dirname(_HERE), "tests", "golden", "ref_answers")
 REC_DTYPE = np.dtype([("id", "<u4"), ("block", "<u4"), ("to", "<u8")])
 
 _libs = {}
+_answers = None      # digest -> (records, value), loaded from ANSWERS_DIR on first use
+_recorded = {}       # test module -> {digest: (records, value)}, written at exit under HS_REF_RECORD=1
+_calls = {}          # test node id -> reference calls made so far
 
 
 def cpu_flags():
@@ -37,7 +51,122 @@ def best_isa():
 
 
 def available():
+    """The reference runtime itself is built (oracle/_ref)."""
     return os.path.exists(os.path.join(REF_DIR, "libhsref_%s.so" % best_isa()))
+
+
+def live():
+    return available() and os.environ.get("HS_REF_REPLAY") != "1"
+
+
+def usable():
+    """Reference answers can be had: from the runtime itself, or recorded."""
+    return live() or bool(_load_answers())
+
+
+def _load_answers():
+    global _answers
+    if _answers is None:
+        _answers = {}
+        if os.path.isdir(ANSWERS_DIR):
+            for name in sorted(os.listdir(ANSWERS_DIR)):
+                if name.endswith(".npz"):
+                    _answers.update(_read_answers(os.path.join(ANSWERS_DIR, name)))
+    return _answers
+
+
+def _read_answers(path):
+    """Stored as columns, block and `to` as differences from the previous record."""
+    z = np.load(path)
+    recs = np.zeros(int(z["counts"].sum()), REC_DTYPE)
+    recs["id"] = z["id"]
+    recs["block"] = np.cumsum(z["dblock"])
+    recs["to"] = np.cumsum(z["dto"])
+    starts = np.zeros(z["counts"].size + 1, np.int64)
+    starts[1:] = np.cumsum(z["counts"])
+    return {k.tobytes(): (recs[starts[i]:starts[i + 1]], int(v)) for i, (k, v) in enumerate(zip(z["keys"], z["vals"]))}
+
+
+def _write_answers():
+    """One file per test module, split into parts of at most ~800 KB; processes that record
+    at the same time (a test's worker processes) take turns."""
+    import fcntl
+    os.makedirs(ANSWERS_DIR, exist_ok=True)
+    fd = os.open(ANSWERS_DIR, os.O_RDONLY)
+    fcntl.flock(fd, fcntl.LOCK_EX)
+    try:
+        _merge_answers()
+    finally:
+        os.close(fd)
+
+
+def _merge_answers():
+    for module, new in _recorded.items():
+        olds = [os.path.join(ANSWERS_DIR, f) for f in os.listdir(ANSWERS_DIR)
+                if f == module + ".npz" or (f.startswith(module + ".") and f.endswith(".npz"))]
+        table = {}
+        for path in olds:
+            table.update(_read_answers(path))
+            os.remove(path)
+        table.update(new)
+        keys = sorted(table)
+        parts = 1
+        while True:
+            paths = [os.path.join(ANSWERS_DIR, module + ("" if parts == 1 else ".%d" % i) + ".npz") for i in range(parts)]
+            for i, path in enumerate(paths):
+                _save_answers(path, {k: table[k] for k in keys[i::parts]})
+            size = max(os.path.getsize(path) for path in paths)
+            if size <= 800 << 10:
+                break
+            for path in paths:
+                os.remove(path)
+            parts = parts * size // (700 << 10) + 1
+
+
+def _save_answers(path, table):
+    keys = sorted(table)
+    recs = np.concatenate([table[k][0] for k in keys] + [np.zeros(0, REC_DTYPE)])
+    np.savez_compressed(path, keys=np.frombuffer(b"".join(keys), dtype=np.uint8).reshape(-1, 8),
+                        vals=np.array([table[k][1] for k in keys], dtype=np.int64),
+                        counts=np.array([table[k][0].size for k in keys], dtype=np.uint32), id=recs["id"],
+                        dblock=np.diff(recs["block"].astype(np.int64), prepend=0),
+                        dto=np.diff(recs["to"].astype(np.int64), prepend=0))
+
+
+def _part(x):
+    if isinstance(x, (bytes, bytearray, memoryview, np.ndarray)):
+        b = _u8(x).tobytes()
+    else:
+        b = repr(x).encode()
+    return len(b).to_bytes(8, "little") + b
+
+
+def recorded(kind, parts, compute):
+    """The reference's answer to question `kind` on inputs `parts`, asked by the
+    running test: compute() with the reference runtime where it is built, else the
+    recorded answer.  An answer is (records as REC_DTYPE, an int)."""
+    test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
+    node = "::".join([os.path.basename(test[0])] + test[1:])     # module.py::test[params]
+    n = _calls.get(node, 0)
+    _calls[node] = n + 1
+    h = hashlib.sha1(kind.encode())
+    for p in [node, n] + list(parts):
+        h.update(_part(p))
+    key = h.digest()[:8]
+    if live():
+        recs, val = compute()
+        recs = np.ascontiguousarray(recs, dtype=REC_DTYPE)
+        if os.environ.get("HS_REF_RECORD") == "1":
+            module = os.path.splitext(node.split("::")[0])[0] or "other"
+            if not _recorded:
+                atexit.register(_write_answers)
+            _recorded.setdefault(module, {})[key] = (recs.copy(), int(val))
+        return recs, int(val)
+    ans = _load_answers().get(key)
+    if ans is None:
+        raise RuntimeError("no recorded reference answer for this %s call (%s): build the reference runtime "
+                           "(oracle/ref/Makefile) and rerun the test with HS_REF_RECORD=1" % (kind, key.hex()))
+    return ans[0].copy(), ans[1]
 
 
 def lib(isa=None):
@@ -45,8 +174,8 @@ def lib(isa=None):
     if isa not in _libs:
         path = os.path.join(REF_DIR, "libhsref_%s.so" % isa)
         if not os.path.exists(path):
-            raise RuntimeError("reference runtime not built: %s (run `make -C oracle/ref` where "
-                               "/root/reference exists)" % path)
+            raise RuntimeError("reference runtime not built: %s (run `make -C oracle/ref REF=<intel/hyperscan "
+                               "5.4.2 checkout>`)" % path)
         L = C.CDLL(path)
         vp = C.c_void_p
         L.ref_scan_collect.restype = C.c_long
@@ -82,6 +211,13 @@ def _u8(data):
 def scan_collect(db_ptr, data, offsets, lengths, stop_after=0, isa=None, cap=None):
     """Reference hs_scan() over blocks; records in delivery order.
     Returns (records, last_error)."""
+    off = np.ascontiguousarray(offsets, dtype=np.uint64)
+    ln = np.ascontiguousarray(lengths, dtype=np.uint32)
+    return recorded("scan_collect", [data, off, ln, stop_after, isa],
+                    lambda: _scan_collect(db_ptr, data, off, ln, stop_after, isa, cap))
+
+
+def _scan_collect(db_ptr, data, offsets, lengths, stop_after, isa, cap):
     a = _u8(data)
     keep = a if a.size else np.zeros(1, dtype=np.uint8)
     off = np.ascontiguousarray(offsets, dtype=np.uint64)
@@ -102,6 +238,12 @@ def scan_collect(db_ptr, data, offsets, lengths, stop_after=0, isa=None, cap=Non
 def stream_collect(db_ptr, data, write_lengths, stop_after=0, isa=None):
     """Reference streaming scan of `data` cut into consecutive writes; records
     (id, write index, to = stream offset) in delivery order + last error."""
+    wl = np.ascontiguousarray(write_lengths, dtype=np.uint32)
+    return recorded("stream_collect", [data, wl, stop_after, isa],
+                    lambda: _stream_collect(db_ptr, data, wl, stop_after, isa))
+
+
+def _stream_collect(db_ptr, data, write_lengths, stop_after, isa):
     a = _u8(data)
     keep = a if a.size else np.zeros(1, dtype=np.uint8)
     wl = np.ascontiguousarray(write_lengths, dtype=np.uint32)
@@ -123,6 +265,12 @@ def vector_collect(db_ptr, data, buf_lengths, stop_after=0, isa=None):
     """Reference hs_scan_vector over `data` cut into consecutive buffers; records
     (id, 0, to counted from the first buffer) in delivery order + the call's
     return code."""
+    bl = np.ascontiguousarray(buf_lengths, dtype=np.uint32)
+    return recorded("vector_collect", [data, bl, stop_after, isa],
+                    lambda: _vector_collect(db_ptr, data, bl, stop_after, isa))
+
+
+def _vector_collect(db_ptr, data, buf_lengths, stop_after, isa):
     a = _u8(data)
     keep = a if a.size else np.zeros(1, dtype=np.uint8)
     bl = np.ascontiguousarray(buf_lengths, dtype=np.uint32)
@@ -190,7 +338,13 @@ def bench_blocks(db_ptr, data, offsets, lengths, threads, repeats, isa=None):
 
 
 def hwlm_exec(hwlm_bytes, data, start=0, groups=0xFFFFFFFFFFFFFFFF, stop_after=0, isa=None):
-    """Reference hwlmExec() on a raw HWLM table (64-byte aligned copy)."""
+    """Reference hwlmExec() on a raw HWLM table (64-byte aligned copy): [(end, id)]."""
+    recs, _ = recorded("hwlm_exec", [data, start, groups, stop_after, isa],
+                       lambda: (_hwlm_exec(hwlm_bytes, data, start, groups, stop_after, isa), 0))
+    return [(int(r["to"]), int(r["id"])) for r in recs]
+
+
+def _hwlm_exec(hwlm_bytes, data, start, groups, stop_after, isa):
     raw = np.zeros(len(hwlm_bytes) + 64, dtype=np.uint8)
     o = (-raw.ctypes.data) % 64
     raw[o:o + len(hwlm_bytes)] = np.frombuffer(hwlm_bytes, dtype=np.uint8)
@@ -202,12 +356,20 @@ def hwlm_exec(hwlm_bytes, data, start=0, groups=0xFFFFFFFFFFFFFFFF, stop_after=0
     out = np.zeros(cap, dtype=REC_DTYPE)
     n = lib(isa).ref_hwlm_exec(raw.ctypes.data + o, buf.ctypes.data + 64, a.size, start, groups,
                                out.ctypes.data, cap, stop_after)
-    return [(int(r["to"]), int(r["id"])) for r in out[:min(n, cap)]]
+    return out[:min(n, cap)]
 
 
 def nfa_exec_blocks(nfa_bytes, data, offsets, lengths, isa=None, cap=1 << 20):
     """Reference nfaExecMcClellan8_B / 16_B / nfaExecSheng_B over every block (offset 0):
     the callbacks as records sorted by (block, to, id)."""
+    off = np.ascontiguousarray(offsets, dtype=np.uint64)
+    ln = np.ascontiguousarray(lengths, dtype=np.uint32)
+    recs, _ = recorded("nfa_exec_blocks", [data, off, ln, isa],
+                       lambda: (_nfa_exec_blocks(nfa_bytes, data, off, ln, isa, cap), 0))
+    return recs
+
+
+def _nfa_exec_blocks(nfa_bytes, data, offsets, lengths, isa, cap):
     a = _u8(data)
     keep = a if a.size else np.zeros(1, dtype=np.uint8)
     off = np.ascontiguousarray(offsets, dtype=np.uint64)

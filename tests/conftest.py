@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 # HSB200_EMU=1: run the tests marked `gpu` on a CPU against the SIMT-emulated build of the
@@ -43,11 +43,13 @@ def real_gpu():
 
 @pytest.fixture(scope="session")
 def ref():
-    """The unmodified reference runtime (oracle/_ref); skipped if not built."""
+    """The unmodified reference runtime (oracle/_ref), or where it is not built, its answers
+    recorded under tests/golden/ref_answers (oracle/ref.py)."""
     import oracle.ref as r
-    if not r.available():
-        pytest.skip("oracle/_ref not built (needs /root/reference at build time)")
-    r.lib()
+    if not r.usable():
+        pytest.skip("neither oracle/_ref nor recorded reference answers")
+    if r.live():
+        r.lib()
     return r
 
 

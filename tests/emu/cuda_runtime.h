@@ -23,7 +23,7 @@ enum cudaMemcpyKind { cudaMemcpyHostToHost, cudaMemcpyHostToDevice, cudaMemcpyDe
 enum { cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2, cudaEventBlockingSync = 1,
        cudaIpcMemLazyEnablePeerAccess = 1 };
 enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount, cudaDevAttrMaxSharedMemoryPerBlockOptin,
-                      cudaDevAttrComputeCapabilityMajor };
+                      cudaDevAttrComputeCapabilityMajor, cudaDevAttrComputeCapabilityMinor };
 enum cudaFuncAttribute { cudaFuncAttributeMaxDynamicSharedMemorySize };
 
 static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
@@ -39,7 +39,8 @@ static inline cudaError_t cudaDeviceGetAttribute(int *v, cudaDeviceAttr a, int) 
         break;
     }
     case cudaDevAttrMaxSharedMemoryPerBlockOptin: *v = 232448; break;
-    case cudaDevAttrComputeCapabilityMajor: *v = 10; break;
+    case cudaDevAttrComputeCapabilityMajor: *v = 9; break;
+    case cudaDevAttrComputeCapabilityMinor: *v = 0; break;
     }
     return cudaSuccess;
 }

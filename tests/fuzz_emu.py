@@ -21,7 +21,7 @@ import build_emu  # noqa: E402
 import oracle.ref as ref  # noqa: E402
 
 DEFAULTS = {"warps": 0, "tile_bytes": 1024, "stages": 2, "wide_fdr": 0, "stride": 1, "prefilter": 1, "rebuild": 1,
-            "domain": 0, "direct": 1, "replicas": 1, "pf_dist": 8, "queue": 2, "first_stage": 3, "wide": 1,
+            "domain": 0, "direct": 1, "replicas": 1, "pf_dist": 4, "queue": 2, "first_stage": 3, "wide": 1,
             "split": 1, "big_set": 0, "big_set_classes": 4, "heavy": 1, "gram": 1, "fat_pair": 1,
             "initial_ring": 1 << 20}
 

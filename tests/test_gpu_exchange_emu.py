@@ -2,7 +2,7 @@
 stores every record into every rank's exchange buffer, publishCountKernel the
 count) with both "ranks" in one process -- possible only on the SIMT emulator,
 where a peer mapping is a plain pointer.  On real GPUs this path is exercised
-by bench.py --gpus N under torchrun (profiles/r01_bench_n2.json, _n4.json)."""
+by bench.py --gpus N under torchrun."""
 import ctypes as C
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""Parity of the B200 scan path (through the C ABI) against the unmodified
+"""Parity of the H100 scan path (through the C ABI) against the unmodified
 reference runtime scanning the SAME database, and against the definition-level
 brute-force oracle.  Bit-exact on the sorted (block, to, id) multiset."""
 import numpy as np

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""hsbench for the B200 runtime: the reference benchmark's command line, inputs and report
+"""hsbench for the H100 runtime: the reference benchmark's command line, inputs and report
 (tools/hsbench/main.cpp:190-240 options, :503-527 scan loops, :721-725 Mbit/s, :773-860 the
 report) over this library's C ABI.
 
@@ -123,7 +123,7 @@ def mbps(seconds, nbytes):
 
 
 def main(argv=None):
-    ap = argparse.ArgumentParser(description="hsbench over the B200 runtime", add_help=True)
+    ap = argparse.ArgumentParser(description="hsbench over the H100 runtime", add_help=True)
     ap.add_argument("-e", dest="expr", required=True, help="signature file or directory")
     ap.add_argument("-s", dest="sigfile", help="file with the signature IDs to use")
     ap.add_argument("-z", dest="sigid", type=int, help="one signature ID to use")
@@ -189,7 +189,7 @@ def main(argv=None):
     scratch = capi.Scratch(db)
 
     print("Signatures:        %s" % args.expr)
-    print("Hyperscan info:    B200 runtime (hs-b200), reference-format database; %s"
+    print("Hyperscan info:    H100 runtime (hs-b200), reference-format database; %s"
           % ("pure literal" if info.runtime_impl == 1 else "single outfix" if info.runtime_impl == 2 else "rose"))
     print("Expression count:  %d" % len(sigs))
     print("Bytecode size:     %d bytes" % info.bytecode_len)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Condense an .ncu-rep (ncu --set full) into the metrics profiles/README.md quotes:
-  python tools/ncu_summary.py gpurun_out/x.ncu-rep > profiles/r02_ncu_x_summary.csv"""
+"""Condense an .ncu-rep (ncu --set full) into a CSV of the key metrics:
+  python tools/ncu_summary.py x.ncu-rep > x_summary.csv"""
 import csv
 import subprocess
 import sys

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Instruction histogram per kernel of the built CUDA objects (cuobjdump -sass), so that
 claims about what a loop compiles to -- how many LDS / PRMT / LOP3 per step, whether the
-TMA build carries UBLKCP, stack use -- can be checked against a committed artefact.
+TMA build carries UBLKCP, stack use -- can be checked.
 
-  python tools/sass_summary.py > profiles/r02_sass_summary.txt
+  python tools/sass_summary.py > sass_summary.txt
 """
 import collections
 import hashlib

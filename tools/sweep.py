@@ -19,7 +19,7 @@ DEFAULT = ("replicas=1;replicas=2;replicas=4;domain=12,replicas=8;domain=12,repl
            "domain=14,replicas=2;domain=14,replicas=1;domain=10,replicas=16;domain=12,replicas=8,warps=20;"
            "replicas=4,direct=0,warps=24,tile_bytes=1024;replicas=4,tile_bytes=4096")
 BASE = {"warps": 0, "tile_bytes": 1024, "stages": 2, "wide_fdr": 0, "stride": 1, "prefilter": 1,
-        "rebuild": 1, "domain": 0, "direct": 1, "replicas": 1, "pf_dist": 8, "queue": 2, "first_stage": 3, "wide": 1,
+        "rebuild": 1, "domain": 0, "direct": 1, "replicas": 1, "pf_dist": 4, "queue": 2, "first_stage": 3, "wide": 1,
         "split": 1, "big_set": 0, "big_set_classes": 4, "heavy": 1, "gram": 1, "fat_pair": 1}
 
 
