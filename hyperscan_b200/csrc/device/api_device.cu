@@ -43,47 +43,23 @@ const size_t FRONT_PAD = 256;         /* readable bytes before corpus position 0
 
 std::atomic<unsigned long long> g_launches{0};
 
-/* runtime tunables (hs_b200_set_runtime_option / HSB200_* environment) */
+/* runtime tunables (hs_b200_set_runtime_option / HSB200_* environment): the scan
+ * geometry, and two switches that force either side of a choice the library
+ * otherwise makes from the database */
 struct RuntimeOpts {
-    int warps = 0;           /* per CTA; 0 = the kernel's default (28 in direct mode: 896 threads x 72
-                              * registers; 32 with TMA staging) */
+    int warps = 0;           /* per CTA; 0 = 28 (896 threads x 72 registers) */
     int tileBytes = 1024;
-    int stages = 2;
-    int wideFdr = 0;         /* 1: use all 8 FDR slots (u64 entries) when they fit */
-    int stride = 1;          /* first-stage sampling stride (0 = as compiled into the FDR table) */
-    int prefilter = 1;       /* shared-memory bitmap in front of the hash confirm */
-    int rebuild = 1;         /* rebuild the FDR first-stage table over slots 1..4 from the literals */
-    int domain = 0;          /* rebuilt table: hash domain bits (0 = as compiled) */
-    int direct = 1;          /* 1: corpus straight into registers; 0: TMA-staged tiles */
-    int pfDist = 4;          /* direct mode: L2 prefetch distance in 512-byte steps.  On an H100 SXM (700 W)
+    int pfDist = 4;          /* L2 prefetch distance (kernels.h ScanParams.pfDist).  On an H100 SXM (700 W)
                               * 4 against 8 took 17 % off the Teddy-48 and noodle kernels and 3 % off FDR with
                               * 1 000 literals, and left 5 000 / 50 000 literals unchanged (1 GiB, tools/sweep.py);
                               * on a card limited to 400 W, whose clock is power-bound, 4 and 8 are level */
-    int replicas = 1;        /* rebuilt table: copies per entry (0 = fill up to 128 KB, max 16);
-                              * a small footprint lets NCCL CTAs co-reside */
-    int queue = 2;           /* candidates go through the per-warp shared-memory queue: 0 never, 1 always,
-                              * 2 for the per-byte tables (Teddy, noodle) but not for the
-                              * FDR hash table, whose kernel is shared-memory bound either way */
-    int wide = 1;            /* 1: wide-step kernel (32-byte lanes, always queued) for FK_BYTE32 / FK_HASH32,
-                              * 0: the 16-byte queued kernel */
-    int split = 1;           /* 1 (with wide): scan kernel stops at the prefilter, confirmKernel finishes the
-                              * candidates from a list in HBM (second half of the record ring) */
-    int firstStage = 3;      /* FDR databases: 3 = class-pair tables (FK_PAIR32: two conflict-free lookups per
-                              * byte), 1 = two-byte hash table (FK_HASH32, ~3.3-way bank conflicts), 2 = per-byte
-                              * table (FK_BYTE32, conflict-free, many more candidates), 0 = choose between 1
-                              * and 2 by the modelled candidate rate of the per-byte table */
-    int bigSet = 0;          /* FK_PAIR32: sets that would overfill the 32 KiB bitmap trade classes of the
-                              * second byte for a large contiguous bitmap */
     int gram = 1;            /* FDR sets: 1 = class 4-gram first stage (FK_GRAM4) for sets that would fill the
                               * pair kernel's 32 KiB bitmap beyond 10 % (all literals >= 4 bytes), 2 = whenever
                               * possible, 0 = never */
     int heavy = 1;           /* FK_PAIR32 candidate path: 0 = per-lane entries, 2 = per-word entries (sets that
                               * pass many candidates), 1 = by the modelled first-stage rate */
-    int bigSetClasses = 4;   /* ... classes left to the second byte (pair table = 4 KiB each) */
     int dfaIlp = 1;          /* DFA kernels: blocks walked by one lane at a time; 2 = two interleaved state chains
                               * per lane (half the warps for the same block count) */
-    int fatPair = 1;         /* fat Teddy (16 buckets): 1 = class-pair first stage with the buckets folded onto
-                              * 8 bits, 0 = 64-bit per-byte entries (FK_BYTE64) */
     int chunkMB = 128;       /* host->device pipeline granularity */
     int initialRing = 1 << 20;
 };
@@ -97,17 +73,9 @@ void initOpts() {
     g_optsInit = true;
     struct { const char *env; int *v; } e[] = {
         {"HSB200_WARPS", &g_opts.warps},       {"HSB200_TILE", &g_opts.tileBytes},
-        {"HSB200_STAGES", &g_opts.stages},     {"HSB200_WIDE_FDR", &g_opts.wideFdr},
         {"HSB200_CHUNK_MB", &g_opts.chunkMB},  {"HSB200_RING", &g_opts.initialRing},
-        {"HSB200_STRIDE", &g_opts.stride},     {"HSB200_PREFILTER", &g_opts.prefilter},
-        {"HSB200_REBUILD", &g_opts.rebuild},   {"HSB200_DOMAIN", &g_opts.domain},
-        {"HSB200_DIRECT", &g_opts.direct},     {"HSB200_REPLICAS", &g_opts.replicas},
-        {"HSB200_PF_DIST", &g_opts.pfDist},    {"HSB200_QUEUE", &g_opts.queue},
-        {"HSB200_FIRST_STAGE", &g_opts.firstStage}, {"HSB200_WIDE", &g_opts.wide},
-        {"HSB200_SPLIT", &g_opts.split},       {"HSB200_BIG_SET", &g_opts.bigSet},
-        {"HSB200_BIG_SET_CLASSES", &g_opts.bigSetClasses}, {"HSB200_HEAVY", &g_opts.heavy},
-        {"HSB200_GRAM", &g_opts.gram},         {"HSB200_FAT_PAIR", &g_opts.fatPair},
-        {"HSB200_DFA_ILP", &g_opts.dfaIlp}};
+        {"HSB200_PF_DIST", &g_opts.pfDist},    {"HSB200_HEAVY", &g_opts.heavy},
+        {"HSB200_GRAM", &g_opts.gram},         {"HSB200_DFA_ILP", &g_opts.dfaIlp}};
     for (auto &x : e) {
         const char *s = getenv(x.env);
         if (s && *s) {
@@ -130,7 +98,7 @@ struct DevImage {
     u32 tableBytes = 0;
     u8 *d_bitmap = nullptr;
     u32 bitmapBytes = 0, bitmapShift = 0, keyBytes = 0;
-    u32 pairBytes = 0, bitmapHoles = 0, bitmapBits = 0; /* FK_PAIR32 layout (kernels.h) */
+    u32 pairBytes = 0, bitmapBits = 0; /* FK_PAIR32 layout (kernels.h) */
     u32 bucketFold = 0;
     u32 nfaOffset = 0, nfaLength = 0;   /* FK_OUTFIX: the sole engine (bytecode offset, NFA.length) */
     DfaParams nfaParams;                /* ... and what launchDfa needs to know about it */
@@ -140,10 +108,7 @@ struct DevImage {
     u8 *d_bitmap2 = nullptr; /* second level (HBM / L2) for large literal sets */
     u32 bitmap2Shift = 0;
     int kind = FK_BYTE32;
-    int stride = 1;
     int slotBase = 0;
-    u32 repShift = 0;
-    u32 indexMask = 0;
     u32 confOff = 0, engineOff = 0;
     u32 confirmKind = CK_FDR;
     u64 groups = 0;
@@ -385,7 +350,7 @@ bool buildGramTables(const std::vector<LitTail> &tails, std::vector<u8> *classWo
         memcpy(classWords->data() + 4 * b, &e, 4);
     }
     /* word index c[e-3] + 33 c[e-2] + 1025 c[e-1] (kernels.h FK_GRAM4): sized like the kernel's window */
-    bitmap->assign((size_t)scanSmemBytes(FK_GRAM4, 0, 0, 0, 0, 0, 0) - 65536, 0);
+    bitmap->assign((size_t)scanSmemBytes(FK_GRAM4, 0, 0, 0) - 65536, 0);
     for (const LitTail &t : tails) {
         /* classes each of the last four bytes can take: [0] = byte e-3 ... [3] = byte e */
         u32 opts[4] = {0, 0, 0, 0}; /* bitmask over classes */
@@ -413,105 +378,6 @@ bool buildGramTables(const std::vector<LitTail> &tails, std::vector<u8> *classWo
         }
     }
     return true;
-}
-
-/* First-stage table rebuilt from the literal tails (LitInfo v/msk) and their
- * bucket assignment: u32 entry = 4 slots x 8 buckets indexed by the FDR hash
- * (two bytes & domain mask, src/fdr/fdr.c:157-170); slot i stands for suffix
- * distance i + slotBase.  With slotBase 1 the sample at x tests the pairs
- * (char 1, char 0) .. (char 4, char 3): every character of a 4-byte tail is in a
- * full two-byte sample, which the reference's slot 0 (second byte unknown)
- * cannot give, and literals of 5+ bytes gain a sample.  Same construction as
- * setupTab (src/fdr/fdr_compile.cpp:527-632): bit SET = impossible. */
-std::vector<u8> rebuildHashTable(const std::vector<LitTail> &tails, u32 domain, u32 slotBase) {
-    const u32 entries = 1u << domain, dmask = entries - 1;
-    std::vector<u32> tab(entries, 0xffffffffu);
-    u32 dead = 0;
-    const u32 hiBits = domain - 8;
-    for (const LitTail &t : tails) {
-        for (u32 i = 0; i < 4; i++) {
-            const u32 p = i + slotBase;
-            const u32 bit = 1u << (8 * i + t.bucket);
-            if (p >= t.size) {
-                dead |= bit; /* shorter literal: this slot cannot constrain the bucket */
-                continue;
-            }
-            const u8 c0 = (u8)(t.v >> (8 * (7 - p))), m0 = (u8)(t.msk >> (8 * (7 - p)));
-            u8 c1 = 0, m1 = 0; /* p == 0: the following byte is unknown */
-            if (p > 0) {
-                c1 = (u8)(t.v >> (8 * (8 - p)));
-                m1 = (u8)(t.msk >> (8 * (8 - p)));
-            }
-            const u8 hm = (u8)((1u << hiBits) - 1);
-            bool seen1[256] = {false};
-            for (u32 b1 = 0; b1 < 256; b1++) {
-                if ((b1 & m1) != c1 || seen1[b1 & hm]) {
-                    continue;
-                }
-                seen1[b1 & hm] = true;
-                for (u32 b0 = 0; b0 < 256; b0++) {
-                    if ((b0 & m0) == c0) {
-                        tab[(b0 | (b1 << 8)) & dmask] &= ~bit;
-                    }
-                }
-            }
-        }
-    }
-    std::vector<u8> out((size_t)entries * 4);
-    for (u32 i = 0; i < entries; i++) {
-        const u32 e = tab[i] & ~dead;
-        memcpy(&out[(size_t)i * 4], &e, 4);
-    }
-    return out;
-}
-
-/* Per-byte first-stage table for an FDR literal set: entry b, slot i, bucket k
- * is CLEAR iff some literal of bucket k can have byte b at suffix distance i
- * (caseless letters through LitInfo.msk).  The Teddy construction
- * (src/fdr/teddy_compile.cpp:440-509) applied to the FDR buckets: a weaker
- * filter than the two-byte hash, but its 256-row table is replicated per lane,
- * so the lookups are bank-conflict free.  *rate = modelled candidates per byte
- * on uniformly random printable ASCII. */
-std::vector<u8> buildByteTable(const std::vector<LitTail> &tails, double *rate) {
-    u32 tab[256];
-    for (u32 b = 0; b < 256; b++) {
-        tab[b] = 0xffffffffu;
-    }
-    u32 dead = 0;
-    for (const LitTail &t : tails) {
-        for (u32 i = 0; i < 4; i++) {
-            const u32 bit = 1u << (8 * i + t.bucket);
-            if (i >= t.size) {
-                dead |= bit;
-                continue;
-            }
-            const u8 c = (u8)(t.v >> (8 * (7 - i))), m = (u8)(t.msk >> (8 * (7 - i)));
-            for (u32 b = 0; b < 256; b++) {
-                if ((b & m) == c) {
-                    tab[b] &= ~bit;
-                }
-            }
-        }
-    }
-    std::vector<u8> out(256 * 4);
-    double total = 0;
-    for (u32 k = 0; k < 8; k++) {
-        double pr = 1;
-        for (u32 i = 0; i < 4; i++) {
-            u32 n = 0;
-            for (u32 b = 0x20; b < 0x7f; b++) {
-                n += !(((tab[b] & ~dead) >> (8 * i + k)) & 1);
-            }
-            pr *= n / 95.0;
-        }
-        total += pr;
-    }
-    *rate = total;
-    for (u32 b = 0; b < 256; b++) {
-        const u32 e = tab[b] & ~dead;
-        memcpy(&out[b * 4], &e, 4);
-    }
-    return out;
 }
 
 /* What launchDfa needs to know about a serialized engine (struct NFA + McClellan 8 / 16,
@@ -697,84 +563,64 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
     /* FK_PAIR32 / FK_GRAM4 tables from the literals' tails (FDR sets, and fat Teddy with its 16
      * buckets folded onto 8 first-stage bits) */
     auto pairStage = [&](bool allowGram) {
-        int dev = 0, maxSmem = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&maxSmem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-                u32 minSize = 8;
-                for (const LitTail &t : tails) {
-                    minSize = std::min(minSize, t.size);
-                }
-                im->kind = FK_PAIR32;
-                im->stride = 1;
-                im->slotBase = minSize >= 2 ? 1 : 0;
-                /* shared memory: 64 KiB class rows + pair table + (large sets) bitmap +
-                 * queues.  Small sets: 32 x 32 classes (128 KiB pair table), the 32 KiB
-                 * bitmap in the class rows' upper halves.  Sets whose keys would fill that
-                 * bitmap beyond ~10 %: the pair filter is saturated anyway, so the second
-                 * byte gets few classes and the freed space a large contiguous bitmap. */
-                std::vector<u32> keys;
-                u32 kb = 0;
-                const bool keyed = g_opts.prefilter && tailKeys(tails, &kb, &keys);
-                const bool large = keyed && keys.size() * 10 > 262144; /* would fill the 32 KiB bitmap > 10 % */
-                std::vector<u8> gramBitmap;
-                /* measured crossover (DESIGN.md section 3.7): 5 000 literals (12.5 k keys) scan
-                 * 10 % faster through the 4-gram kernel, 1 000 literals 38 % slower */
-                const bool gramWorth = keys.size() >= 10000;
-                if (allowGram && (g_opts.gram == 2 || (g_opts.gram == 1 && gramWorth)) && keyed && kb == 4 &&
-                    buildGramTables(tails, &table, &gramBitmap)) {
-                    /* the pair evidence saturates for such sets: exact class 4-gram membership
-                     * instead (FK_GRAM4), exact raw 4-byte keys in L2 behind it */
-                    im->kind = FK_GRAM4;
-                    im->keyBytes = 4;
-                    pairBitmap.swap(gramBitmap);
-                    /* second level in L2: one BYTE per slot = the buckets of the literals whose
-                     * raw 4-byte key hashes there (~64 slots per key, <= 64 MB), so that a
-                     * survivor reaches confirm with its real buckets, not all eight */
-                    u32 lg2 = 16;
-                    while (lg2 < 26 && (1ull << lg2) < (u64)keys.size() * 64) {
-                        lg2++;
-                    }
-                    pairBitmap2.assign((size_t)1 << lg2, 0);
-                    for (const LitTail &t : tails) {
-                        const u32 v = (u32)(t.v >> 32), care = (u32)(t.msk >> 32), dc = ~care;
-                        u32 sub = 0;
-                        do {
-                            const u32 k = (v & care) | sub;
-                            pairBitmap2[(k * 0x85EBCA6Bu) >> (32 - lg2)] |= (u8)(1u << (t.bucket & 7));
-                            sub = (sub - dc) & dc;
-                        } while (sub);
-                    }
-                    im->bitmap2Shift = 32 - lg2;
-                    return;
-                }
-                {
-                const bool big = large && g_opts.bigSet != 0;
-                PairTables pt;
-                buildPairTables(tails, (u32)im->slotBase, &pt, 32, big ? (u32)std::max(1, g_opts.bigSetClasses) : 32);
-                im->pairBytes = pt.nClass1 * 4096;
-                im->pairRate = pt.modelRate;
-                if (getenv("HSB200_TRACE")) {
-                    fprintf(stderr, "[hs_b200] class-pair tables: %u x %u classes, modelled %.4f candidates/byte, "
-                                    "%zu prefilter keys%s\n", pt.nClass0, pt.nClass1, pt.modelRate, keys.size(),
-                            big ? " (large-set layout)" : "");
-                }
-                table.resize(sizeof(pt.classWord) + sizeof(pt.pair));
-                memcpy(table.data(), pt.classWord, sizeof(pt.classWord));
-                memcpy(table.data() + sizeof(pt.classWord), pt.pair, sizeof(pt.pair));
-                if (keyed) {
-                    im->keyBytes = kb;
-                    im->bitmapHoles = big ? 0 : 1;
-                    u32 bits = 262144;
-                    if (big) {
-                        /* everything the pair table and 27 queues leave of the 227 KiB */
-                        const u32 queues = (u32)scanSmemBytes(FK_PAIR32, 0, 0, 0, 0, 0, 27) - 65536u;
-                        const u32 room = (u32)maxSmem - 65536u - im->pairBytes - queues;
-                        bits = (room & ~127u) * 8;
-                    }
-                    im->bitmapBits = bits;
-                    buildPairBitmaps(keys, bits, &pairBitmap, &pairBitmap2, &im->bitmap2Shift);
-                }
-                }
+        u32 minSize = 8;
+        for (const LitTail &t : tails) {
+            minSize = std::min(minSize, t.size);
+        }
+        im->kind = FK_PAIR32;
+        im->slotBase = minSize >= 2 ? 1 : 0;
+        /* shared memory: 64 KiB class rows (the 32 KiB prefilter bitmap in their upper
+         * halves) + 32 x 32 classes (128 KiB pair table) + queues */
+        std::vector<u32> keys;
+        u32 kb = 0;
+        const bool keyed = tailKeys(tails, &kb, &keys);
+        std::vector<u8> gramBitmap;
+        /* measured crossover (DESIGN.md section 3.7): 5 000 literals (12.5 k keys) scan
+         * 10 % faster through the 4-gram kernel, 1 000 literals 38 % slower */
+        const bool gramWorth = keys.size() >= 10000;
+        if (allowGram && (g_opts.gram == 2 || (g_opts.gram == 1 && gramWorth)) && keyed && kb == 4 &&
+            buildGramTables(tails, &table, &gramBitmap)) {
+            /* the pair evidence saturates for such sets: exact class 4-gram membership
+             * instead (FK_GRAM4), exact raw 4-byte keys in L2 behind it */
+            im->kind = FK_GRAM4;
+            im->keyBytes = 4;
+            pairBitmap.swap(gramBitmap);
+            /* second level in L2: one BYTE per slot = the buckets of the literals whose
+             * raw 4-byte key hashes there (~64 slots per key, <= 64 MB), so that a
+             * survivor reaches confirm with its real buckets, not all eight */
+            u32 lg2 = 16;
+            while (lg2 < 26 && (1ull << lg2) < (u64)keys.size() * 64) {
+                lg2++;
+            }
+            pairBitmap2.assign((size_t)1 << lg2, 0);
+            for (const LitTail &t : tails) {
+                const u32 v = (u32)(t.v >> 32), care = (u32)(t.msk >> 32), dc = ~care;
+                u32 sub = 0;
+                do {
+                    const u32 k = (v & care) | sub;
+                    pairBitmap2[(k * 0x85EBCA6Bu) >> (32 - lg2)] |= (u8)(1u << (t.bucket & 7));
+                    sub = (sub - dc) & dc;
+                } while (sub);
+            }
+            im->bitmap2Shift = 32 - lg2;
+            return;
+        }
+        PairTables pt;
+        buildPairTables(tails, (u32)im->slotBase, &pt, 32, 32);
+        im->pairBytes = pt.nClass1 * 4096;
+        im->pairRate = pt.modelRate;
+        if (getenv("HSB200_TRACE")) {
+            fprintf(stderr, "[hs_b200] class-pair tables: %u x %u classes, modelled %.4f candidates/byte, "
+                            "%zu prefilter keys\n", pt.nClass0, pt.nClass1, pt.modelRate, keys.size());
+        }
+        table.resize(sizeof(pt.classWord) + sizeof(pt.pair));
+        memcpy(table.data(), pt.classWord, sizeof(pt.classWord));
+        memcpy(table.data() + sizeof(pt.classWord), pt.pair, sizeof(pt.pair));
+        if (keyed) {
+            im->keyBytes = kb;
+            im->bitmapBits = 262144;
+            buildPairBitmaps(keys, im->bitmapBits, &pairBitmap, &pairBitmap2, &im->bitmap2Shift);
+        }
     };
     if (hw->type == HWLM_ENGINE_NOOD) {
         /* single literal: one bucket, slots = the last <= 4 bytes of msk/cmp
@@ -784,7 +630,6 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
         im->confirmKind = CK_NOODLE;
         im->engineOff = engOff;
         im->kind = FK_BYTE32;
-        im->stride = 1;
         table.assign(256 * 4, 0);
         for (u32 b = 0; b < 256; b++) {
             u32 e = 0;
@@ -808,91 +653,30 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
         im->confirmKind = CK_FDR;
         im->confOff = engOff + f.confOffset;
         if (f.engineID == 0) {
-            const u32 entries = 1u << f.domain;
-            const u8 *src = bc + engOff + FDR_TABLE_OFFSET;
-            im->stride = f.stride;
-            im->indexMask = f.domainMask;
-            int dev = 0, maxSmem = 0;
-            cudaGetDevice(&dev);
-            cudaDeviceGetAttribute(&maxSmem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-            const size_t wideNeed = (size_t)entries * 8 + 48 * 1024;
             programsOk = walkConfirm(bc, h->length, im->confOff, 8, &im->exhaustible, &tails);
-            double byteRate = 1;
-            std::vector<u8> byteTab;
-            if (g_opts.firstStage != 1) {
-                byteTab = buildByteTable(tails, &byteRate);
-            }
-            if (g_opts.wideFdr && wideNeed <= (size_t)maxSmem) {
-                im->kind = FK_HASH64;
-                table.assign(src, src + (size_t)entries * 8);
-            } else if (g_opts.firstStage == 3) {
-                pairStage(true);
-            } else if (g_opts.firstStage == 2 || (g_opts.firstStage == 0 && byteRate < 0.01)) {
-                im->kind = FK_BYTE32;
-                im->stride = 1;
-                im->slotBase = 0;
-                table.swap(byteTab);
-            } else if (g_opts.rebuild) {
-                u32 minSize = 8, d = f.domain;
-                for (const LitTail &t : tails) {
-                    minSize = std::min(minSize, t.size);
-                }
-                if (g_opts.domain >= 9 && g_opts.domain <= 15) {
-                    d = (u32)g_opts.domain;
-                }
-                im->kind = FK_HASH32;
-                im->slotBase = minSize >= 2 ? 1 : 0;
-                im->indexMask = (1u << d) - 1;
-                std::vector<u8> one = rebuildHashTable(tails, d, (u32)im->slotBase);
-                /* copies of every entry in adjacent words: lane l reads copy
-                 * l & (R-1), so a lookup's lanes fall into R bank groups */
-                u32 R = 1;
-                const u32 want = g_opts.replicas > 0 ? (u32)g_opts.replicas : 16;
-                while (R * 2 <= want && one.size() * R * 2 <= 128u * 1024) {
-                    R *= 2;
-                }
-                im->repShift = (u32)__builtin_ctz(R);
-                table.resize(one.size() * R);
-                for (size_t i = 0; i < one.size() / 4; i++) {
-                    for (u32 g = 0; g < R; g++) {
-                        memcpy(&table[(i * R + g) * 4], &one[i * 4], 4);
-                    }
-                }
-            } else {
-                im->kind = FK_HASH32; /* FDR suffix slots 0..3 as compiled */
-                table.resize((size_t)entries * 4);
-                for (u32 i = 0; i < entries; i++) {
-                    memcpy(&table[(size_t)i * 4], src + (size_t)i * 8, 4);
-                }
-            }
+            pairStage(true);
         } else if (teddyIdValid(f.engineID)) {
-            /* per-byte entry: slot m = lo_m[b & 15] | hi_m[b >> 4]
-             * (src/fdr/teddy.c:918-969, teddy_compile.cpp:440-509) */
-            const u32 nm = teddyNumMasks(f.engineID);
             const u32 oct = teddyNumBuckets(f.engineID) / 8;
-            const u8 *mb = bc + engOff + TEDDY_MASK_OFFSET;
-            im->stride = 1;
-            im->kind = oct == 2 ? FK_BYTE64 : FK_BYTE32;
-            table.assign(256 * 4 * oct, 0);
-            for (u32 b = 0; b < 256; b++) {
-                for (u32 o = 0; o < oct; o++) {
-                    u32 e = 0;
-                    for (u32 m = 0; m < nm; m++) {
-                        const u8 *lo = mb + ((2 * m) * oct + o) * 16;
-                        const u8 *hi = mb + ((2 * m + 1) * oct + o) * 16;
-                        e |= (u32)(u8)(lo[b & 15] | hi[b >> 4]) << (8 * m);
-                    }
-                    memcpy(&table[(b * oct + o) * 4], &e, 4);
-                }
-            }
             programsOk = walkConfirm(bc, h->length, im->confOff, 8 * oct, &im->exhaustible, &tails);
-            if (oct == 2 && g_opts.fatPair && g_opts.split && !tails.empty()) {
-                /* 49..96 literals: the class-pair kernel filters them faster than the 64-bit
-                 * per-byte entries cost two shared-memory wavefronts a byte; its 8 bucket bits
+            if (oct == 2) {
+                /* fat Teddy (49..96 literals): the class-pair kernel with 8 bucket bits that
                  * carry buckets i and i + 8 (confirmKernel unfolds them) */
-                table.clear();
                 pairStage(false);
                 im->bucketFold = 1;
+            } else {
+                /* per-byte entry: slot m = lo_m[b & 15] | hi_m[b >> 4]
+                 * (src/fdr/teddy.c:918-969, teddy_compile.cpp:440-509) */
+                const u32 nm = teddyNumMasks(f.engineID);
+                const u8 *mb = bc + engOff + TEDDY_MASK_OFFSET;
+                im->kind = FK_BYTE32;
+                table.assign(256 * 4, 0);
+                for (u32 b = 0; b < 256; b++) {
+                    u32 e = 0;
+                    for (u32 m = 0; m < nm; m++) {
+                        e |= (u32)(u8)(mb[2 * m * 16 + (b & 15)] | mb[(2 * m + 1) * 16 + (b >> 4)]) << (8 * m);
+                    }
+                    memcpy(&table[b * 4], &e, 4);
+                }
             }
         } else {
             delete im;
@@ -914,7 +698,7 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
     if (im->kind == FK_PAIR32 || im->kind == FK_GRAM4) {
         bitmap.swap(pairBitmap);
         bitmap2.swap(pairBitmap2);
-    } else if (g_opts.prefilter) {
+    } else {
         bitmap = buildBitmap(tails, &im->keyBytes, &im->bitmapShift, &bitmap2, &im->bitmap2Shift);
     }
     im->bitmapBytes = (u32)bitmap.size();
@@ -983,9 +767,8 @@ struct hs_scratch {
     cudaEvent_t evDone;       /* counters of the pending scan have landed on the host */
     std::vector<cudaEvent_t> *chunkEvents;
     std::vector<DevImage *> *images;
-    DevMatch *d_out;
+    DevMatch *d_out;         /* 2 * outCap records: the ring, then the scan kernels' candidate list */
     u32 outCap;
-    bool ringSplit;          /* d_out holds 2 * outCap records: ring + candidate list (split mode) */
     u32 *d_counters;
     u32 *h_counters;         /* pinned */
     hs_b200_corpus *inlineCorpus; /* staging for hs_scan / hs_b200_scan_blocks */
@@ -1065,19 +848,15 @@ hs_error_t findImage(hs_scratch *s, const hs_database_t *db, const DevImage **ou
 }
 
 hs_error_t growRing(hs_scratch *s, u32 cap) {
-    initOpts();
-    const bool split = true; /* second half = candidate list of the split kernels (FK_PAIR32 always) */
-    if (cap <= s->outCap && (s->ringSplit || !split)) {
+    if (cap <= s->outCap) {
         return HS_SUCCESS;
     }
-    cap = std::max(cap, s->outCap);
     DeviceGuard guard(s->device);
     DevMatch *n = nullptr;
-    CUDA_TRY(cudaMalloc(&n, (size_t)cap * sizeof(DevMatch) * (split ? 2 : 1)));
+    CUDA_TRY(cudaMalloc(&n, (size_t)cap * sizeof(DevMatch) * 2));
     cudaFree(s->d_out);
     s->d_out = n;
     s->outCap = cap;
-    s->ringSplit = split;
     return HS_SUCCESS;
 }
 
@@ -1140,121 +919,43 @@ u32 detectPitch(const u64 *off, const u32 *len, size_t n) {
 
 struct ScanPlan {
     LaunchCfg cfg;
-    u32 tileBytes, nstages;
+    u32 tileBytes, pfDist;
 };
 
 hs_error_t planScan(const hs_scratch *s, const DevImage *im, ScanPlan *pl) {
     initOpts();
+    memset(&pl->cfg, 0, sizeof(pl->cfg));
     if (im->kind == FK_OUTFIX) { /* one launch over all blocks once the corpus has arrived (launchRange) */
-        memset(&pl->cfg, 0, sizeof(pl->cfg));
         pl->tileBytes = 1u << 20;
-        pl->nstages = 0;
+        pl->pfDist = 0;
         return HS_SUCCESS;
     }
-    const int direct = g_opts.direct ? 1 : 0;
-    int warps = g_opts.warps > 0 ? std::min(32, g_opts.warps) : (direct ? 28 : 32);
-    u32 tile = (u32)std::max(512, g_opts.tileBytes) & ~511u;
-    u32 stages = (u32)std::max(2, std::min(8, g_opts.stages));
-    /* shrink until the table + staging fit the opt-in shared memory */
-    int stride = im->stride;
-    if ((g_opts.stride == 1 || g_opts.stride == 2 || g_opts.stride == 4) &&
-        (im->kind == FK_HASH32 || im->kind == FK_HASH64)) {
-        stride = g_opts.stride; /* any sampling subset is a sound filter */
+    /* the wide kernel (FK_BYTE32) is built for 768, 896 and 1024 threads, the pair and
+     * gram kernels for 768 and 896; as many warps as the shared memory has queues for */
+    const bool wide = im->kind == FK_BYTE32;
+    int warps = g_opts.warps > 0 ? std::min(wide ? 32 : 28, g_opts.warps) : 28;
+    const u32 tableBytes = im->kind == FK_PAIR32 ? im->pairBytes : im->tableBytes;
+    while (warps > 1 && scanSmemBytes(im->kind, tableBytes, im->bitmapBytes, warps) > (size_t)s->maxSmem) {
+        warps--;
     }
-    if (im->kind == FK_GRAM4) {
-        warps = std::min(warps, 28);
-        while (warps > 1 && scanSmemBytes(FK_GRAM4, 0, 0, 0, 0, 0, warps) > (size_t)s->maxSmem) {
-            warps--;
-        }
-        pl->cfg.smemBytes = scanSmemBytes(FK_GRAM4, 0, 0, 0, 0, 0, warps);
-        if (pl->cfg.smemBytes > (size_t)s->maxSmem || !s->ringSplit) {
-            return HS_NOMEM;
-        }
-        pl->cfg.kind = im->kind;
-        pl->cfg.slotBase = 0;
-        pl->cfg.direct = 1;
-        pl->cfg.stride = 1;
-        pl->cfg.queued = 1;
-        pl->cfg.wide = 0;
-        pl->cfg.split = 1;
-        pl->cfg.grid = s->smCount;
-        pl->cfg.warps = warps;
-        pl->tileBytes = tile;
-        pl->nstages = (u32)std::max(0, std::min(64, g_opts.pfDist));
-        return HS_SUCCESS;
-    }
-    if (im->kind == FK_PAIR32) {
-        /* class-pair kernel: direct loads, stride 1, queued candidates, split confirm;
-         * as many warps as the queues leave room for (896 threads x 72 registers at most) */
-        const u32 contiguous = im->bitmapHoles ? 0 : im->bitmapBytes;
-        warps = std::min(warps, 28);
-        while (warps > 1 && scanSmemBytes(FK_PAIR32, im->pairBytes, contiguous, 0, 0, 0, warps) > (size_t)s->maxSmem) {
-            warps--;
-        }
-        pl->cfg.smemBytes = scanSmemBytes(FK_PAIR32, im->pairBytes, contiguous, 0, 0, 0, warps);
-        if (pl->cfg.smemBytes > (size_t)s->maxSmem || !s->ringSplit) {
-            return HS_NOMEM;
-        }
-        pl->cfg.kind = im->kind;
-        pl->cfg.slotBase = im->slotBase;
-        pl->cfg.direct = 1;
-        pl->cfg.stride = 1;
-        /* candidate path: per-lane queue entries while candidates are rare; one entry per
-         * word with candidates for sets that saturate the first stage (heavy=2 forces it).
-         * The modelled rate assumes independent slots and is ~30x below the observed one:
-         * 0.0015 modelled is ~40 candidates per KiB, where the per-word path starts to win */
-        pl->cfg.queued = g_opts.heavy == 2 || (g_opts.heavy == 1 && im->pairRate > 0.0015) ? 2 : 1;
-        pl->cfg.wide = 0;
-        pl->cfg.split = 1;
-        pl->cfg.grid = s->smCount;
-        pl->cfg.warps = warps;
-        pl->tileBytes = tile;
-        pl->nstages = (u32)std::max(0, std::min(64, g_opts.pfDist));
-        return HS_SUCCESS;
-    }
-    const bool byteKind = im->kind == FK_BYTE32 || im->kind == FK_BYTE64;
-    const int wide = g_opts.wide && direct && stride == 1 && (im->kind == FK_BYTE32 || im->kind == FK_HASH32);
-    const int queued = direct && stride == 1 && (g_opts.queue == 1 || (g_opts.queue == 2 && byteKind));
-    const int split = wide && g_opts.split && s->ringSplit;
-    if (direct && !(wide && split)) {
-        warps = std::min(warps, 28); /* direct kernels are built for 896 threads (72 registers); the
-                                      * split wide variant also for 1024 (64 registers, spill-free) */
-    }
-    if (wide) {
-        tile = std::max(1024u, tile & ~1023u); /* a warp-iteration covers 1 KiB */
-    }
-    for (;;) {
-        const size_t need = scanSmemBytes(im->kind, im->tableBytes, im->bitmapBytes, direct ? 0 : warps,
-                                          stages, tile, wide ? -warps : queued ? warps : 0);
-        if (need <= (size_t)s->maxSmem) {
-            pl->cfg.smemBytes = need;
-            break;
-        }
-        if (stages > 2) {
-            stages--;
-        } else if (tile > 1024) {
-            tile >>= 1;
-        } else if (warps > 4) {
-            warps -= 4;
-        } else if (tile > 512) {
-            tile >>= 1;
-        } else if (warps > 1) {
-            warps--;
-        } else {
-            return HS_NOMEM;
-        }
+    pl->cfg.smemBytes = scanSmemBytes(im->kind, tableBytes, im->bitmapBytes, warps);
+    if (pl->cfg.smemBytes > (size_t)s->maxSmem) {
+        return HS_NOMEM;
     }
     pl->cfg.kind = im->kind;
     pl->cfg.slotBase = im->slotBase;
-    pl->cfg.direct = direct;
-    pl->cfg.stride = stride;
-    pl->cfg.queued = queued;
-    pl->cfg.wide = wide;
-    pl->cfg.split = split;
+    /* pair-kernel candidate path: per-lane queue entries while candidates are rare; one entry
+     * per word with candidates for sets that saturate the first stage (heavy=2 forces it).
+     * The modelled rate assumes independent slots and is ~30x below the observed one:
+     * 0.0015 modelled is ~40 candidates per KiB, where the per-word path starts to win */
+    pl->cfg.heavy = im->kind == FK_PAIR32 && (g_opts.heavy == 2 || (g_opts.heavy == 1 && im->pairRate > 0.0015));
     pl->cfg.grid = s->smCount;
     pl->cfg.warps = warps;
-    pl->tileBytes = tile;
-    pl->nstages = direct ? (u32)std::max(0, std::min(64, g_opts.pfDist)) : stages;
+    pl->tileBytes = (u32)std::max(512, g_opts.tileBytes) & ~511u;
+    if (wide) {
+        pl->tileBytes = std::max(1024u, pl->tileBytes & ~1023u); /* a warp-iteration covers 1 KiB */
+    }
+    pl->pfDist = (u32)std::max(0, std::min(64, g_opts.pfDist));
     return HS_SUCCESS;
 }
 
@@ -1265,7 +966,7 @@ void fillParams(const hs_scratch *s, const DevImage *im, const hs_b200_corpus *c
     p->corpusBytes = c->bytes;
     p->readableEnd = c->readableEnd;
     p->tileBytes = pl.tileBytes;
-    p->nstages = pl.nstages;
+    p->pfDist = pl.pfDist;
     p->blockOff = c->d_off;
     p->blockLen = c->d_len;
     p->nblocks = (u32)c->nblocks;
@@ -1274,12 +975,9 @@ void fillParams(const hs_scratch *s, const DevImage *im, const hs_b200_corpus *c
     p->bc = im->d_bc;
     p->table = im->d_table;
     p->tableBytes = im->tableBytes;
-    p->indexMask = im->indexMask;
-    p->repShift = im->repShift;
     p->bitmap = im->d_bitmap;
     p->bitmapBytes = im->bitmapBytes;
     p->pairBytes = im->pairBytes;
-    p->bitmapHoles = im->bitmapHoles;
     p->bucketFold = im->bucketFold;
     p->bitmapBits = im->bitmapBits;
     p->bitmapShift = im->bitmapShift;
@@ -1341,15 +1039,11 @@ hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
     LaunchCfg cfg = pl.cfg;
     const u32 perCta = (u32)cfg.warps;
     cfg.grid = (int)std::min<u32>((u32)cfg.grid, (p.ntiles + perCta - 1) / perCta);
-    if (cfg.split) {
-        CUDA_TRY(cudaMemsetAsync(s->d_counters + CTR_CANDQ, 0, sizeof(u32), stream));
-    }
+    CUDA_TRY(cudaMemsetAsync(s->d_counters + CTR_CANDQ, 0, sizeof(u32), stream));
     CUDA_TRY(launchScan(cfg, p, stream));
     g_launches++;
-    if (cfg.split) {
-        CUDA_TRY(launchConfirm(cfg, p, stream));
-        g_launches++;
-    }
+    CUDA_TRY(launchConfirm(cfg, p, stream));
+    g_launches++;
     return HS_SUCCESS;
 }
 
@@ -1556,17 +1250,9 @@ hs_error_t hs_b200_set_runtime_option(const char *key, int value) {
     }
     struct { const char *n; int *v; } k[] = {
         {"warps", &g_opts.warps},       {"tile_bytes", &g_opts.tileBytes},
-        {"stages", &g_opts.stages},     {"wide_fdr", &g_opts.wideFdr},
-        {"chunk_mb", &g_opts.chunkMB},  {"initial_ring", &g_opts.initialRing},
-        {"stride", &g_opts.stride},     {"prefilter", &g_opts.prefilter},
-        {"rebuild", &g_opts.rebuild},   {"domain", &g_opts.domain},
-        {"direct", &g_opts.direct},     {"replicas", &g_opts.replicas},
-        {"pf_dist", &g_opts.pfDist},    {"queue", &g_opts.queue},
-        {"first_stage", &g_opts.firstStage}, {"wide", &g_opts.wide},
-        {"split", &g_opts.split},       {"big_set", &g_opts.bigSet},
-        {"big_set_classes", &g_opts.bigSetClasses}, {"heavy", &g_opts.heavy},
-        {"gram", &g_opts.gram},                {"fat_pair", &g_opts.fatPair},
-        {"dfa_ilp", &g_opts.dfaIlp}};
+        {"pf_dist", &g_opts.pfDist},    {"chunk_mb", &g_opts.chunkMB},
+        {"initial_ring", &g_opts.initialRing}, {"heavy", &g_opts.heavy},
+        {"gram", &g_opts.gram},         {"dfa_ilp", &g_opts.dfaIlp}};
     for (auto &x : k) {
         if (!strcmp(key, x.n)) {
             *x.v = value;
@@ -2327,7 +2013,7 @@ static hs_error_t scanHostBlocks(const DevImage *im, hs_scratch *s, const char *
         CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
         s->chunkEvents->push_back(ev);
     }
-    /* a second pass after the record ring grew; split mode may need a third (its
+    /* a second pass after the record ring grew; a third may be needed (the
      * candidate list can overflow before the ring does) */
     for (int attempt = 0; attempt < 3; attempt++) {
         CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), s->stream));
@@ -3088,7 +2774,7 @@ static hs_error_t streamsScanImpl(hs_b200_stream_set_t *set, const char *data,
             e = cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), st);
             if (e == cudaSuccess) e = cudaEventRecord(s->evStart, st);
             if (e == cudaSuccess) e = launchScan(cfg, p, st);
-            if (e == cudaSuccess && cfg.split) {
+            if (e == cudaSuccess) {
                 e = launchConfirm(cfg, p, st); /* candidate list -> records (counters were just cleared) */
                 g_launches++;
             }

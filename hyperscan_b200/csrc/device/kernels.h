@@ -25,8 +25,7 @@
 #define HSB_DYNAMIC_SMEM(name) extern __shared__ __align__(128) u8 name[]
 #define HSB_NOINLINE __noinline__
 /* kernel parameters whose address is taken (passed by reference into the out-of-line
- * candidate path) stay in the constant bank instead of being copied to every
- * thread's stack */
+ * drains) stay in the constant bank instead of being copied to every thread's stack */
 #define HSB_GRID_CONSTANT __grid_constant__
 #endif
 
@@ -46,14 +45,11 @@ struct DevMatch {
  * src/fdr/teddy.c:918-969 -- see DESIGN.md section 3 for the derivation). */
 enum FilterKind {
     FK_BYTE32 = 0, /* index = 1 byte; u32 entry (4 slots x 8 buckets); table
-                      replicated per lane (bank-conflict free). Teddy, noodle, and
-                      FDR sets whose tails keep the per-byte filter sparse */
-    FK_BYTE64 = 1, /* index = 1 byte; 2 x u32 (4 slots x 16 buckets). Fat Teddy */
-    FK_HASH32 = 2, /* index = 2-byte FDR hash; u32 entry (slots 0..3 of FDR) */
-    FK_HASH64 = 3, /* index = 2-byte FDR hash; u64 entry (all 8 FDR slots)   */
+                      replicated per lane (bank-conflict free).  8-bucket Teddy, noodle */
     FK_PAIR32 = 4, /* index = (class of byte 0, class of byte 1), 5 bits each, classes
                       from a per-lane byte table; u32 entry; both tables replicated per
-                      lane (bank-conflict free).  FDR sets.  Table image: 256 class words
+                      lane (bank-conflict free).  FDR sets, and fat Teddy with its 16
+                      buckets folded onto 8 bits.  Table image: 256 class words
                       (c0 << 7 | c1 << 12), then 1024 pair entries */
     FK_GRAM4 = 5,  /* index = classes of the FOUR bytes ending at a position (5 bits each) into
                       a 1 Mbit bitmap in shared memory; no buckets.  Large FDR sets whose
@@ -71,13 +67,12 @@ enum ConfirmKind {
 
 enum { MAX_PEERS = 8 };
 enum { CTR_MATCHES = 0, CTR_ERROR = 1, CTR_CANDIDATES = 2, CTR_CONFIRMED = 3,
-       CTR_PREFILTER_PASS = 4, CTR_CANDQ = 5 /* split mode: candidates handed to the confirm kernel */,
+       CTR_PREFILTER_PASS = 4, CTR_CANDQ = 5 /* candidates handed to the confirm kernel */,
        CTR_COUNT = 8 };
 
-/* Split mode (opt-in): the scan kernel stops at the prefilter and appends the
- * surviving candidates to a list in HBM; confirmKernel finishes them, one thread
- * per candidate.  The list is the SECOND half of the record ring the scratch
- * allocated (records [outCap, 2 * outCap) of ScanParams.out), so no launch
+/* Every scan kernel stops at the prefilter and appends the surviving candidates
+ * to a list in HBM; confirmKernel finishes them, one thread per candidate.  The
+ * list is the SECOND half of the record ring the scratch allocated (records [outCap, 2 * outCap) of ScanParams.out), so no launch
  * parameter changes; if it overflows, the record count is raised above outCap
  * and the caller's grow-and-rescan path takes over. */
 struct DevCand {
@@ -92,11 +87,12 @@ struct ScanParams {
      * [-16, paddedBytes + 16) are readable; blocks start 16-byte aligned */
     const u8 *corpus;
     u64 corpusBytes;       /* end of the last block */
-    u64 readableEnd;       /* multiple of 16, >= corpusBytes: TMA may read up to here */
+    u64 readableEnd;       /* multiple of 16, >= corpusBytes: loads may read up to here */
     u32 tileFirst;         /* tiles [tileFirst, tileFirst + ntiles) are scanned */
     u32 ntiles;
     u32 tileBytes;         /* multiple of 512 */
-    u32 nstages;           /* per-warp TMA ring depth */
+    u32 pfDist;            /* L2 prefetch distance: in 512-byte steps (pair, gram kernels),
+                            * in 1 KiB iterations (wide kernel) */
     const u64 *blockOff;   /* ascending, 16-byte aligned */
     const u32 *blockLen;
     u32 nblocks;
@@ -112,16 +108,13 @@ struct ScanParams {
     const u8 *bc;          /* RoseEngine bytecode (device copy) */
     const u8 *table;       /* first-stage table in HBM (copied to smem) */
     u32 tableBytes;
-    u32 indexMask;         /* FK_HASH*: FDR domainMask */
-    u32 repShift;          /* FK_HASH32: log2 of the copies per entry (bank partition) */
-    const u8 *bitmap;      /* second-stage prefilter (copied to smem), may be null */
+    const u8 *bitmap;      /* second-stage prefilter (copied to smem), may be null; FK_PAIR32: the
+                            * (32 KiB) bitmap goes to the class rows' upper halves */
     u32 bitmapBytes;       /* power of two >= 16, or 0 = no prefilter */
     u32 bitmapShift;       /* 32 - log2(bits) */
     u32 keyBytes;          /* 1..4: literal tail bytes hashed into the bitmap */
     u32 pairBytes;         /* FK_PAIR32: shared-memory bytes of the pair table = 4 KiB x classes of the
                             * second byte (<= 128 KiB) */
-    u32 bitmapHoles;       /* FK_PAIR32: 1 = the (32 KiB) bitmap sits in the class rows' upper halves;
-                            * 0 = bitmapBytes contiguous bytes after the pair table (large sets) */
     u32 bitmapBits;        /* FK_PAIR32: bits of the first-level bitmap; index = mulhi(key * K, bits) */
     u32 bucketFold;        /* 1 = 16 confirm buckets (fat Teddy) behind 8 first-stage bits: bit i of a
                             * candidate stands for buckets i and i + 8 */
@@ -146,27 +139,24 @@ struct ScanParams {
 };
 
 struct LaunchCfg {
-    int kind;      /* FilterKind */
-    int stride;    /* 1, 2, 4 */
-    int slotBase;  /* FK_HASH32: 0 = slots 0..3 (reference numbering), 1 = slots 1..4 */
-    int direct;    /* 1: corpus loaded straight into registers; 0: TMA-staged tiles */
-    int queued;    /* 1 (direct, stride 1 only): candidates go through the per-warp queue */
-    int wide;      /* 1 (direct, stride 1, FK_BYTE32 / FK_HASH32, tileBytes % 1024 == 0): 32-byte lanes */
-    int split;     /* 1 (wide only): candidates go to the list in HBM, confirmKernel finishes them */
+    int kind;      /* FilterKind: FK_BYTE32 = wide kernel, FK_PAIR32 = pair kernel, FK_GRAM4 = gram kernel */
+    int slotBase;  /* FK_PAIR32: 0 = slots 0..3 (reference numbering), 1 = slots 1..4 */
+    int heavy;     /* FK_PAIR32: 1 = one queue entry per word with candidates (saturating sets) */
     int grid;      /* CTAs (one per SM) */
-    int warps;     /* per CTA */
+    int warps;     /* per CTA: up to 32 (wide kernel) or 28 (pair, gram) */
     size_t smemBytes;
 };
 
-/* Dynamic shared memory the kernel needs (warps = warps with TMA stages, 0 in
- * direct mode; queueWarps = warps with a candidate queue, 0 without, negative =
- * that many warps of the wide-step variant). */
-size_t scanSmemBytes(int kind, u32 tableBytes, u32 bitmapBytes, int warps, u32 nstages,
-                     u32 tileBytes, int queueWarps);
+/* Dynamic shared memory the scan kernel of `kind` needs with queueWarps warps
+ * (tableBytes: FK_PAIR32 = the pair table's shared-memory bytes; bitmapBytes:
+ * FK_BYTE32 = the prefilter bitmap). */
+size_t scanSmemBytes(int kind, u32 tableBytes, u32 bitmapBytes, int queueWarps);
 
+/* Scan tiles [p.tileFirst, p.tileFirst + p.ntiles) up to the candidate list;
+ * launchConfirm must follow on the same stream. */
 cudaError_t launchScan(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream);
 
-/* Split mode: finish the candidates the scan kernel left in the list (same stream, after it). */
+/* Finish the candidates the scan kernel left in the list (same stream, after it). */
 cudaError_t launchConfirm(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream);
 
 /* Publish the record count of a finished scan into slot 0 of this rank's

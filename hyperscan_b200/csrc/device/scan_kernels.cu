@@ -10,27 +10,31 @@
  * (src/rose/match.c:479-527, src/rose/program_runtime.c:3101-3522).
  *
  * Execution model (DESIGN.md section 3):
- *   - persistent grid, one CTA per SM; the first-stage table is pinned in
+ *   - persistent grid, one CTA per SM; the first-stage tables are pinned in
  *     shared memory once per CTA;
  *   - the packed corpus is cut into fixed-size tiles regardless of block
  *     boundaries (the first stage is position-only; block membership is
  *     checked in the confirm stage); every warp owns a CONTIGUOUS run of
  *     tiles so the shift-OR state carries across tiles;
- *   - corpus staging, two modes (template DIRECT): each lane loads its 16
- *     bytes per step straight from HBM into registers one step ahead, with
- *     prefetch.global.L2 several steps ahead (default); or tiles are staged
- *     global -> shared with 1-D TMA bulk copies (cp.async.bulk + mbarrier
- *     complete_tx), an NSTAGE-deep ring per warp, and read as uint4;
- *   - per 512-byte step every lane does 16/STRIDE table lookups and merges
- *     the four entries of one in-word position as a 128-bit stream with one
- *     funnel shift per output word; the 3 (or 7) bytes that overflow into the
- *     next lane travel by __shfl_up_sync; a zero bit = candidate (bucket, end);
- *   - candidates (rare) first probe a bitmap over hashes of literal tails in
- *     shared memory (+ a sparser second level in L2 for large sets); survivors
- *     are confirmed in place: FDRConfirm hash -> LitInfo chain -> block lookup
- *     -> rose literal program -> 16-byte match record appended to a ring in
- *     HBM and, in multi-GPU runs, stored into every rank's exchange buffer over
- *     NVLink peer mappings (the scan IS the all-gather).
+ *   - every lane loads its bytes straight from HBM into registers, a step or
+ *     two ahead, with prefetch.global.L2 pfDist steps ahead;
+ *   - three first stages, chosen by the host from the database:
+ *       scanKernelWide (FK_BYTE32: noodle, 8-bucket Teddy): 32 bytes per lane
+ *         and 1 KiB per warp iteration, one per-lane-replicated byte table;
+ *       scanKernelPair (FK_PAIR32: FDR sets, fat Teddy with its buckets
+ *         folded): two conflict-free class lookups and one pair lookup per byte;
+ *       scanKernelGram (FK_GRAM4: large FDR sets): class 4-gram membership in
+ *         a 1 Mbit shared-memory bitmap;
+ *     a zero bit of the shift-OR state = candidate (bucket, end);
+ *   - candidates (rare) go through a per-warp queue in shared memory, probe a
+ *     bitmap over hashes of literal tails (shared memory, + a sparser second
+ *     level in L2 for large sets), and the survivors are appended to a
+ *     candidate list in HBM;
+ *   - confirmKernel, launched after every scan, finishes the list: FDRConfirm
+ *     hash -> LitInfo chain -> block lookup -> rose literal program -> 16-byte
+ *     match record appended to a ring in HBM and, in multi-GPU runs, stored
+ *     into every rank's exchange buffer over NVLink peer mappings (the scan IS
+ *     the all-gather).
  */
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -41,64 +45,18 @@ namespace hsb {
 
 namespace {
 
-/* ---- PTX wrappers: mbarrier + 1-D TMA bulk copy, shared-memory access, streaming
- * loads.  The HSB_HOST_EMU forms belong to the SIMT emulator of tests/emu (test
- * infrastructure): shared-memory "addresses" are offsets into the block's window
- * and a bulk copy completes at once. */
+/* ---- PTX wrappers: shared-memory addresses, streaming loads.  The HSB_HOST_EMU
+ * forms belong to the SIMT emulator of tests/emu (test infrastructure):
+ * shared-memory "addresses" are offsets into the block's window. */
 #ifdef HSB_HOST_EMU
 __device__ __forceinline__ u32 smemAddr(const void *p) {
     return (u32)((const u8 *)p - hsb_emu::dynamicSmem());
 }
-/* the barrier word counts completed phases; try_wait.parity(P) succeeds once the
- * barrier's current phase differs from P */
-__device__ __forceinline__ void mbarInit(u64 *bar, u32) { *bar = 0; }
-__device__ __forceinline__ void mbarExpectTx(u64 *, u32) {}
-__device__ __forceinline__ void tmaLoad1d(void *dst, const void *src, u32 bytes, u64 *bar) {
-    memcpy(dst, src, bytes);
-    (*bar)++;
-    hsb_emu::noteProgress();
-}
-__device__ __forceinline__ void mbarWait(u64 *bar, u32 parity) {
-    while (((u32)*(volatile u64 *)bar & 1) == parity) {
-        hsb_emu::yieldThread();
-    }
-}
-__device__ __forceinline__ void fenceMbarInit() {}
 __device__ __forceinline__ uint4 ldCs128(const u8 *p) { return *reinterpret_cast<const uint4 *>(p); }
 __device__ __forceinline__ void prefetchL2(const void *) {}
 #else
 __device__ __forceinline__ u32 smemAddr(const void *p) {
     return (u32)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbarInit(u64 *bar, u32 count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smemAddr(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbarExpectTx(u64 *bar, u32 bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smemAddr(bar)),
-                 "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void tmaLoad1d(void *dst, const void *src, u32 bytes, u64 *bar) {
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::
-            "r"(smemAddr(dst)),
-        "l"(src), "r"(bytes), "r"(smemAddr(bar))
-        : "memory");
-}
-__device__ __forceinline__ void mbarWait(u64 *bar, u32 parity) {
-    u32 done;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(smemAddr(bar)), "r"(parity)
-            : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void fenceMbarInit() {
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 /* volatile: keeps the load where it is written (ptxas otherwise sinks it next to
  * its first use and the prefetch is lost) */
@@ -508,12 +466,6 @@ __device__ void confirmNoodle(const ScanParams &p, u64 g, u64 confVal, u32 *ncon
 
 /* ---- first stage ----------------------------------------------------------- */
 
-template <int KIND> struct Kind {
-    static constexpr int NOCT = KIND == FK_BYTE64 ? 2 : 1;  /* bucket octets */
-    static constexpr int SPILL = KIND == FK_HASH64 ? 2 : 1; /* words overflowing into the next lane */
-    static constexpr bool HASH = KIND == FK_HASH32 || KIND == FK_HASH64;
-};
-
 #ifdef HSB_HOST_EMU
 __device__ __forceinline__ u32 lds32(u32 addr) {
     u32 v;
@@ -587,92 +539,31 @@ template <int O> __device__ __forceinline__ void orStream(u32 (&a)[6], const u32
     }
 }
 
-/* Shift-OR contributions of one lane's 16 positions.  a[o][0..3]: bytes for
- * the lane's own 16 end positions (bit set = bucket impossible); a[o][4..]:
- * overflow that belongs to the NEXT lane's first positions.  An entry read at
- * position x applies to end positions x+SB .. x+SB+3 (SB = slot base: 0 for
- * tables in the reference's own slot numbering, 1 for tables rebuilt over
- * slots 1..4).  Only positions = 0 mod STRIDE are sampled; skipped positions
- * contribute nothing, i.e. "possible" (src/fdr/fdr.c:247-327). */
-template <int KIND, int STRIDE, int SB>
-__device__ __forceinline__ void laneFilter(const u32 (&w)[5], u32 tabAddr, u32 laneOff,
-                                           u32 indexMask, u32 repShift, u32 (&a)[2][6]) {
+/* Shift-OR contributions of one lane's 16 positions through the FK_BYTE32 table.
+ * a[0..3]: bytes for the lane's own 16 end positions (bit set = bucket
+ * impossible); a[4]: overflow that belongs to the NEXT lane's first positions.
+ * An entry read at position x applies to end positions x .. x+3. */
+__device__ __forceinline__ void laneFilter(const u32 (&w)[5], u32 tabAddr, u32 laneOff, u32 (&a)[6]) {
 #pragma unroll
-    for (int o = 0; o < 2; o++) {
-#pragma unroll
-        for (int i = 0; i < 6; i++) {
-            a[o][i] = 0;
-        }
+    for (int i = 0; i < 6; i++) {
+        a[i] = 0;
     }
-    if (KIND == FK_HASH64) {
+    /* gather the entries of in-word position r for all four words, then merge
+     * the stream with funnel shifts */
 #pragma unroll
-        for (int j = 0; j < 16; j += STRIDE) {
-            const int k = j >> 2, r = j & 3;
-            u32 off;
-            if (r == 0) {
-                off = w[k] << 3;
-            } else if (r == 3) {
-                off = __funnelshift_r(w[k], w[k + 1], 21);
-            } else {
-                off = w[k] >> (8 * r - 3);
-            }
-            const uint2 e = lds64(tabAddr + (off & (indexMask << 3)));
-            if (r == 0) {
-                a[0][k] |= e.x;
-                a[0][k + 1] |= e.y;
-            } else {
-                a[0][k] |= e.x << (8 * r);
-                a[0][k + 1] |= __funnelshift_l(e.x, e.y, 8 * r);
-                a[0][k + 2] |= e.y >> (32 - 8 * r);
-            }
-        }
-        return;
-    }
-    /* 32-bit entries: gather the entries of in-word position r for all four
-     * words, then merge the stream with funnel shifts */
-    constexpr int RSTEP = KIND == FK_HASH64 ? 4 : STRIDE; /* (FK_HASH64 returned above) */
-#pragma unroll
-    for (int r = 0; r < 4; r += RSTEP) {
-        u32 E0[4], E1[4];
+    for (int r = 0; r < 4; r++) {
+        u32 E[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) {
-            if (KIND == FK_HASH32) {
-                /* entry (h & indexMask) has 2^repShift copies in adjacent words;
-                 * tabAddr already points at this lane's copy (bank partition) */
-                const u32 sh = 2 + repShift;
-                u32 off;
-                if (r == 0) {
-                    off = w[k] << sh;
-                } else if (r == 3) {
-                    off = __funnelshift_r(w[k], w[k + 1], 24 - sh);
-                } else {
-                    off = w[k] >> (8 * r - sh);
-                }
-                E0[k] = lds32(tabAddr + (off & (indexMask << sh)));
-            } else {
-                /* row b of the table is 256 bytes: lane l's copy of the entry at
-                 * l * 4 (second bucket octet at 128 + l * 4), so the row offset
-                 * b << 8 | l << 2 is ONE byte permute of (word, laneOff) and every
-                 * lookup is bank-conflict free */
-                const u32 row = __byte_perm(w[k], laneOff, 0x5504 + (r << 4));
-                E0[k] = lds32(tabAddr + row);
-                if (KIND == FK_BYTE64) {
-                    E1[k] = lds32(tabAddr + row + 128);
-                }
-            }
+            /* row b of the table is 256 bytes: lane l's copy of the entry at
+             * l * 4, so the row offset b << 8 | l << 2 is ONE byte permute of
+             * (word, laneOff) and every lookup is bank-conflict free */
+            E[k] = lds32(tabAddr + __byte_perm(w[k], laneOff, 0x5504 + (r << 4)));
         }
-        if (r + SB == 0) orStream<0>(a[0], E0);
-        if (r + SB == 1) orStream<1>(a[0], E0);
-        if (r + SB == 2) orStream<2>(a[0], E0);
-        if (r + SB == 3) orStream<3>(a[0], E0);
-        if (r + SB == 4) orStream<4>(a[0], E0);
-        if (KIND == FK_BYTE64) {
-            if (r + SB == 0) orStream<0>(a[1], E1);
-            if (r + SB == 1) orStream<1>(a[1], E1);
-            if (r + SB == 2) orStream<2>(a[1], E1);
-            if (r + SB == 3) orStream<3>(a[1], E1);
-            if (r + SB == 4) orStream<4>(a[1], E1);
-        }
+        if (r == 0) orStream<0>(a, E);
+        if (r == 1) orStream<1>(a, E);
+        if (r == 2) orStream<2>(a, E);
+        if (r == 3) orStream<3>(a, E);
     }
 }
 
@@ -702,29 +593,17 @@ __device__ __forceinline__ u64 confValAt(const ScanParams &p, u64 g) {
     return ((u64)hi << 32) | lo;
 }
 
-/* All candidates of one lane: c[o][k] has a set bit per (bucket, byte).  `pw` is
- * the word before the lane's 16 bytes.  Per candidate byte: hash the last
- * keyBytes bytes into the prefilter bitmap (shared memory); only survivors pay
- * for the hash confirm in HBM/L2. */
-/* First-level prefilter bitmap word holding bit `hsh`.  HOLES (class-pair kernel):
- * the 32 KB bitmap lives in the unused upper halves of the 256-byte class rows,
- * word i at row i >> 5, byte 128 + 4 * (i & 31). */
-template <int HOLES> __device__ __forceinline__ u32 bitmapWord(u32 bitmapAddr, u32 hsh) {
-    if (HOLES) {
-        return lds32(bitmapAddr + ((hsh >> 10) << 8) + ((hsh >> 3) & 0x7cu));
-    }
-    return lds32(bitmapAddr + ((hsh >> 5) << 2));
-}
-
-template <int NOCT, int SPLIT, int HOLES = 0>
-__device__ __forceinline__ void laneCandidatesBody(const ScanParams &p, u32 bitmapAddr, u32 c00, u32 c01,
-                                                   u32 c02, u32 c03, u32 c10, u32 c11, u32 c12, u32 c13,
-                                                   u32 w0, u32 w1, u32 w2, u32 w3, u32 pw, u64 g0,
-                                                   u32 *stats) {
+/* Candidates of one lane's 16 bytes: c[k] has a set bit per (bucket, byte) of word
+ * k, w[k] is the word itself and `pw` the word before it.  Per candidate byte: hash
+ * the last keyBytes bytes into the prefilter bitmap (shared memory); survivors are
+ * appended to the candidate list (second half of the record ring) for confirmKernel. */
+__device__ __forceinline__ void laneCandidates(const ScanParams &p, u32 bitmapAddr, u32 c0, u32 c1, u32 c2,
+                                               u32 c3, u32 w0, u32 w1, u32 w2, u32 w3, u32 pw, u64 g0,
+                                               u32 *stats) {
     /* 16-bit map of bytes that carry a candidate */
     u32 cm = 0;
     {
-        const u32 n[4] = {c00 | c10, c01 | c11, c02 | c12, c03 | c13};
+        const u32 n[4] = {c0, c1, c2, c3};
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             u32 t = n[k] | (n[k] >> 4);
@@ -740,19 +619,15 @@ __device__ __forceinline__ void laneCandidatesBody(const ScanParams &p, u32 bitm
         const u32 k = x >> 2, q = x & 3;
         const u32 cur = k == 0 ? w0 : k == 1 ? w1 : k == 2 ? w2 : w3;
         const u32 prv = k == 0 ? pw : k == 1 ? w0 : k == 2 ? w1 : w2;
-        const u32 b0 = k == 0 ? c00 : k == 1 ? c01 : k == 2 ? c02 : c03;
-        u32 buckets = (b0 >> (8 * q)) & 0xff;
-        if (NOCT == 2) {
-            const u32 b1 = k == 0 ? c10 : k == 1 ? c11 : k == 2 ? c12 : c13;
-            buckets |= ((b1 >> (8 * q)) & 0xff) << 8;
-        }
+        const u32 b0 = k == 0 ? c0 : k == 1 ? c1 : k == 2 ? c2 : c3;
+        const u32 buckets = (b0 >> (8 * q)) & 0xff;
         stats[0]++;
         if (p.bitmapBytes) {
             /* the 4 bytes ending at x, then the last keyBytes of them */
             const u32 last4 = q == 3 ? cur : __funnelshift_r(prv, cur, 8 * (q + 1));
             const u32 key = last4 >> (8 * (4 - p.keyBytes));
             const u32 hsh = (key * 0x9E3779B1u) >> p.bitmapShift;
-            if (!((bitmapWord<HOLES>(bitmapAddr, hsh) >> (hsh & 31)) & 1)) {
+            if (!((lds32(bitmapAddr + ((hsh >> 5) << 2)) >> (hsh & 31)) & 1)) {
                 continue; /* no literal of any bucket ends here */
             }
             if (p.bitmap2Shift) {
@@ -765,461 +640,36 @@ __device__ __forceinline__ void laneCandidatesBody(const ScanParams &p, u32 bitm
             }
         }
         stats[1]++;
-        const u64 g = g0 + x;
-        if (SPLIT) {
-            /* hand the candidate to confirmKernel (list = second half of the ring) */
-            const u32 i = atomicAdd(p.counters + CTR_CANDQ, 1u);
-            if (i < p.outCap) {
-                DevCand cnd;
-                cnd.g = g;
-                cnd.buckets = buckets;
-                cnd.pad = 0;
-                *reinterpret_cast<uint4 *>(reinterpret_cast<DevCand *>(p.out + p.outCap) + i) =
-                    *reinterpret_cast<const uint4 *>(&cnd);
-            }
-            continue;
-        }
-        const u64 confVal = confValAt(p, g);
-        if (p.confirmKind == CK_NOODLE) {
-            if (buckets & 1) {
-                confirmNoodle(p, g, confVal, &stats[2]);
-            }
-        } else {
-            while (buckets) {
-                const u32 bucket = __ffs(buckets) - 1;
-                buckets &= buckets - 1;
-                confirmFdr(p, bucket, g, confVal, &stats[2]);
-            }
-        }
-    }
-}
-
-/* Out of line in the fused kernels (it carries the confirm and the literal
- * programs); the split kernels inline the body, which then ends at the append
- * to the candidate list, so nothing in them takes the parameters' address (no
- * per-thread copy of ScanParams on the stack). */
-template <int NOCT>
-__device__ HSB_NOINLINE void laneCandidates(const ScanParams &p, u32 bitmapAddr, u32 c00, u32 c01,
-                                            u32 c02, u32 c03, u32 c10, u32 c11, u32 c12, u32 c13,
-                                            u32 w0, u32 w1, u32 w2, u32 w3, u32 pw, u64 g0,
-                                            u32 *stats) {
-    laneCandidatesBody<NOCT, 0>(p, bitmapAddr, c00, c01, c02, c03, c10, c11, c12, c13, w0, w1, w2, w3, pw, g0,
-                                stats);
-}
-
-/* Candidate queue (template QUEUED): instead of every lane walking its own
- * candidates while the other 31 idle, lanes append {candidate words, chunk
- * number} to a per-warp queue in shared memory and the warp drains it 32
- * entries at a time, one entry per lane, all lanes in step through the
- * prefilter probe.  An entry is NOCT x 16 bytes of candidate bits + the number
- * of the 16-byte chunk relative to the warp's run; the chunk's bytes are read
- * back from L2. */
-template <int NOCT> struct QueueEntry {
-    static constexpr u32 BYTES = NOCT == 1 ? 32 : 48;
-    static constexpr u32 SLOTS = 64;                     /* < 32 pending + <= 32 appended per step */
-    static constexpr u32 RUN_START = BYTES * SLOTS;      /* u64: corpus position of the run's chunk 0 */
-    static constexpr u32 WARP_BYTES = RUN_START + 16;    /* one warp's share of shared memory */
-};
-
-template <int NOCT>
-__device__ HSB_NOINLINE void drainQueue(const ScanParams &p, u32 bitmapAddr, u32 qAddr, u32 first,
-                                        u32 count, u32 lane, u32 *stats) {
-    if (lane >= count) {
-        return;
-    }
-    const uint2 rs = lds64(qAddr + QueueEntry<NOCT>::RUN_START);
-    const u64 runStart = ((u64)rs.y << 32) | rs.x;
-    const u32 e = qAddr + (first + lane) * QueueEntry<NOCT>::BYTES;
-    const uint4 c0 = lds128(e);
-    uint4 c1 = make_uint4(0, 0, 0, 0);
-    if (NOCT == 2) {
-        c1 = lds128(e + 16);
-    }
-    const u64 g0 = runStart + (u64)lds32(e + 16 * NOCT) * 16;
-    uint4 v = make_uint4(0, 0, 0, 0);
-    if (g0 + 16 <= p.readableEnd) {
-        v = __ldg(reinterpret_cast<const uint4 *>(p.corpus + g0));
-    }
-    const u32 pw = g0 ? __ldg(reinterpret_cast<const u32 *>(p.corpus + g0 - 4)) : 0u;
-    laneCandidates<NOCT>(p, bitmapAddr, c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w, v.x, v.y, v.z,
-                         v.w, pw, g0, stats);
-}
-
-/* per-warp queue state carried through the run */
-struct WarpQueue {
-    u32 addr; /* shared-memory address of this warp's slots */
-    u32 n;    /* entries pending (warp-uniform) */
-};
-
-/* ---- the scan kernel -------------------------------------------------------- */
-
-__host__ __device__ inline u32 tableSmemBytes(int kind, u32 tableBytes) {
-    if (kind == FK_BYTE32 || kind == FK_BYTE64) {
-        return 256 * 256; /* 256 rows: 32 lane copies x (1 or 2) bucket octets */
-    }
-    return (tableBytes + 127u) & ~127u;
-}
-
-/* One 512-byte step of a warp: v = the lane's own 16 bytes, w4 = the word after
- * them, pwSrc = loader of the word before the warp's 512 bytes (lane 0 only,
- * rare path). */
-template <int KIND, int STRIDE, int SB, int QUEUED, class PrevWord>
-__device__ __forceinline__ void scanStep(const ScanParams &p, const uint4 v, u32 w4, u32 lane,
-                                         u32 tabAddr, u32 laneOff, u32 bitmapAddr,
-                                         u32 (&carry)[2][2], u64 g0, u32 *stats, PrevWord prevWord,
-                                         WarpQueue &wq, u32 chunk) {
-    typedef Kind<KIND> K;
-    const u32 w[5] = {v.x, v.y, v.z, v.w, w4};
-    u32 a[2][6];
-    laneFilter<KIND, STRIDE, SB>(w, tabAddr, laneOff, p.indexMask, p.repShift, a);
-    u32 c[2][4];
-    u32 any = 0;
-#pragma unroll
-    for (int o = 0; o < K::NOCT; o++) {
-#pragma unroll
-        for (int x = 0; x < K::SPILL; x++) {
-            /* ONE rotate-by-one shuffle: lanes 1..31 receive their left
-             * neighbour's overflow; lane 0 receives lane 31's, which is exactly
-             * the carry into the next step (shuffles ride the shared-memory
-             * data pipe, the limiter of this kernel) */
-            u32 in = __shfl_sync(0xffffffffu, a[o][4 + x], (lane + 31) & 31);
-            if (lane == 0) {
-                const u32 next = in;
-                in = carry[o][x];
-                carry[o][x] = next;
-            }
-            a[o][x] |= in;
-        }
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            c[o][k] = ~a[o][k];
-            any |= c[o][k];
-        }
-    }
-    if (K::NOCT == 1) {
-        c[1][0] = c[1][1] = c[1][2] = c[1][3] = 0;
-    }
-    if (QUEUED) {
-        const u32 bal = __ballot_sync(0xffffffffu, any != 0);
-        if (bal) {
-            typedef QueueEntry<K::NOCT> Q;
-            if (any) {
-                const u32 e = wq.addr + (wq.n + __popc(bal & ((1u << lane) - 1))) * Q::BYTES;
-                sts128(e, c[0][0], c[0][1], c[0][2], c[0][3]);
-                if (K::NOCT == 2) {
-                    sts128(e + 16, c[1][0], c[1][1], c[1][2], c[1][3]);
-                }
-                sts32(e + 16 * K::NOCT, chunk);
-            }
-            wq.n += __popc(bal);
-            if (wq.n >= 32) {
-                __syncwarp();
-                wq.n -= 32;
-                drainQueue<K::NOCT>(p, bitmapAddr, wq.addr, wq.n, 32, lane, stats);
-                __syncwarp();
-            }
-        }
-    } else if (__any_sync(0xffffffffu, any != 0)) {
-        u32 pw = __shfl_up_sync(0xffffffffu, v.w, 1);
-        if (lane == 0) {
-            pw = prevWord();
-        }
-        if (any) {
-            laneCandidates<K::NOCT>(p, bitmapAddr, c[0][0], c[0][1], c[0][2], c[0][3], c[1][0], c[1][1],
-                                    c[1][2], c[1][3], v.x, v.y, v.z, v.w, pw, g0, stats);
+        const u32 i = atomicAdd(p.counters + CTR_CANDQ, 1u);
+        if (i < p.outCap) {
+            DevCand cnd;
+            cnd.g = g0 + x;
+            cnd.buckets = buckets;
+            cnd.pad = 0;
+            *reinterpret_cast<uint4 *>(reinterpret_cast<DevCand *>(p.out + p.outCap) + i) =
+                *reinterpret_cast<const uint4 *>(&cnd);
         }
     }
 }
 
 /* State entering a run of tiles: every lane evaluates the 16 bytes before the
- * run as if it were "lane -1" and keeps only the overflow. */
-template <int KIND, int STRIDE, int SB>
-__device__ __forceinline__ void haloStep(const ScanParams &p, const uint4 v, u32 w4, u32 tabAddr,
-                                         u32 laneOff, u32 (&carry)[2][2]) {
-    typedef Kind<KIND> K;
+ * run (v, then w4 = the run's first word) as if it were "lane -1" and keeps only
+ * the overflow. */
+__device__ __forceinline__ u32 haloStep(const uint4 v, u32 w4, u32 tabAddr, u32 laneOff) {
     const u32 w[5] = {v.x, v.y, v.z, v.w, w4};
-    u32 a[2][6];
-    laneFilter<KIND, STRIDE, SB>(w, tabAddr, laneOff, p.indexMask, p.repShift, a);
-#pragma unroll
-    for (int o = 0; o < K::NOCT; o++) {
-#pragma unroll
-        for (int x = 0; x < K::SPILL; x++) {
-            carry[o][x] = a[o][4 + x];
-        }
-    }
+    u32 a[6];
+    laneFilter(w, tabAddr, laneOff, a);
+    return a[4];
 }
 
-template <int KIND, int STRIDE, int SB, int DIRECT, int QUEUED>
-__global__ void __launch_bounds__(DIRECT ? 896 : 1024, 1) scanKernel(const HSB_GRID_CONSTANT ScanParams p) {
-    static_assert(!QUEUED || DIRECT, "the candidate queue reads chunks back from the corpus (direct mode)");
-    HSB_DYNAMIC_SMEM(smem);
-    typedef Kind<KIND> K;
-    const u32 lane = threadIdx.x & 31;
-    const u32 warp = threadIdx.x >> 5;
-    const u32 nwarps = blockDim.x >> 5;
-    const u32 stageBytes = p.tileBytes + 32;
-    const u32 tab0 = tableSmemBytes(KIND, p.tableBytes);
-    const u32 tabBytes = tab0 + p.bitmapBytes;
-
-    /* pin the first-stage table in shared memory */
-    if (KIND == FK_BYTE32 || KIND == FK_BYTE64) {
-        /* word i of the table image: row i >> 6, octet (i >> 5) & 1, lane i & 31 */
-        const u32 *g = reinterpret_cast<const u32 *>(p.table);
-        u32 *s = reinterpret_cast<u32 *>(smem);
-        for (u32 i = threadIdx.x; i < 256 * 64; i += blockDim.x) {
-            const u32 b = i >> 6, o = (i >> 5) & 1;
-            s[i] = KIND == FK_BYTE64 ? __ldg(g + b * 2 + o) : (o ? 0xffffffffu : __ldg(g + b));
-        }
-    } else {
-        const uint4 *g = reinterpret_cast<const uint4 *>(p.table);
-        uint4 *s = reinterpret_cast<uint4 *>(smem);
-        for (u32 i = threadIdx.x; i < p.tableBytes / 16; i += blockDim.x) {
-            s[i] = __ldg(g + i);
-        }
-    }
-    /* second-stage prefilter: one bit per hash of a literal's last bytes */
-    if (p.bitmapBytes) {
-        const uint4 *g = reinterpret_cast<const uint4 *>(p.bitmap);
-        uint4 *sdst = reinterpret_cast<uint4 *>(smem + tab0);
-        for (u32 i = threadIdx.x; i < p.bitmapBytes / 16; i += blockDim.x) {
-            sdst[i] = __ldg(g + i);
-        }
-    }
-    u8 *stages = smem + tabBytes + (size_t)warp * p.nstages * stageBytes;
-    u64 *bars = reinterpret_cast<u64 *>(smem + tabBytes + (size_t)nwarps * p.nstages * stageBytes) +
-                warp * p.nstages;
-    if (!DIRECT && lane == 0) {
-        for (u32 s = 0; s < p.nstages; s++) {
-            mbarInit(&bars[s], 1);
-        }
-    }
-    if (!DIRECT) {
-        fenceMbarInit();
-    }
-    __syncthreads();
-
-    const u32 bitmapAddr = smemAddr(smem) + tab0;
-    /* FK_HASH32: each lane reads its own copy of the table (lane & (R-1)) */
-    const u32 tabAddr = smemAddr(smem) + (KIND == FK_HASH32 ? (lane & ((1u << p.repShift) - 1)) * 4 : 0);
-    const u32 laneOff = lane * 4;
-
-    /* this warp's contiguous run of tiles */
-    const u32 gwarp = blockIdx.x * nwarps + warp;
-    const u32 totalWarps = gridDim.x * nwarps;
-    const u32 q = p.ntiles / totalWarps, rem = p.ntiles % totalWarps;
-    const u32 myCount = q + (gwarp < rem ? 1u : 0u);
-    const u32 myFirst = p.tileFirst + gwarp * q + min(gwarp, rem);
-    if (myCount == 0) {
-        return;
-    }
-
-    u32 carry[2][2] = {{0, 0}, {0, 0}}; /* lane 31's overflow of the previous step */
-    u32 stats[3] = {0, 0, 0};           /* candidates, prefilter passes, confirmed */
-    WarpQueue wq;
-    wq.addr = smemAddr(smem) + tabBytes + warp * QueueEntry<K::NOCT>::WARP_BYTES;
-    wq.n = 0;
-
-    if (DIRECT && QUEUED) {
-        /* corpus bytes straight from HBM into registers: one coalesced
-         * 16-byte load per lane and step, three steps in flight per warp */
-        const u64 runStart = (u64)myFirst * p.tileBytes;
-        u64 runEnd = runStart + (u64)myCount * p.tileBytes;
-        if (runEnd > p.corpusBytes) {
-            runEnd = p.corpusBytes;
-        }
-        const u32 nsteps = (u32)((runEnd - runStart + 511) >> 9);
-        const u8 *ptr = p.corpus + runStart + lane * 16; /* this lane's 16 bytes of the current step */
-        const u8 *const endPtr = p.corpus + p.readableEnd;
-        if (QUEUED && lane == 0) {
-            sts64(wq.addr + QueueEntry<K::NOCT>::RUN_START, (u32)runStart, (u32)(runStart >> 32));
-        }
-        auto load = [&](const u8 *q, bool guard) -> uint4 {
-            uint4 r = make_uint4(0, 0, 0, 0);
-            if (!guard || q + 16 <= endPtr) {
-                r = ldCs128(q);
-            }
-            return r;
-        };
-        /* two-level prefetch: every fourth step the even lanes pull the 2 KiB
-         * that lie `pfDist` steps ahead into L2 (16 x 128 B), the register copy
-         * runs one step ahead and so only has to cover an L2 hit */
-        const size_t pfBytes = (size_t)p.nstages * 512 + lane * 48; /* + (lane / 2) * 128 - lane * 16 */
-        uint4 nxt = load(ptr, true);
-        if (runStart != 0) {
-            const uint4 hv = __ldg(reinterpret_cast<const uint4 *>(p.corpus + runStart - 16));
-            const u32 first = __shfl_sync(0xffffffffu, nxt.x, 0);
-            haloStep<KIND, STRIDE, SB>(p, hv, first, tabAddr, laneOff, carry);
-        }
-        u32 step = 0;
-        auto body = [&](const bool guard) {
-            const uint4 cur = nxt;
-            nxt = load(ptr + 512, guard);
-            if ((step & 3) == 0 && (lane & 1) == 0) {
-                const u8 *pf = ptr + pfBytes;
-                if (pf < endPtr) {
-                    prefetchL2(pf);
-                }
-            }
-            u32 w4 = 0;
-            if (K::HASH) {
-                /* the word after the lane's 16 bytes: one rotate shuffle in
-                 * which lane 0 offers the NEXT step's first word (for lane 31) */
-                w4 = __shfl_sync(0xffffffffu, lane == 0 ? nxt.x : cur.x, (lane + 1) & 31);
-            }
-            const u64 g0 = (u64)(ptr - p.corpus);
-            scanStep<KIND, STRIDE, SB, QUEUED>(
-                p, cur, w4, lane, tabAddr, laneOff, bitmapAddr, carry, g0, stats,
-                [&]() { return g0 ? __ldg(reinterpret_cast<const u32 *>(ptr - 4)) : 0u; }, wq,
-                step * 32 + lane);
-        };
-        /* the load issued in iteration `step` fetches step + 1: it needs no
-         * bounds check while the whole warp's 512 bytes of that step are
-         * readable -- everywhere except at the very end of the corpus */
-        const u64 readableSteps = (p.readableEnd - runStart) >> 9;
-        const u32 nFast = readableSteps >= (u64)nsteps + 1 ? nsteps : (readableSteps ? (u32)readableSteps - 1 : 0);
-#pragma unroll 1
-        for (; step < nFast; step++, ptr += 512) {
-            body(false);
-        }
-#pragma unroll 1
-        for (; step < nsteps; step++, ptr += 512) {
-            body(true);
-        }
-        if (QUEUED && wq.n) {
-            __syncwarp();
-            drainQueue<K::NOCT>(p, bitmapAddr, wq.addr, 0, wq.n, lane, stats);
-        }
-    } else if (DIRECT) {
-        /* corpus bytes straight from HBM into registers: one coalesced
-         * 16-byte load per lane and step, three steps in flight per warp */
-        const u64 runStart = (u64)myFirst * p.tileBytes;
-        u64 runEnd = runStart + (u64)myCount * p.tileBytes;
-        if (runEnd > p.corpusBytes) {
-            runEnd = p.corpusBytes;
-        }
-        const u32 nsteps = (u32)((runEnd - runStart + 511) >> 9);
-        const u8 *base = p.corpus + runStart + lane * 16;
-        const u64 lanePos = runStart + lane * 16;
-        auto load = [&](u32 step) -> uint4 {
-            const u64 pos = lanePos + (u64)step * 512;
-            uint4 r = make_uint4(0, 0, 0, 0);
-            if (pos + 16 <= p.readableEnd) {
-                r = ldCs128(base + (size_t)step * 512);
-            }
-            return r;
-        };
-        /* two-level prefetch: lines are pulled into L2 `pfDist` steps ahead
-         * (4 lanes x 128 B per step), the register copy runs one step ahead and
-         * so only has to cover an L2 hit */
-        const u32 pfDist = p.nstages; /* direct mode: L2 prefetch distance in steps */
-        uint4 nxt = load(0);
-        if (runStart != 0) {
-            const uint4 hv = __ldg(reinterpret_cast<const uint4 *>(p.corpus + runStart - 16));
-            const u32 first = __shfl_sync(0xffffffffu, nxt.x, 0);
-            haloStep<KIND, STRIDE, SB>(p, hv, first, tabAddr, laneOff, carry);
-        }
-        for (u32 step = 0; step < nsteps; step++) {
-            const uint4 cur = nxt;
-            nxt = load(step + 1);
-            if ((lane & 7) == 0) {
-                const u64 pos = lanePos + (u64)(step + pfDist) * 512;
-                if (pos < p.readableEnd) {
-                    prefetchL2(p.corpus + pos);
-                }
-            }
-            u32 w4 = 0;
-            if (K::HASH) {
-                /* the word after the lane's 16 bytes: one rotate shuffle in
-                 * which lane 0 offers the NEXT step's first word (for lane 31) */
-                w4 = __shfl_sync(0xffffffffu, lane == 0 ? nxt.x : cur.x, (lane + 1) & 31);
-            }
-            const u64 g0 = lanePos + (u64)step * 512;
-            scanStep<KIND, STRIDE, SB, 0>(
-                p, cur, w4, lane, tabAddr, laneOff, bitmapAddr, carry, g0, stats,
-                [&]() { return g0 ? __ldg(reinterpret_cast<const u32 *>(p.corpus + g0 - 4)) : 0u; }, wq, 0);
-        }
-    } else {
-        const u32 stepsPerTile = p.tileBytes >> 9;
-        auto issue = [&](u32 t, u32 s) { /* lane 0: TMA bulk copy of tile t -> stage s */
-            const u64 base = (u64)t * p.tileBytes;
-            u8 *dst = stages + (size_t)s * stageBytes;
-            const u64 readEnd = p.readableEnd;
-            u64 from = base - 16;
-            if (t == 0) { /* nothing before the corpus: stage bytes [0,16) stay unset */
-                from = 0;
-                dst += 16;
-            }
-            u64 to = base + p.tileBytes + 16;
-            if (to > readEnd) {
-                to = readEnd;
-            }
-            const u32 bytes = (u32)(to - from);
-            mbarExpectTx(&bars[s], bytes);
-            tmaLoad1d(dst, p.corpus + from, bytes, &bars[s]);
-        };
-        if (lane == 0) {
-            for (u32 i = 0; i < p.nstages && i < myCount; i++) {
-                issue(myFirst + i, i);
-            }
-        }
-        u32 s = 0, parity = 0;
-        for (u32 i = 0; i < myCount; i++) {
-            const u32 t = myFirst + i;
-            const u64 tileBase = (u64)t * p.tileBytes;
-            const u8 *st = stages + (size_t)s * stageBytes; /* st[16 + x] = corpus[tileBase + x] */
-            mbarWait(&bars[s], parity);
-            if (i == 0 && t != 0) {
-                const uint4 hv = *reinterpret_cast<const uint4 *>(st);
-                haloStep<KIND, STRIDE, SB>(p, hv, *reinterpret_cast<const u32 *>(st + 16), tabAddr, laneOff,
-                                           carry);
-            }
-            u32 nsteps = stepsPerTile;
-            if (tileBase + p.tileBytes > p.corpusBytes) {
-                nsteps = (u32)((p.corpusBytes - tileBase + 511) >> 9);
-            }
-            for (u32 step = 0; step < nsteps; step++) {
-                const u8 *sp = st + 16 + step * 512 + lane * 16;
-                const uint4 v = *reinterpret_cast<const uint4 *>(sp);
-                u32 w4 = 0;
-                if (K::HASH) {
-                    w4 = __shfl_down_sync(0xffffffffu, v.x, 1);
-                    if (lane == 31) {
-                        w4 = *reinterpret_cast<const u32 *>(sp + 16);
-                    }
-                }
-                const u64 g0 = tileBase + step * 512 + lane * 16;
-                scanStep<KIND, STRIDE, SB, 0>(p, v, w4, lane, tabAddr, laneOff, bitmapAddr, carry, g0, stats,
-                                              [&]() { return *reinterpret_cast<const u32 *>(sp - 4); }, wq, 0);
-            }
-            __syncwarp();
-            if (lane == 0 && i + p.nstages < myCount) {
-                issue(t + p.nstages, s); /* refill the stage just drained */
-            }
-            if (++s == p.nstages) {
-                s = 0;
-                parity ^= 1;
-            }
-        }
-    }
-    if (stats[0]) {
-        atomicAdd(p.counters + CTR_CANDIDATES, stats[0]);
-    }
-    if (stats[1]) {
-        atomicAdd(p.counters + CTR_PREFILTER_PASS, stats[1]);
-    }
-    if (stats[2]) {
-        atomicAdd(p.counters + CTR_CONFIRMED, stats[2]);
-    }
-}
-
-/* ---- wide-step variant (opt-in, runtime option `wide`) ---------------------------
+/* ---- wide-step kernel (FK_BYTE32) ------------------------------------------------
  *
  * Every lane owns 32 CONTIGUOUS bytes (8 words) per iteration and the warp 1 KiB:
- * the per-step overhead (carry shuffle, vote, loop, prefetch, next-word shuffle)
- * is paid once per 1 KiB instead of once per 512 bytes and the overflow into the
- * next lane once per 32 bytes.  Direct mode, stride 1, FK_BYTE32 / FK_HASH32 only;
- * candidates always go through the per-warp queue (entry = 8 candidate words +
- * the number of the 32-byte chunk). */
+ * the per-step overhead (carry shuffle, vote, loop, prefetch) is paid once per 1 KiB
+ * instead of once per 512 bytes and the overflow into the next lane once per 32
+ * bytes.  Candidates go through the per-warp queue (entry = 8 candidate words + the
+ * number of the 32-byte chunk). */
+enum { BYTE_TABLE_BYTES = 256 * 256 }; /* 256 rows x 32 lane copies (+ 128 B unused) */
 
 struct WideQueue {
     static constexpr u32 BYTES = 48;
@@ -1244,9 +694,7 @@ template <int O> __device__ __forceinline__ void orStreamWide(u32 (&a)[9], const
 }
 
 /* a[0..7]: the lane's own 32 end positions, a[8]: overflow into the next lane */
-template <int KIND, int SB>
-__device__ __forceinline__ void laneFilterWide(const u32 (&w)[9], u32 tabAddr, u32 laneOff, u32 indexMask,
-                                               u32 repShift, u32 (&a)[9]) {
+__device__ __forceinline__ void laneFilterWide(const u32 (&w)[8], u32 tabAddr, u32 laneOff, u32 (&a)[9]) {
 #pragma unroll
     for (int i = 0; i < 9; i++) {
         a[i] = 0;
@@ -1256,36 +704,19 @@ __device__ __forceinline__ void laneFilterWide(const u32 (&w)[9], u32 tabAddr, u
         u32 E[8];
 #pragma unroll
         for (int k = 0; k < 8; k++) {
-            if (KIND == FK_HASH32) {
-                const u32 sh = 2 + repShift;
-                u32 off;
-                if (r == 0) {
-                    off = w[k] << sh;
-                } else if (r == 3) {
-                    off = __funnelshift_r(w[k], w[k + 1], 24 - sh);
-                } else {
-                    off = w[k] >> (8 * r - sh);
-                }
-                /* (masked offset | this lane's copy) is ONE three-input logic op and
-                 * the table base stays a uniform register of the load: 3 instructions
-                 * per lookup (the 16-byte kernels spend a 4th on adding a per-lane
-                 * base; to be folded the same way once this variant is measured) */
-                E[k] = lds32(tabAddr + ((off & (indexMask << sh)) | laneOff));
-            } else {
-                E[k] = lds32(tabAddr + __byte_perm(w[k], laneOff, 0x5504 + (r << 4)));
-            }
+            E[k] = lds32(tabAddr + __byte_perm(w[k], laneOff, 0x5504 + (r << 4)));
         }
-        if (r + SB == 0) orStreamWide<0>(a, E);
-        if (r + SB == 1) orStreamWide<1>(a, E);
-        if (r + SB == 2) orStreamWide<2>(a, E);
-        if (r + SB == 3) orStreamWide<3>(a, E);
-        if (r + SB == 4) orStreamWide<4>(a, E);
+        if (r == 0) orStreamWide<0>(a, E);
+        if (r == 1) orStreamWide<1>(a, E);
+        if (r == 2) orStreamWide<2>(a, E);
+        if (r == 3) orStreamWide<3>(a, E);
     }
 }
 
-template <int SPLIT>
-__device__ __forceinline__ void drainWideBody(const ScanParams &p, u32 bitmapAddr, u32 qAddr, u32 first, u32 count,
-                                       u32 lane, u32 *stats) {
+/* One queue entry per lane: the two 16-byte halves of its 32-byte chunk, bytes read
+ * back from L2, through laneCandidates. */
+__device__ __forceinline__ void drainWide(const ScanParams &p, u32 bitmapAddr, u32 qAddr, u32 first, u32 count,
+                                          u32 lane, u32 *stats) {
     if (lane >= count) {
         return;
     }
@@ -1303,68 +734,41 @@ __device__ __forceinline__ void drainWideBody(const ScanParams &p, u32 bitmapAdd
     }
     const u32 pw = g0 ? __ldg(reinterpret_cast<const u32 *>(p.corpus + g0 - 4)) : 0u;
     if (c0.x | c0.y | c0.z | c0.w) {
-        if constexpr (SPLIT) {
-            laneCandidatesBody<1, 1>(p, bitmapAddr, c0.x, c0.y, c0.z, c0.w, 0, 0, 0, 0, v0.x, v0.y, v0.z, v0.w,
-                                     pw, g0, stats);
-        } else {
-            laneCandidates<1>(p, bitmapAddr, c0.x, c0.y, c0.z, c0.w, 0, 0, 0, 0, v0.x, v0.y, v0.z, v0.w, pw, g0,
-                              stats);
-        }
+        laneCandidates(p, bitmapAddr, c0.x, c0.y, c0.z, c0.w, v0.x, v0.y, v0.z, v0.w, pw, g0, stats);
     }
     if (c1.x | c1.y | c1.z | c1.w) {
-        if constexpr (SPLIT) {
-            laneCandidatesBody<1, 1>(p, bitmapAddr, c1.x, c1.y, c1.z, c1.w, 0, 0, 0, 0, v1.x, v1.y, v1.z, v1.w,
-                                     v0.w, g0 + 16, stats);
-        } else {
-            laneCandidates<1>(p, bitmapAddr, c1.x, c1.y, c1.z, c1.w, 0, 0, 0, 0, v1.x, v1.y, v1.z, v1.w, v0.w,
-                              g0 + 16, stats);
-        }
+        laneCandidates(p, bitmapAddr, c1.x, c1.y, c1.z, c1.w, v1.x, v1.y, v1.z, v1.w, v0.w, g0 + 16, stats);
     }
 }
 
-__device__ HSB_NOINLINE void drainWide(const ScanParams &p, u32 bitmapAddr, u32 qAddr, u32 first, u32 count,
-                                       u32 lane, u32 *stats) {
-    drainWideBody<0>(p, bitmapAddr, qAddr, first, count, lane, stats);
-}
-
-template <int KIND, int SB, int SPLIT, int MAXT>
+template <int MAXT>
 __global__ void __launch_bounds__(MAXT, 1) scanKernelWide(const HSB_GRID_CONSTANT ScanParams p) {
-    static_assert(KIND == FK_BYTE32 || KIND == FK_HASH32, "wide steps: 8-bucket tables only");
     HSB_DYNAMIC_SMEM(smem);
     const u32 lane = threadIdx.x & 31;
     const u32 warp = threadIdx.x >> 5;
     const u32 nwarps = blockDim.x >> 5;
-    const u32 tab0 = tableSmemBytes(KIND, p.tableBytes);
-    const u32 tabBytes = tab0 + p.bitmapBytes;
 
-    if (KIND == FK_BYTE32) {
+    {
         const u32 *g = reinterpret_cast<const u32 *>(p.table);
         u32 *s = reinterpret_cast<u32 *>(smem);
         for (u32 i = threadIdx.x; i < 256 * 64; i += blockDim.x) {
             s[i] = ((i >> 5) & 1) ? 0xffffffffu : __ldg(g + (i >> 6));
         }
-    } else {
-        const uint4 *g = reinterpret_cast<const uint4 *>(p.table);
-        uint4 *s = reinterpret_cast<uint4 *>(smem);
-        for (u32 i = threadIdx.x; i < p.tableBytes / 16; i += blockDim.x) {
-            s[i] = __ldg(g + i);
-        }
     }
+    /* second-stage prefilter: one bit per hash of a literal's last bytes */
     if (p.bitmapBytes) {
         const uint4 *g = reinterpret_cast<const uint4 *>(p.bitmap);
-        uint4 *sdst = reinterpret_cast<uint4 *>(smem + tab0);
+        uint4 *sdst = reinterpret_cast<uint4 *>(smem + BYTE_TABLE_BYTES);
         for (u32 i = threadIdx.x; i < p.bitmapBytes / 16; i += blockDim.x) {
             sdst[i] = __ldg(g + i);
         }
     }
     __syncthreads();
 
-    const u32 bitmapAddr = smemAddr(smem) + tab0;
-    /* laneOff: FK_BYTE32 = the lane's column of a table row; FK_HASH32 = the
-     * lane's copy of an entry (bank partition), OR-ed into the masked offset */
     const u32 tabAddr = smemAddr(smem);
-    const u32 laneOff = KIND == FK_HASH32 ? (lane & ((1u << p.repShift) - 1)) * 4 : lane * 4;
-    const u32 qAddr = smemAddr(smem) + tabBytes + warp * WideQueue::WARP_BYTES;
+    const u32 bitmapAddr = tabAddr + BYTE_TABLE_BYTES;
+    const u32 laneOff = lane * 4; /* the lane's column of a table row */
+    const u32 qAddr = bitmapAddr + p.bitmapBytes + warp * WideQueue::WARP_BYTES;
 
     /* this warp's contiguous run of tiles (tileBytes is a multiple of 1024 here) */
     const u32 gwarp = blockIdx.x * nwarps + warp;
@@ -1387,8 +791,8 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelWide(const HSB_GRID_CONSTAN
         sts64(qAddr + WideQueue::RUN_START, (u32)runStart, (u32)(runStart >> 32));
     }
 
-    u32 carry[2][2] = {{0, 0}, {0, 0}};
-    u32 stats[3] = {0, 0, 0};
+    u32 carry = 0; /* lane 31's overflow of the previous iteration */
+    u32 stats[2] = {0, 0}; /* candidates, prefilter passes */
     u32 qn = 0;
 
     auto load = [&](u32 it, uint4 &lo, uint4 &hi) {
@@ -1403,18 +807,18 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelWide(const HSB_GRID_CONSTAN
             lo = ldCs128(q0);
         }
     };
-    const u32 pfDist = p.nstages; /* L2 prefetch distance in 1 KiB iterations */
+    const u32 pfDist = p.pfDist; /* in 1 KiB iterations */
     uint4 nlo, nhi;
     load(0, nlo, nhi);
     if (runStart != 0) {
         /* only the 4 bytes before the run (and its first word) reach into it */
         const uint4 hv = __ldg(reinterpret_cast<const uint4 *>(p.corpus + runStart - 16));
         const u32 first = __shfl_sync(0xffffffffu, nlo.x, 0);
-        haloStep<KIND, 1, SB>(p, hv, first, tabAddr, laneOff, carry);
+        carry = haloStep(hv, first, tabAddr, laneOff);
     }
-    /* one iteration; `fast` (split variants, every iteration but the last ones of
-     * the corpus): the load of iteration it + 1 needs no bounds check because that
-     * whole KiB is readable for every lane */
+    /* one iteration; `fast` (every iteration but the last ones of the corpus): the
+     * load of iteration it + 1 needs no bounds check because that whole KiB is
+     * readable for every lane */
     auto iteration = [&](const u32 it, const bool fast) {
         const uint4 lo = nlo, hi = nhi;
         if (fast) {
@@ -1430,19 +834,15 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelWide(const HSB_GRID_CONSTAN
                 prefetchL2(p.corpus + pos);
             }
         }
-        u32 w8 = 0;
-        if (KIND == FK_HASH32) {
-            w8 = __shfl_sync(0xffffffffu, lane == 0 ? nlo.x : lo.x, (lane + 1) & 31);
-        }
-        const u32 w[9] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w, w8};
+        const u32 w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
         u32 a[9];
-        laneFilterWide<KIND, SB>(w, tabAddr, laneOff, p.indexMask, p.repShift, a);
+        laneFilterWide(w, tabAddr, laneOff, a);
         {
             u32 in = __shfl_sync(0xffffffffu, a[8], (lane + 31) & 31);
             if (lane == 0) {
                 const u32 next = in;
-                in = carry[0][0];
-                carry[0][0] = next;
+                in = carry;
+                carry = next;
             }
             a[0] |= in;
         }
@@ -1464,23 +864,17 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelWide(const HSB_GRID_CONSTAN
             if (qn >= 32) {
                 __syncwarp();
                 qn -= 32;
-                if constexpr (SPLIT) {
-                    drainWideBody<1>(p, bitmapAddr, qAddr, qn, 32, lane, stats);
-                } else {
-                    drainWide(p, bitmapAddr, qAddr, qn, 32, lane, stats);
-                }
+                drainWide(p, bitmapAddr, qAddr, qn, 32, lane, stats);
                 __syncwarp();
             }
         }
     };
+    const u64 readableIters = (p.readableEnd - runStart) >> 10;
+    const u32 nFast = readableIters >= (u64)niter + 1 ? niter : (readableIters ? (u32)readableIters - 1 : 0);
     u32 it = 0;
-    if (SPLIT) {
-        const u64 readableIters = (p.readableEnd - runStart) >> 10;
-        const u32 nFast = readableIters >= (u64)niter + 1 ? niter : (readableIters ? (u32)readableIters - 1 : 0);
 #pragma unroll 1
-        for (; it < nFast; it++) {
-            iteration(it, true);
-        }
+    for (; it < nFast; it++) {
+        iteration(it, true);
     }
 #pragma unroll 1
     for (; it < niter; it++) {
@@ -1488,11 +882,7 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelWide(const HSB_GRID_CONSTAN
     }
     if (qn) {
         __syncwarp();
-        if constexpr (SPLIT) {
-            drainWideBody<1>(p, bitmapAddr, qAddr, 0, qn, lane, stats);
-        } else {
-            drainWide(p, bitmapAddr, qAddr, 0, qn, lane, stats);
-        }
+        drainWide(p, bitmapAddr, qAddr, 0, qn, lane, stats);
     }
     if (stats[0]) {
         atomicAdd(p.counters + CTR_CANDIDATES, stats[0]);
@@ -1500,14 +890,11 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelWide(const HSB_GRID_CONSTAN
     if (stats[1]) {
         atomicAdd(p.counters + CTR_PREFILTER_PASS, stats[1]);
     }
-    if (stats[2]) {
-        atomicAdd(p.counters + CTR_CONFIRMED, stats[2]);
-    }
 }
 
-/* ---- class-pair variant (FK_PAIR32): conflict-free two-byte first stage -------------
+/* ---- class-pair kernel (FK_PAIR32): conflict-free two-byte first stage -------------
  *
- * The FDR hash lookup costs ~3.3 shared-memory wavefronts (random 4-byte gather of
+ * An FDR hash lookup costs ~3.3 shared-memory wavefronts (random 4-byte gather of
  * 32 lanes into 32 banks; replicas only help once every lane has its own copy).
  * A copy per lane needs a table of <= 1024 entries, i.e. a 10-bit key for the two
  * bytes: each byte is first mapped to a 5-bit CLASS by a per-lane byte table
@@ -1522,9 +909,10 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelWide(const HSB_GRID_CONSTAN
  *
  * so the pair address is ONE logic op of the two class words and every lookup is
  * PRMT/LOP3 + LDS.  Sample at x = bytes (x, x+1) keyed (c0(byte x), c1(byte x+1));
- * entry byte i says which buckets cannot END at x + i + SB (as FK_HASH32).
+ * entry byte i says which buckets cannot END at x + i + SB (SB = slot base: 1 when every
+ * literal has at least two bytes, so that all four samples see both bytes of a pair).
  * Candidates: per-warp queue -> prefilter bitmaps -> candidate list in HBM ->
- * confirmKernel (always "split": the hot kernel carries no confirm code). */
+ * confirmKernel (the hot kernel carries no confirm code). */
 
 struct PairQueue {
     static constexpr u32 SLOTS = 64;                      /* < 32 pending + <= 32 appended per step */
@@ -1582,13 +970,12 @@ __device__ __forceinline__ void pairFilter(const u32 (&w)[5], u32 clsAddr, u32 l
     }
 }
 
-/* First-level bitmap word of the class-pair kernel: index = mulhi(key * K, bits).
- * holes: word i lives in class row i >> 5 at byte 128 + 4 * (i & 31). */
+/* First-level bitmap word of the class-pair kernel: index = mulhi(key * K, bits);
+ * word i lives in class row i >> 5 at byte 128 + 4 * (i & 31). */
 __device__ __forceinline__ bool pairBitmapTest(const ScanParams &p, u32 bitmapAddr, u32 key) {
     const u32 h = __umulhi(key * 0x9E3779B1u, p.bitmapBits);
     const u32 wi = h >> 5;
-    const u32 addr = p.bitmapHoles ? bitmapAddr + ((wi >> 5) << 8) + ((wi & 31u) << 2) : bitmapAddr + (wi << 2);
-    return (lds32(addr) >> (h & 31)) & 1;
+    return (lds32(bitmapAddr + ((wi >> 5) << 8) + ((wi & 31u) << 2)) >> (h & 31)) & 1;
 }
 
 /* One queue entry per lane: the lane's candidate bytes go through the prefilter
@@ -1732,16 +1119,17 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelPair(const HSB_GRID_CONSTAN
     const u32 warp = threadIdx.x >> 5;
     const u32 nwarps = blockDim.x >> 5;
 
-    /* expand the tables: p.table = 256 class words, then 1024 pair entries */
+    /* expand the tables: p.table = 256 class words, then 1024 pair entries; the
+     * (32 KiB) prefilter bitmap, if any, fills the class rows' upper halves */
     {
         const u32 *g = reinterpret_cast<const u32 *>(p.table);
         const u32 *bm = reinterpret_cast<const u32 *>(p.bitmap);
         u32 *s = reinterpret_cast<u32 *>(smem);
-        const bool holes = p.bitmapHoles && p.bitmapBytes;
+        const bool keyed = p.bitmapBytes != 0;
         for (u32 i = threadIdx.x; i < 256 * 64; i += blockDim.x) {
             const u32 row = i >> 6, l = i & 31;
             if ((i >> 5) & 1) {
-                s[i] = holes ? __ldg(bm + row * 32 + l) : 0u;
+                s[i] = keyed ? __ldg(bm + row * 32 + l) : 0u;
             } else {
                 s[i] = __ldg(g + row) | (l << 2);
             }
@@ -1750,20 +1138,13 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelPair(const HSB_GRID_CONSTAN
         for (u32 i = threadIdx.x; i < p.pairBytes / 4; i += blockDim.x) {
             sp[i] = __ldg(g + 256 + (i >> 5));
         }
-        if (p.bitmapBytes && !holes) {
-            u32 *sb = sp + p.pairBytes / 4;
-            for (u32 i = threadIdx.x; i < p.bitmapBytes / 4; i += blockDim.x) {
-                sb[i] = __ldg(bm + i);
-            }
-        }
     }
     __syncthreads();
 
     const u32 clsAddr = smemAddr(smem);
-    const u32 contiguous = (p.bitmapHoles || !p.bitmapBytes) ? 0u : p.bitmapBytes;
-    const u32 bitmapAddr = p.bitmapHoles ? clsAddr + 128 : clsAddr + PAIR_CLASS_BYTES + p.pairBytes;
+    const u32 bitmapAddr = clsAddr + 128;
     const u32 laneOff = lane * 4;
-    const u32 qAddr = clsAddr + PAIR_CLASS_BYTES + p.pairBytes + contiguous + warp * PairQueue::WARP_BYTES;
+    const u32 qAddr = clsAddr + PAIR_CLASS_BYTES + p.pairBytes + warp * PairQueue::WARP_BYTES;
 
     /* this warp's contiguous run of tiles */
     const u32 gwarp = blockIdx.x * nwarps + warp;
@@ -1797,7 +1178,7 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelPair(const HSB_GRID_CONSTAN
         }
         return r;
     };
-    const size_t pfBytes = (size_t)p.nstages * 512 + lane * 48; /* even lanes: 16 x 128 B, 2 KiB */
+    const size_t pfBytes = (size_t)p.pfDist * 512 + lane * 48; /* even lanes: 16 x 128 B, 2 KiB */
     uint4 nxt = load(ptr, true);
     u32 prevW = 0; /* heavy: the last word of the previous step (own lane's; lane 31's is the one used) */
     if (runStart != 0) {
@@ -2037,7 +1418,7 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelGram(const HSB_GRID_CONSTAN
         return r;
     };
     auto cls = [&](u32 w, int r) -> u32 { return lds32(clsAddr + __byte_perm(w, laneOff, 0x5504 + (r << 4))); };
-    const size_t pfBytes = (size_t)p.nstages * 512 + lane * 48;
+    const size_t pfBytes = (size_t)p.pfDist * 512 + lane * 48;
 
     /* carryPack: E of the three bytes before the lane's chunk, one per byte lane (E < 128);
      * lane 0 inherits lane 31's of the previous step.  Entering a run: the bytes before it;
@@ -2158,7 +1539,7 @@ cudaError_t launchGram(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t s
     return cudaGetLastError();
 }
 
-/* Split mode, second kernel: one thread per candidate of the list the scan
+/* Second kernel of every scan: one thread per candidate of the list the scan
  * kernel filled -- hash confirm, block lookup, literal program, record. */
 __global__ void __launch_bounds__(256) confirmKernel(const HSB_GRID_CONSTANT ScanParams p) {
     const u32 total = p.counters[CTR_CANDQ];
@@ -2195,17 +1576,11 @@ __global__ void __launch_bounds__(256) confirmKernel(const HSB_GRID_CONSTANT Sca
     }
 }
 
-template <int KIND, int SB>
 cudaError_t launchWide(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream) {
-    /* builds for 768 threads (80 registers), 896 (72) and, split variant only, 1024 (64) */
-    void (*kern)(const ScanParams);
-    if (cfg.warps <= 24) {
-        kern = cfg.split ? scanKernelWide<KIND, SB, 1, 768> : scanKernelWide<KIND, SB, 0, 768>;
-    } else if (cfg.warps <= 28 || !cfg.split) {
-        kern = cfg.split ? scanKernelWide<KIND, SB, 1, 896> : scanKernelWide<KIND, SB, 0, 896>;
-    } else {
-        kern = scanKernelWide<KIND, SB, 1, 1024>; /* split only: 64 registers, still no spills */
-    }
+    /* builds for 768 threads (80 registers), 896 (72) and 1024 (64, still no spills) */
+    void (*kern)(const ScanParams) = cfg.warps <= 24   ? scanKernelWide<768>
+                                     : cfg.warps <= 28 ? scanKernelWide<896>
+                                                       : scanKernelWide<1024>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.smemBytes);
     if (e != cudaSuccess) {
         return e;
@@ -2215,69 +1590,29 @@ cudaError_t launchWide(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t s
 }
 
 template <int SB> cudaError_t launchPair(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream) {
-    /* cfg.queued == 2: the heavy candidate path (one queue entry per word with candidates) */
+    /* heavy: the candidate path with one queue entry per word with candidates */
     void (*kern)(const ScanParams) =
-        cfg.queued == 2 ? (cfg.warps <= 24 ? scanKernelPair<SB, 768, 1> : scanKernelPair<SB, 896, 1>)
-                        : (cfg.warps <= 24 ? scanKernelPair<SB, 768, 0> : scanKernelPair<SB, 896, 0>);
+        cfg.heavy ? (cfg.warps <= 24 ? scanKernelPair<SB, 768, 1> : scanKernelPair<SB, 896, 1>)
+                  : (cfg.warps <= 24 ? scanKernelPair<SB, 768, 0> : scanKernelPair<SB, 896, 0>);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.smemBytes);
     if (e != cudaSuccess) {
         return e;
     }
     HSB_LAUNCH(kern, cfg.grid, cfg.warps * 32, cfg.smemBytes, stream, p);
     return cudaGetLastError();
-}
-
-template <int KIND, int STRIDE, int SB, int DIRECT, int QUEUED>
-cudaError_t launchOne(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream) {
-    void (*kern)(const ScanParams) = scanKernel<KIND, STRIDE, SB, DIRECT, QUEUED>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.smemBytes);
-    if (e != cudaSuccess) {
-        return e;
-    }
-    HSB_LAUNCH(kern, cfg.grid, cfg.warps * 32, cfg.smemBytes, stream, p);
-    return cudaGetLastError();
-}
-
-template <int KIND, int STRIDE, int SB>
-cudaError_t launchStaging(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream) {
-    if (cfg.direct && cfg.queued) {
-        /* the queue variant is built for the default sampling stride only */
-        if constexpr (STRIDE == 1) {
-            return launchOne<KIND, STRIDE, SB, 1, 1>(cfg, p, stream);
-        } else {
-            return cudaErrorInvalidValue;
-        }
-    }
-    return cfg.direct ? launchOne<KIND, STRIDE, SB, 1, 0>(cfg, p, stream)
-                      : launchOne<KIND, STRIDE, SB, 0, 0>(cfg, p, stream);
-}
-
-template <int KIND, int SB>
-cudaError_t launchStride(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream) {
-    if (cfg.stride == 1) return launchStaging<KIND, 1, SB>(cfg, p, stream);
-    if (cfg.stride == 2) return launchStaging<KIND, 2, SB>(cfg, p, stream);
-    if (cfg.stride == 4) return launchStaging<KIND, 4, SB>(cfg, p, stream);
-    return cudaErrorInvalidValue;
 }
 
 } // namespace
 
-size_t scanSmemBytes(int kind, u32 tableBytes, u32 bitmapBytes, int warps, u32 nstages,
-                     u32 tileBytes, int queueWarps) {
+size_t scanSmemBytes(int kind, u32 tableBytes, u32 bitmapBytes, int queueWarps) {
     if (kind == FK_GRAM4) { /* class rows + 1 Mbit class 4-gram bitmap + queues */
         return (size_t)GRAM_CLASS_BYTES + GRAM_BITMAP_BYTES + (size_t)queueWarps * GramQueue::WARP_BYTES;
     }
-    if (kind == FK_PAIR32) { /* class rows + pair table (tableBytes) + contiguous bitmap, if any + queues */
-        return (size_t)PAIR_CLASS_BYTES + tableBytes + bitmapBytes + (size_t)queueWarps * PairQueue::WARP_BYTES;
+    if (kind == FK_PAIR32) { /* class rows (with the bitmap in their upper halves) + pair table + queues */
+        return (size_t)PAIR_CLASS_BYTES + tableBytes + (size_t)queueWarps * PairQueue::WARP_BYTES;
     }
-    const size_t perWarp = queueWarps < 0          ? WideQueue::WARP_BYTES /* wide-step variant */
-                           : kind == FK_BYTE64     ? QueueEntry<2>::WARP_BYTES
-                                                   : QueueEntry<1>::WARP_BYTES;
-    if (queueWarps < 0) {
-        queueWarps = -queueWarps;
-    }
-    return tableSmemBytes(kind, tableBytes) + bitmapBytes + (size_t)warps * nstages * (tileBytes + 32) +
-           (size_t)warps * nstages * 8 + (size_t)queueWarps * perWarp;
+    /* FK_BYTE32: lane-replicated byte table + bitmap + queues */
+    return (size_t)BYTE_TABLE_BYTES + bitmapBytes + (size_t)queueWarps * WideQueue::WARP_BYTES;
 }
 
 namespace {
@@ -2368,41 +1703,17 @@ cudaError_t launchPublishCount(const ScanParams &p, cudaStream_t stream) {
 }
 
 cudaError_t launchScan(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream) {
+    if (cfg.warps > (cfg.kind == FK_BYTE32 ? 32 : 28)) {
+        return cudaErrorInvalidValue;
+    }
     if (cfg.kind == FK_GRAM4) {
-        if (!cfg.split || cfg.warps > 28) {
-            return cudaErrorInvalidValue;
-        }
         return launchGram(cfg, p, stream);
     }
     if (cfg.kind == FK_PAIR32) {
-        if (!cfg.split || cfg.warps > 28) {
-            return cudaErrorInvalidValue;
-        }
         return cfg.slotBase ? launchPair<1>(cfg, p, stream) : launchPair<0>(cfg, p, stream);
     }
-    if (cfg.wide) {
-        if (!cfg.direct || cfg.stride != 1 || (p.tileBytes & 1023)) {
-            return cudaErrorInvalidValue;
-        }
-        if (cfg.kind == FK_BYTE32) {
-            return launchWide<FK_BYTE32, 0>(cfg, p, stream);
-        }
-        if (cfg.kind == FK_HASH32) {
-            return cfg.slotBase ? launchWide<FK_HASH32, 1>(cfg, p, stream)
-                                : launchWide<FK_HASH32, 0>(cfg, p, stream);
-        }
-        return cudaErrorInvalidValue;
-    }
-    switch (cfg.kind) {
-    case FK_BYTE32:
-        return launchStaging<FK_BYTE32, 1, 0>(cfg, p, stream);
-    case FK_BYTE64:
-        return launchStaging<FK_BYTE64, 1, 0>(cfg, p, stream);
-    case FK_HASH32:
-        return cfg.slotBase ? launchStride<FK_HASH32, 1>(cfg, p, stream)
-                            : launchStride<FK_HASH32, 0>(cfg, p, stream);
-    case FK_HASH64:
-        return launchStride<FK_HASH64, 0>(cfg, p, stream);
+    if (cfg.kind == FK_BYTE32 && !(p.tileBytes & 1023)) {
+        return launchWide(cfg, p, stream);
     }
     return cudaErrorInvalidValue;
 }

@@ -538,27 +538,17 @@ hs_error_t hs_b200_test_compile_programs(const char *const *lits, const size_t *
  * device, so a thread whose current device differs -- e.g. a fresh thread, device 0 --
  * can scan with a scratch that lives on another GPU. */
 
-/* Runtime tunables (process-wide; also HSB200_* environment variables):
- * "warps" per CTA, "tile_bytes", "stages" (TMA ring depth per warp),
- * "wide_fdr" (1: use all 8 FDR suffix slots), "stride" (first-stage sampling
- * stride override, 0 = as compiled), "prefilter" (shared-memory bitmap before
- * the hash confirm), "rebuild" (1: rebuild the FDR first-stage table over
- * suffix slots 1..4 from the literals; 0: use the table as compiled), "domain"
- * (rebuilt table's hash bits, 0 = as compiled), "direct" (1: corpus loaded
- * straight into registers, 0: TMA-staged tiles in shared memory), "chunk_mb"
- * (host->device pipeline granularity),
- * "initial_ring" (match records); kernel selection: "first_stage" (FDR sets: 3 =
- * class-pair tables, 1 = two-byte hash table, 2 = per-byte table), "wide" / "split"
- * (per-byte tables: 32-byte lanes / confirm in a second kernel), "queue", "replicas",
- * "pf_dist", "gram" (class 4-gram first stage: 0 never, 1 from 10 000 prefilter keys,
- * 2 whenever all literals have 4 bytes), "heavy" (class-pair candidate path: per-word
- * queue entries 0 never / 1 by the modelled rate / 2 always), "big_set",
- * "big_set_classes", "fat_pair" (fat Teddy through the class-pair kernel, 1) and
- * "dfa_ilp" (DFA kernels: blocks per lane, 1).  Options that shape the device image
- * ("wide_fdr", "prefilter", "rebuild", "domain", "first_stage", "gram", "big_set*",
- * "fat_pair") apply to scratches allocated afterwards.  The defaults are the measured
- * best (DESIGN.md section 3); the others exist for A/B runs (tools/sweep.py) and are all
- * covered by the parity tests and the fuzzer. */
+/* Runtime tunables (process-wide; also HSB200_* environment variables): the scan
+ * geometry -- "warps" per CTA (0 = 28), "tile_bytes", "pf_dist" (L2 prefetch
+ * distance), "chunk_mb" (host->device pipeline granularity), "initial_ring" (match
+ * records) -- and switches that force either side of a choice the library makes
+ * from the database: "gram" (class 4-gram first stage for FDR sets: 0 never, 1 from
+ * 10 000 prefilter keys, 2 whenever all literals have 4 bytes), "heavy" (class-pair
+ * candidate path: per-word queue entries 0 never / 1 by the modelled rate / 2
+ * always) and "dfa_ilp" (DFA kernels: blocks per lane, 1).  "gram" applies to
+ * scratches allocated afterwards.  The defaults are the measured best (DESIGN.md
+ * section 3); the others exist for A/B runs (tools/sweep.py) and tests.  Any other
+ * key: HS_INVALID. */
 hs_error_t hs_b200_set_runtime_option(const char *key, int value);
 
 /* Counters of the last finished scan: [0] raw records, [1] error, [2]

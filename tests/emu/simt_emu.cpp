@@ -76,8 +76,6 @@ void trampoline() {
 ThreadCtx *g_cur = nullptr;
 
 uint8_t *dynamicSmem() { return g_blk->smem; }
-void yieldThread() { yield(); }
-void noteProgress() { g_blk->progress++; }
 
 uint32_t warpCollective(Op op, uint32_t value, uint32_t aux) {
     Fiber *f = g_fiber;

@@ -45,8 +45,6 @@ uint8_t *dynamicSmem();               /* base of the block's dynamic shared memo
 enum Op { OP_SHFL_IDX, OP_SHFL_UP, OP_SHFL_DOWN, OP_BALLOT, OP_SYNCWARP };
 uint32_t warpCollective(Op op, uint32_t value, uint32_t aux);
 void blockBarrier();
-void yieldThread();                   /* let the other threads of the block run (spin-wait bodies) */
-void noteProgress();                  /* a spin-wait condition may have changed (deadlock detector) */
 
 /* run `body` once per thread of every block (threadIdx etc. set up) */
 void launch(dim3 grid, dim3 block, size_t smemBytes, const std::function<void()> &body);

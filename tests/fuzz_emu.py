@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Randomised parity fuzzing of the kernels on the SIMT emulator (tests/emu) against the
 unmodified reference runtime: random literal sets, block layouts and runtime options
-(default and opt-in kernel variants).  Not collected by pytest; run by hand:
+(scan geometry and the switches that force either side of the library's own choices).  Not collected by pytest; run by hand:
 
   python tests/fuzz_emu.py [--seconds 300] [--seed 1]
 """
@@ -20,10 +20,7 @@ from hyperscan_b200 import capi, synth  # noqa: E402
 import build_emu  # noqa: E402
 import oracle.ref as ref  # noqa: E402
 
-DEFAULTS = {"warps": 0, "tile_bytes": 1024, "stages": 2, "wide_fdr": 0, "stride": 1, "prefilter": 1, "rebuild": 1,
-            "domain": 0, "direct": 1, "replicas": 1, "pf_dist": 4, "queue": 2, "first_stage": 3, "wide": 1,
-            "split": 1, "big_set": 0, "big_set_classes": 4, "heavy": 1, "gram": 1, "fat_pair": 1,
-            "initial_ring": 1 << 20}
+DEFAULTS = {"warps": 0, "tile_bytes": 1024, "pf_dist": 4, "heavy": 1, "gram": 1, "initial_ring": 1 << 20}
 
 
 def fuzz_streams(args, rng):
@@ -40,7 +37,6 @@ def fuzz_streams(args, rng):
         for k, v in DEFAULTS.items():
             capi.set_runtime_option(k, v)
         capi.set_runtime_option("warps", int(rng.choice([1, 2, 5])))
-        capi.set_runtime_option("direct", int(rng.integers(0, 2)))
         total = int(rng.choice([50, 700, 5000]))
         data, _, _ = synth.ragged_corpus([total], lits, seed=int(rng.integers(1 << 30)), plant_per_kb=20, alphabet=al)
         data = data[:total]
@@ -159,35 +155,17 @@ def main():
                 flags[k] = (flags[k] & ~8) | fm[ids[k]]
         opts = dict(DEFAULTS)
         opts["warps"] = int(rng.choice([1, 2, 3, 5, 8]))
-        mode = rng.integers(0, 10)
-        if mode == 0:
-            opts.update(direct=0, wide=0, split=0, first_stage=int(rng.choice([1, 2])),
-                        tile_bytes=int(rng.choice([512, 1024, 2048])), stages=int(rng.choice([2, 3])))
-        elif mode == 1:
-            opts.update(wide=1, split=int(rng.integers(0, 2)), first_stage=int(rng.choice([1, 2, 3])),
-                        tile_bytes=int(rng.choice([1024, 4096])))
-        elif mode == 2:
-            opts.update(wide=1, split=1, first_stage=1, domain=int(rng.choice([0, 10, 12])),
-                        replicas=int(rng.choice([1, 4, 8])))
-        elif mode == 3:
-            opts.update(wide=0, split=0, queue=int(rng.integers(0, 2)), first_stage=int(rng.choice([1, 2])))
-        elif mode == 4:
-            opts.update(wide=0, split=0, first_stage=1, stride=int(rng.choice([0, 2, 4])),
-                        rebuild=int(rng.integers(0, 2)), prefilter=int(rng.integers(0, 2)))
-        elif mode == 5:
-            opts.update(wide=int(rng.integers(0, 2)), first_stage=1, domain=int(rng.choice([9, 11, 14])),
-                        replicas=int(rng.choice([0, 2, 16])), wide_fdr=int(rng.integers(0, 2)))
-        elif mode == 6:
-            opts.update(initial_ring=int(rng.choice([16, 256])), wide=int(rng.integers(0, 2)),
-                        split=int(rng.integers(0, 2)), first_stage=int(rng.choice([1, 3])))
-        elif mode == 7:   # class-pair kernel: layouts and prefilter
-            opts.update(first_stage=3, big_set=int(rng.integers(0, 2)), big_set_classes=int(rng.choice([1, 2, 4, 8])),
-                        heavy=int(rng.choice([0, 1, 2])), gram=int(rng.choice([0, 1, 2, 2])),
-                        prefilter=int(rng.integers(0, 2)), tile_bytes=int(rng.choice([512, 1024, 4096])))
-        # modes 8, 9: the defaults (class-pair for FDR sets, wide + split for the per-byte tables)
+        mode = rng.integers(0, 4)
+        if mode == 0:     # scan geometry
+            opts.update(tile_bytes=int(rng.choice([512, 1024, 2048, 4096])))
+        elif mode == 1:   # candidate list and record ring overflow -> grow and rescan
+            opts.update(initial_ring=int(rng.choice([16, 256])))
+        elif mode == 2:   # class-pair candidate paths, class 4-gram first stage
+            opts.update(heavy=int(rng.choice([0, 1, 2])), gram=int(rng.choice([0, 1, 2, 2])),
+                        tile_bytes=int(rng.choice([512, 1024, 4096])))
+        # mode 3: the defaults
+        # 16 buckets: fat Teddy, through the class-pair kernel with folded buckets
         fat = 48 < nl <= 96 and rng.random() < 0.5 and ref.best_isa() != "corei7"
-        if fat:   # 16 buckets: through the class-pair kernel (folded buckets) or the 64-bit per-byte entries
-            opts["fat_pair"] = int(rng.integers(0, 2))
         for k, v in opts.items():
             capi.set_runtime_option(k, v)
         lens = [int(x) for x in rng.choice([0, 1, 2, 3, 15, 16, 17, 31, 32, 33, 63, 511, 512, 513, 1023, 1024, 1025, 3000, 9000],
@@ -208,7 +186,7 @@ def main():
         try:
             import ctypes as C
             plat = C.byref(capi.PlatformInfo(0, capi.HS_CPU_FEATURES_AVX2, 0, 0)) if fat else None
-            db = capi.compile_lit_multi(lits, flags, ids, platform=plat)   # fat: 16-bucket Teddy (FK_BYTE64)
+            db = capi.compile_lit_multi(lits, flags, ids, platform=plat)
         except capi.HsError:
             skipped += 1
             continue

@@ -1,7 +1,6 @@
 """Kernel LOGIC on a CPU: the tests marked `gpu` (parity against the unmodified
 reference runtime, golden and recorded vectors, API behaviour, streaming,
-vectored mode) and the opt-in kernel variants of tests/test_gpu_experimental.py
-run against the SIMT-emulated build of the library (tests/emu: the kernels' own
+vectored mode) run against the SIMT-emulated build of the library (tests/emu: the kernels' own
 sources compiled as plain C++, one fiber per CUDA thread, warp intrinsics as
 rendezvous).
 
@@ -17,8 +16,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_gpu_suite_passes_on_the_simt_emulator():
-    env = dict(os.environ, HSB200_EMU="1", HSB200_EXPERIMENTAL="1", HSB200_WARPS="4", HSB_EMU_SMS="3")
+def test_gpu_suite_on_the_simt_emulator():
+    env = dict(os.environ, HSB200_EMU="1", HSB200_WARPS="4", HSB_EMU_SMS="3")
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests"), "-q", "-x", "-m", "gpu",
                         "-p", "no:cacheprovider"], cwd=ROOT, env=env, capture_output=True, text=True,
                        timeout=1500)

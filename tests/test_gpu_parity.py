@@ -55,10 +55,11 @@ def _avx2(hs):
 
 
 @pytest.mark.parametrize("nlits,lo,hi", [(49, 2, 8), (64, 3, 12), (90, 3, 8), (96, 4, 12)])
-def test_fat_teddy_16_buckets(hs, ref, nlits, lo, hi):
+def test_fat_teddy_16_buckets_folded(hs, ref, nlits, lo, hi):
     """Databases compiled for an AVX2 platform carry 16-bucket ("fat") Teddy
     (engine ids 3..10, src/fdr/teddy_avx2.c:395-447): the device runs them
-    through the FK_BYTE64 first stage (two u32 lookups per byte)."""
+    through the class-pair kernel with buckets i and i + 8 folded onto one
+    first-stage bit, which confirmKernel unfolds."""
     if ref.best_isa() == "corei7":
         pytest.skip("the reference build on this host has no fat Teddy")
     lits, flags, ids = synth.literal_set(nlits, min_len=lo, max_len=hi, seed=90 + nlits, caseless_frac=0.2,
@@ -68,17 +69,6 @@ def test_fat_teddy_16_buckets(hs, ref, nlits, lo, hi):
     db, want = _check_all(hs, ref, lits, flags, ids, data, off, ln, platform=_avx2(hs))
     assert 3 <= db.info().engine_id <= 10, db.info().engine_id
     assert want.size > 100
-    # the opt-in staging / queue variants of the same first stage
-    try:
-        for opts in ({"queue": 0}, {"direct": 0, "warps": 8, "tile_bytes": 2048, "stages": 3}):
-            for k, v in opts.items():
-                hs.set_runtime_option(k, v)
-            _check_all(hs, ref, lits, flags, ids, data, off, ln, use_brute=False, platform=_avx2(hs))
-            for k, v in (("queue", 2), ("direct", 1), ("warps", 0), ("tile_bytes", 1024), ("stages", 2)):
-                hs.set_runtime_option(k, v)
-    finally:
-        for k, v in (("queue", 2), ("direct", 1), ("warps", 0), ("tile_bytes", 1024), ("stages", 2)):
-            hs.set_runtime_option(k, v)
 
 
 def test_large_literal_set_two_level_prefilter(hs, ref):
@@ -91,24 +81,25 @@ def test_large_literal_set_two_level_prefilter(hs, ref):
     assert want.size > 300
 
 
-@pytest.mark.parametrize("opts", [{"big_set": 0}, {"big_set": 1, "big_set_classes": 1}, {"big_set": 1, "big_set_classes": 8},
-                                  {"first_stage": 1}, {"first_stage": 3, "prefilter": 0}, {"heavy": 0},
-                                  {"heavy": 2, "big_set": 0}, {"heavy": 2, "prefilter": 0}, {"gram": 2},
-                                  {"gram": 0}],
-                         ids=["small-layout", "1-class", "8-classes", "hash-table", "no-prefilter", "lane-entries",
-                              "word-entries", "word-entries-no-prefilter", "class-4-gram", "no-4-gram"])
-def test_large_literal_set_layout_variants(hs, ref, opts):
-    """The class-pair kernel's shared-memory layouts (pair table size vs. bitmap
-    size) and the older hash-table first stage give the same matches."""
+@pytest.mark.parametrize("opts,one_byte", [({}, False), ({"heavy": 0}, False), ({"heavy": 2}, False),
+                                           ({"heavy": 0}, True), ({"heavy": 2}, True), ({"gram": 2}, False),
+                                           ({"gram": 0}, False)],
+                         ids=["default", "lane-entries", "word-entries", "lane-entries-no-prefilter",
+                              "word-entries-no-prefilter", "class-4-gram", "no-4-gram"])
+def test_large_literal_set_candidate_paths(hs, ref, opts, one_byte):
+    """Both candidate paths of the class-pair kernel and the class 4-gram first
+    stage give the same matches.  One 1-byte literal leaves the set without
+    prefilter keys, so the candidates reach the list without the bitmap probe."""
     lits, flags, ids = synth.literal_set(20000, min_len=4, max_len=16, seed=52, caseless_frac=0.1)
     data, off, ln, _ = synth.block_corpus(256, 1024, lits, plant_per_kb=1.0, seed=53)
+    if one_byte:
+        lits, flags, ids = lits + [b"~"], flags + [0], ids + [max(ids) + 1]
     try:
         for k, v in opts.items():
             hs.set_runtime_option(k, v)
         _check_all(hs, ref, lits, flags, ids, data, off, ln, use_brute=False)
     finally:
-        for k, v in (("big_set", 0), ("big_set_classes", 4), ("first_stage", 3), ("prefilter", 1), ("heavy", 1),
-                     ("gram", 1)):
+        for k, v in (("heavy", 1), ("gram", 1)):
             hs.set_runtime_option(k, v)
 
 
@@ -197,49 +188,58 @@ def test_block_boundaries_do_not_leak(hs, ref):
     _check_all(hs, ref, lits, [0, 0, 0], [1, 2, 3], data, off, ln)
 
 
-VARIANT_KEYS = ("stride", "wide_fdr", "prefilter", "rebuild", "domain", "direct", "replicas")
-VARIANT_DEFAULTS = (1, 0, 1, 1, 0, 1, 0)
-
-
-@pytest.mark.parametrize("variant", [(0, 0, 1, 0, 0, 0, 0), (1, 1, 1, 1, 0, 1, 0), (2, 0, 0, 1, 0, 0, 1),
-                                     (4, 1, 1, 0, 0, 1, 0), (1, 0, 0, 0, 0, 1, 0), (1, 0, 1, 1, 11, 1, 16),
-                                     (2, 0, 1, 1, 15, 0, 0), (1, 0, 1, 1, 9, 0, 2), (1, 0, 1, 1, 12, 1, 8)])
-def test_filter_variants_same_matches(hs, ref, variant):
-    """Sampling stride, slot set, hash domain, staging mode and the prefilter only
-    change the candidate set of the first stages, never the matches."""
+def test_short_literals_pair_kernel_paths(hs, ref):
+    """A 500-literal FDR set on the class-pair kernel, then the same set with 1- and
+    2-byte literals added: slot base 0 and no prefilter bitmap."""
     lits, flags, ids = synth.literal_set(500, min_len=4, max_len=14, seed=21, caseless_frac=0.3,
                                          alphabet=b"abcdefgh")
-    lits += [b"ab", b"b", b"cdc"]  # short literals force slot base 0 in some variants
+    lits += [b"ab", b"b", b"cdc"]
     flags += [0, 1, 0]
     ids += [1000, 1001, 1002]
     data, off, ln = synth.ragged_corpus([70000, 33, 5000, 0, 12345], lits, seed=13, plant_per_kb=3,
                                         alphabet=b"abcdefghABCDEFGH")
-    try:
-        for k, v in zip(VARIANT_KEYS, variant):
-            hs.set_runtime_option(k, v)
-        _check_all(hs, ref, lits[:500], flags[:500], ids[:500], data, off, ln, use_brute=False)
-        _check_all(hs, ref, lits, flags, ids, data[:20000], off[:1], ln[:1] // 4, use_brute=False)
-    finally:
-        for k, v in zip(VARIANT_KEYS, VARIANT_DEFAULTS):
-            hs.set_runtime_option(k, v)
+    _check_all(hs, ref, lits[:500], flags[:500], ids[:500], data, off, ln, use_brute=False)
+    _check_all(hs, ref, lits, flags, ids, data[:20000], off[:1], ln[:1] // 4, use_brute=False)
 
 
-@pytest.mark.parametrize("tile,warps,stages,direct", [(512, 1, 2, 0), (1024, 4, 2, 0), (4096, 8, 4, 0),
-                                                       (2048, 16, 3, 0), (512, 3, 2, 1), (8192, 24, 2, 1)])
-def test_tile_geometry_invariance(hs, ref, tile, warps, stages, direct):
+@pytest.mark.parametrize("tile,warps", [(512, 1), (1024, 4), (4096, 8), (2048, 16), (512, 3), (8192, 24)])
+def test_tile_split_invariance(hs, ref, tile, warps):
+    """The split of the tiles over the warps and CTAs never changes the matches."""
     lits, flags, ids = synth.literal_set(300, seed=4, alphabet=b"abcdefgh")
     data, off, ln, _ = synth.block_corpus(257, 1000, lits, plant_per_kb=2.0, seed=8)
     try:
         hs.set_runtime_option("tile_bytes", tile)
         hs.set_runtime_option("warps", warps)
-        hs.set_runtime_option("stages", stages)
-        hs.set_runtime_option("direct", direct)
         _check_all(hs, ref, lits, flags, ids, data, off, ln, use_brute=False)
     finally:
         hs.set_runtime_option("tile_bytes", 1024)
         hs.set_runtime_option("warps", 0)
-        hs.set_runtime_option("stages", 2)
-        hs.set_runtime_option("direct", 1)
+
+
+GEOMETRIES = [{"warps": 24},                        # the 768-thread kernel builds
+              {"warps": 32},                        # the 1024-thread build of the wide kernel
+              {"tile_bytes": 4096, "warps": 5},
+              {"initial_ring": 16}]                 # candidate list and ring overflow -> grow and rescan
+GEOMETRY_DEFAULTS = {"warps": 0, "tile_bytes": 1024, "initial_ring": 1 << 20}
+
+
+@pytest.mark.parametrize("opts", GEOMETRIES, ids=[",".join("%s=%d" % kv for kv in g.items()) for g in GEOMETRIES])
+@pytest.mark.parametrize("nlits", [1, 30, 48, 300, 1000])
+def test_geometry_parity(hs, ref, opts, nlits):
+    """Noodle (1), 8-bucket Teddy (30, 48) and FDR sets (300, 1000) under the kernel
+    builds and ring sizes a geometry option selects."""
+    lits, flags, ids = synth.literal_set(nlits, min_len=2 if nlits < 40 else 4, max_len=12, seed=nlits + 7,
+                                         caseless_frac=0.2, alphabet=b"abcdefgh")
+    data, off, ln = synth.ragged_corpus([0, 1, 3, 15, 16, 17, 31, 32, 33, 100, 511, 512, 513, 1023, 1024, 1025,
+                                         2047, 2048, 2049, 4096, 10000, 65536 + 5, 200000], lits, seed=3,
+                                        alphabet=b"abcdefghABCDxy")
+    try:
+        for k, v in opts.items():
+            hs.set_runtime_option(k, v)
+        _check_all(hs, ref, lits, flags, ids, data, off, ln, use_brute=False)
+    finally:
+        for k, v in GEOMETRY_DEFAULTS.items():
+            hs.set_runtime_option(k, v)
 
 
 def test_config2_shape_sample(hs, ref):

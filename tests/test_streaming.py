@@ -133,7 +133,7 @@ def test_device_stream_termination_copy_reset(hs, ref):
 @pytest.mark.parametrize("nl,wlen,fat", [(40, 64, 0), (300, 1024, 0), (1, 33, 0), (80, 200, 1)])
 def test_stream_set_equals_per_stream_reference(hs, ref, nl, wlen, fat):
     """hs_b200_streams_scan (state in HBM) == one reference stream per stream.
-    fat: compiled for an AVX2 platform -> 16-bucket Teddy (FK_BYTE64 first stage)."""
+    fat: compiled for an AVX2 platform -> 16-bucket Teddy (class-pair first stage, buckets folded)."""
     lits, flags, ids = synth.literal_set(nl, min_len=2, max_len=8, seed=nl + 7, caseless_frac=0.2,
                                          alphabet=b"abcdef")
     plat = None

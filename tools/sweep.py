@@ -15,12 +15,9 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from hyperscan_b200 import capi, synth  # noqa: E402
 
-DEFAULT = ("replicas=1;replicas=2;replicas=4;domain=12,replicas=8;domain=12,replicas=4;domain=11,replicas=16;"
-           "domain=14,replicas=2;domain=14,replicas=1;domain=10,replicas=16;domain=12,replicas=8,warps=20;"
-           "replicas=4,direct=0,warps=24,tile_bytes=1024;replicas=4,tile_bytes=4096")
-BASE = {"warps": 0, "tile_bytes": 1024, "stages": 2, "wide_fdr": 0, "stride": 1, "prefilter": 1,
-        "rebuild": 1, "domain": 0, "direct": 1, "replicas": 1, "pf_dist": 4, "queue": 2, "first_stage": 3, "wide": 1,
-        "split": 1, "big_set": 0, "big_set_classes": 4, "heavy": 1, "gram": 1, "fat_pair": 1}
+DEFAULT = ("pf_dist=4;pf_dist=2;pf_dist=8;pf_dist=16;warps=24;warps=32;tile_bytes=4096;heavy=0;heavy=2;"
+           "gram=0;gram=2")
+BASE = {"warps": 0, "tile_bytes": 1024, "pf_dist": 4, "heavy": 1, "gram": 1}
 
 
 def main():
