@@ -24,6 +24,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <new>
 #include <unordered_map>
 #include <unordered_set>
@@ -148,67 +149,6 @@ struct DeviceGuard {
         }                                                                                  \
     } while (0)
 
-/* Second-stage prefilter: a bitmap over a hash of each literal's last
- * keyBytes bytes (don't-care bits of LitInfo.msk -- caseless letters --
- * enumerated).  A clear bit proves no literal ends at a candidate position, so
- * the hash confirm in HBM/L2 is only reached by ~1% of the first stage's false
- * positives.  Returns an empty vector when the set cannot be keyed usefully. */
-std::vector<u8> buildBitmap(const std::vector<LitTail> &tails, u32 *keyBytes, u32 *shift,
-                            std::vector<u8> *level2 = nullptr, u32 *shift2 = nullptr) {
-    std::vector<u8> bm;
-    if (tails.empty()) {
-        return bm;
-    }
-    u32 m = 4;
-    for (const LitTail &t : tails) {
-        m = std::min(m, t.size);
-    }
-    if (m < 2) {
-        return bm; /* single-byte literals: the first stage is already exact */
-    }
-    std::vector<u32> keys;
-    for (const LitTail &t : tails) {
-        const u32 v = (u32)(t.v >> 32) >> (8 * (4 - m));
-        const u32 care = (u32)(t.msk >> 32) >> (8 * (4 - m));
-        const u32 full = m == 4 ? 0xffffffffu : (1u << (8 * m)) - 1;
-        const u32 dc = ~care & full;
-        if (__builtin_popcount(dc) > 10) {
-            return std::vector<u8>(); /* too loose to enumerate */
-        }
-        u32 sub = 0;
-        do {
-            keys.push_back((v & care) | sub);
-            sub = (sub - dc) & dc;
-        } while (sub);
-    }
-    u32 lg = 13; /* 8 Kbit .. 512 Kbit (64 KB), ~256 bits per key when possible */
-    while (lg < 19 && (1ull << lg) < (u64)keys.size() * 256) {
-        lg++;
-    }
-    bm.assign((size_t)1 << (lg - 3), 0);
-    for (u32 k : keys) {
-        const u32 h = (k * 0x9E3779B1u) >> (32 - lg);
-        bm[h >> 3] |= (u8)(1u << (h & 7));
-    }
-    *keyBytes = m;
-    *shift = 32 - lg;
-    if (level2 && shift2 && keys.size() * 32 > ((size_t)1 << lg)) {
-        /* the shared-memory bitmap is more than ~3 % full: add a level with
-         * ~1024 bits per key (<= 64 MB), probed only by its survivors */
-        u32 lg2 = lg + 1;
-        while (lg2 < 29 && (1ull << lg2) < (u64)keys.size() * 1024) {
-            lg2++;
-        }
-        level2->assign((size_t)1 << (lg2 - 3), 0);
-        for (u32 k : keys) {
-            const u32 h = (k * 0x85EBCA6Bu) >> (32 - lg2);
-            (*level2)[h >> 3] |= (u8)(1u << (h & 7));
-        }
-        *shift2 = 32 - lg2;
-    }
-    return bm;
-}
-
 /* Keys of the prefilter bitmaps: every literal's last m <= 4 bytes with the
  * don't-care bits of LitInfo.msk enumerated.  false = cannot be keyed usefully. */
 bool tailKeys(const std::vector<LitTail> &tails, u32 *keyBytes, std::vector<u32> *keys) {
@@ -220,7 +160,7 @@ bool tailKeys(const std::vector<LitTail> &tails, u32 *keyBytes, std::vector<u32>
         m = std::min(m, t.size);
     }
     if (m < 2) {
-        return false;
+        return false; /* single-byte literals: the first stage is already exact */
     }
     for (const LitTail &t : tails) {
         const u32 v = (u32)(t.v >> 32) >> (8 * (4 - m));
@@ -228,7 +168,7 @@ bool tailKeys(const std::vector<LitTail> &tails, u32 *keyBytes, std::vector<u32>
         const u32 full = m == 4 ? 0xffffffffu : (1u << (8 * m)) - 1;
         const u32 dc = ~care & full;
         if (__builtin_popcount(dc) > 10) {
-            return false;
+            return false; /* too loose to enumerate */
         }
         u32 sub = 0;
         do {
@@ -240,9 +180,51 @@ bool tailKeys(const std::vector<LitTail> &tails, u32 *keyBytes, std::vector<u32>
     return true;
 }
 
+/* Second level of the prefilter bitmaps, in HBM / L2 and probed only by the first
+ * level's survivors: ~1024 bits per key, at least 2^lg bits, <= 64 MB.  Returns
+ * its shift (32 - log2(bits)). */
+u32 buildLevel2(const std::vector<u32> &keys, u32 lg, std::vector<u8> *level2) {
+    while (lg < 29 && (1ull << lg) < (u64)keys.size() * 1024) {
+        lg++;
+    }
+    level2->assign((size_t)1 << (lg - 3), 0);
+    for (u32 k : keys) {
+        const u32 h = (k * 0x85EBCA6Bu) >> (32 - lg);
+        (*level2)[h >> 3] |= (u8)(1u << (h & 7));
+    }
+    return 32 - lg;
+}
+
+/* Second-stage prefilter of the wide kernel: a bitmap over a hash of each literal's
+ * last keyBytes bytes (tailKeys).  A clear bit proves no literal ends at a candidate
+ * position, so the hash confirm in HBM/L2 is only reached by ~1% of the first stage's
+ * false positives.  Returns an empty vector when the set cannot be keyed usefully. */
+std::vector<u8> buildBitmap(const std::vector<LitTail> &tails, u32 *keyBytes, u32 *shift,
+                            std::vector<u8> *level2, u32 *shift2) {
+    std::vector<u32> keys;
+    u32 m = 0;
+    if (!tailKeys(tails, &m, &keys)) {
+        return std::vector<u8>();
+    }
+    u32 lg = 13; /* 8 Kbit .. 512 Kbit (64 KB), ~256 bits per key when possible */
+    while (lg < 19 && (1ull << lg) < (u64)keys.size() * 256) {
+        lg++;
+    }
+    std::vector<u8> bm((size_t)1 << (lg - 3), 0);
+    for (u32 k : keys) {
+        const u32 h = (k * 0x9E3779B1u) >> (32 - lg);
+        bm[h >> 3] |= (u8)(1u << (h & 7));
+    }
+    *keyBytes = m;
+    *shift = 32 - lg;
+    if (keys.size() * 32 > ((size_t)1 << lg)) {
+        *shift2 = buildLevel2(keys, lg + 1, level2); /* the first level is more than ~3 % full */
+    }
+    return bm;
+}
+
 /* FK_PAIR32 bitmaps: first level of `bits` bits (index = mulhi(key * K, bits)) in
- * shared memory, second level (~1024 bits per key, <= 64 MB) in HBM / L2 when the
- * first is more than ~3 % full. */
+ * shared memory, second level in HBM / L2 when the first is more than ~3 % full. */
 void buildPairBitmaps(const std::vector<u32> &keys, u32 bits, std::vector<u8> *level1,
                       std::vector<u8> *level2, u32 *shift2) {
     level1->assign((size_t)(bits + 31) / 32 * 4, 0);
@@ -250,19 +232,7 @@ void buildPairBitmaps(const std::vector<u32> &keys, u32 bits, std::vector<u8> *l
         const u32 h = (u32)(((u64)(k * 0x9E3779B1u) * bits) >> 32);
         (*level1)[h >> 3] |= (u8)(1u << (h & 7));
     }
-    *shift2 = 0;
-    if (keys.size() * 32 > bits) {
-        u32 lg2 = 20;
-        while (lg2 < 29 && (1ull << lg2) < (u64)keys.size() * 1024) {
-            lg2++;
-        }
-        level2->assign((size_t)1 << (lg2 - 3), 0);
-        for (u32 k : keys) {
-            const u32 h = (k * 0x85EBCA6Bu) >> (32 - lg2);
-            (*level2)[h >> 3] |= (u8)(1u << (h & 7));
-        }
-        *shift2 = 32 - lg2;
-    }
+    *shift2 = keys.size() * 32 > bits ? buildLevel2(keys, 20, level2) : 0;
 }
 
 /* FK_GRAM4 tables: a byte -> class map (<= 32 classes) and the 1 Mbit bitmap of the class
@@ -752,6 +722,10 @@ struct hs_b200_corpus {
     u32 uniformLen = 0;      /* all blocks equally long (and uniformPitch set): tables not needed */
     u64 payload = 0;         /* sum of block lengths */
     size_t capData = 0, capBlocks = 0; /* allocation sizes when reused */
+    /* the pitched corpus of a stream set (kernels.h ScanParams.streamPitch) */
+    u32 streamPitch = 0;
+    const u8 *streamHist = nullptr;
+    const u64 *streamOffset = nullptr;
 };
 
 /* ---- scratch ------------------------------------------------------------------ */
@@ -762,7 +736,6 @@ struct hs_scratch {
     int device;
     void *alloc_base;        /* what g_scratch_alloc returned */
     cudaStream_t stream, copyStream;
-    cudaStream_t activeStream; /* stream the pending scan was enqueued on */
     cudaEvent_t evStart, evStop;
     cudaEvent_t evDone;       /* counters of the pending scan have landed on the host */
     std::vector<cudaEvent_t> *chunkEvents;
@@ -776,8 +749,6 @@ struct hs_scratch {
     size_t h_stageCap, h_stage2Cap;
     cudaEvent_t evStage, evStage2;
     std::vector<u64> *tmpOff;
-    const DevImage *lastImage;
-    const hs_b200_corpus *lastCorpus;
     /* fused exchange over peer memory (hs_b200_set_peer_exchange) */
     u32 nPeers, myRank, peerCap, blockBase;
     DevMatch *peers[MAX_PEERS];
@@ -799,6 +770,21 @@ hs_error_t validDb(const hs_database_t *db) { /* src/database.h:125-137 */
     }
     return HS_SUCCESS;
 }
+
+/* A database the scan entry points of `mode` accept: valid, bytecode 16-byte aligned */
+hs_error_t checkDb(const hs_database_t *db, u32 mode) {
+    hs_error_t r = validDb(db);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    const RoseEngine *rose = dbRose(db);
+    if ((uintptr_t)rose % 16) {
+        return HS_INVALID;
+    }
+    return rose->mode == mode ? HS_SUCCESS : HS_DB_MODE_ERROR;
+}
+
+bool validScratch(const hs_scratch *s) { return s && (uintptr_t)s % 64 == 0 && s->magic == SCRATCH_MAGIC; }
 
 hs_error_t dbIsValid(const hs_database_t *db) { /* src/database.c:326-350 */
     hs_error_t r = validDb(db);
@@ -858,6 +844,12 @@ hs_error_t growRing(hs_scratch *s, u32 cap) {
     s->d_out = n;
     s->outCap = cap;
     return HS_SUCCESS;
+}
+
+/* After a scan that produced `count` records into a ring too small for them: grow it
+ * with a quarter to spare, so that the rescan fits */
+hs_error_t growRingFor(hs_scratch *s, u32 count) {
+    return growRing(s, (u32)std::min<u64>((u64)count + count / 4 + 1024, 0xfffffff0ull));
 }
 
 void freeCorpus(hs_b200_corpus *c) {
@@ -972,6 +964,9 @@ void fillParams(const hs_scratch *s, const DevImage *im, const hs_b200_corpus *c
     p->nblocks = (u32)c->nblocks;
     p->uniformPitch = c->uniformPitch;
     p->uniformLen = c->uniformLen;
+    p->streamPitch = c->streamPitch;
+    p->streamHist = c->streamHist;
+    p->streamOffset = c->streamOffset;
     p->bc = im->d_bc;
     p->table = im->d_table;
     p->tableBytes = im->tableBytes;
@@ -1000,7 +995,30 @@ void fillParams(const hs_scratch *s, const DevImage *im, const hs_b200_corpus *c
     }
 }
 
-/* Launch over tiles [t0, t1) of the corpus on `stream`. */
+/* Run an engine (dp from engineParams; its bytes at `nfa` in device memory) over every
+ * block of corpus c, into the record ring out[0, outCap) and its counters. */
+cudaError_t launchEngine(DfaParams dp, const u8 *nfa, const hs_b200_corpus *c, DevMatch *out, u32 outCap,
+                         u32 *counters, int smCount, int maxSmem, cudaStream_t stream) {
+    dp.corpus = c->d_data;
+    dp.readableEnd = c->readableEnd;
+    dp.blockOff = c->d_off;
+    dp.blockLen = c->d_len;
+    dp.nblocks = (u32)c->nblocks;
+    dp.uniformPitch = c->uniformPitch;
+    dp.uniformLen = c->uniformLen;
+    dp.nfa = nfa;
+    dp.out = out;
+    dp.outCap = outCap;
+    dp.counters = counters;
+    const cudaError_t e = launchDfa(dp, smCount, maxSmem, stream);
+    if (e == cudaSuccess) {
+        g_launches++;
+    }
+    return e;
+}
+
+/* Launch over tiles [t0, t1) of the corpus on `stream`; t0 == 0 is the first range of a
+ * scan, whose counters were all cleared just before. */
 hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
                        const ScanPlan &pl, u32 t0, u32 t1, cudaStream_t stream) {
     if (t1 <= t0) {
@@ -1013,23 +1031,8 @@ hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
         if (t1 < ntiles) {
             return HS_SUCCESS;
         }
-        DfaParams dp = im->nfaParams;
-        dp.corpus = c->d_data;
-        dp.readableEnd = c->readableEnd;
-        dp.blockOff = c->d_off;
-        dp.blockLen = c->d_len;
-        dp.nblocks = (u32)c->nblocks;
-        dp.uniformPitch = c->uniformPitch;
-        dp.uniformLen = c->uniformLen;
-        dp.nfa = im->d_bc + im->nfaOffset;
-        dp.out = s->d_out;
-        dp.outCap = s->outCap;
-        dp.counters = s->d_counters;
-        int smCount = 0, maxSmem = 0;
-        cudaDeviceGetAttribute(&smCount, cudaDevAttrMultiProcessorCount, s->device);
-        cudaDeviceGetAttribute(&maxSmem, cudaDevAttrMaxSharedMemoryPerBlockOptin, s->device);
-        CUDA_TRY(launchDfa(dp, smCount, maxSmem, stream));
-        g_launches++;
+        CUDA_TRY(launchEngine(im->nfaParams, im->d_bc + im->nfaOffset, c, s->d_out, s->outCap, s->d_counters,
+                              s->smCount, s->maxSmem, stream));
         return HS_SUCCESS;
     }
     ScanParams p;
@@ -1039,7 +1042,9 @@ hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
     LaunchCfg cfg = pl.cfg;
     const u32 perCta = (u32)cfg.warps;
     cfg.grid = (int)std::min<u32>((u32)cfg.grid, (p.ntiles + perCta - 1) / perCta);
-    CUDA_TRY(cudaMemsetAsync(s->d_counters + CTR_CANDQ, 0, sizeof(u32), stream));
+    if (t0 > 0) {
+        CUDA_TRY(cudaMemsetAsync(s->d_counters + CTR_CANDQ, 0, sizeof(u32), stream));
+    }
     CUDA_TRY(launchScan(cfg, p, stream));
     g_launches++;
     CUDA_TRY(launchConfirm(cfg, p, stream));
@@ -1108,9 +1113,20 @@ hs_error_t finishScan(hs_scratch *s, u32 *count) {
     return HS_SUCCESS;
 }
 
-/* Enqueue: reset counters, scan the whole corpus, read the counters back. */
+/* A corpus still on its way from the host, in nchunks pieces.  chunk(ci, &covered)
+ * issues piece ci's copy, makes the scan stream wait for it, and returns how long a
+ * prefix of the corpus is then on the device.  The scan launches the tiles of that
+ * prefix before it asks for the next piece, so each copy (and the host-side packing
+ * of the next piece) overlaps the kernels of the pieces before it. */
+struct Upload {
+    size_t nchunks;
+    std::function<hs_error_t(size_t ci, u64 *covered)> chunk;
+};
+
+/* Enqueue a scan of the whole corpus on `stream`: reset the counters, launch the tile
+ * ranges, read the counters back.  The only place a scan's stream sequence is issued. */
 hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
-                       cudaStream_t stream) {
+                       cudaStream_t stream, const Upload *up = nullptr) {
     ScanPlan pl;
     hs_error_t r = planScan(s, im, &pl);
     if (r != HS_SUCCESS) {
@@ -1119,7 +1135,22 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
     CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), stream));
     CUDA_TRY(cudaEventRecord(s->evStart, stream));
     const u32 ntiles = (u32)((c->bytes + pl.tileBytes - 1) / pl.tileBytes);
-    r = launchRange(s, im, c, pl, 0, ntiles, stream);
+    u32 tDone = 0;
+    for (size_t ci = 0; up && ci < up->nchunks; ci++) {
+        u64 covered = 0;
+        r = up->chunk(ci, &covered);
+        if (r != HS_SUCCESS) {
+            return r;
+        }
+        /* tiles wholly inside the copied prefix (plus look-ahead) */
+        const u32 tEnd = covered >= c->bytes ? ntiles : covered > 16 ? (u32)((covered - 16) / pl.tileBytes) : 0;
+        r = launchRange(s, im, c, pl, tDone, tEnd, stream);
+        if (r != HS_SUCCESS) {
+            return r;
+        }
+        tDone = std::max(tDone, tEnd);
+    }
+    r = launchRange(s, im, c, pl, tDone, ntiles, stream);
     if (r != HS_SUCCESS) {
         return r;
     }
@@ -1133,47 +1164,89 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
     CUDA_TRY(cudaMemcpyAsync(s->h_counters, s->d_counters, CTR_COUNT * sizeof(u32),
                              cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaEventRecord(s->evDone, stream));
-    s->lastImage = im;
-    s->lastCorpus = c;
-    s->activeStream = stream;
     s->pending = true;
     return HS_SUCCESS;
 }
 
-/* Fill a corpus handle from host blocks.  Returns through *direct whether the
+double nowMs() {
+    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
+}
+
+struct ScanTimes {
+    double enqueued = 0, waited = 0, read = 0; /* nowMs() after each step of the last pass */
+};
+
+/* Scan a corpus on the scratch's stream (uploading it through `up`, if given) and
+ * read its records back: ordered, with the report rules applied (postprocessVec), or
+ * raw when !ordered.  When the record ring overflows, it grows and the corpus, resident
+ * by then, is scanned again as one range.  A second pass finds the real record count;
+ * a third may be needed, because the candidate list can overflow before the ring does.
+ * A third overflow is an error. */
+hs_error_t scanRecords(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c, const Upload *up,
+                       bool ordered, std::vector<DevMatch> *matches, ScanTimes *times = nullptr) {
+    ScanTimes unused;
+    ScanTimes &t = times ? *times : unused;
+    for (int attempt = 0; attempt < 3; attempt++) {
+        hs_error_t r = enqueueScan(s, im, c, s->stream, attempt == 0 ? up : nullptr);
+        if (r != HS_SUCCESS) {
+            return r;
+        }
+        t.enqueued = nowMs();
+        u32 count = 0;
+        r = finishScan(s, &count);
+        t.waited = nowMs();
+        if (r != HS_SUCCESS) {
+            return r;
+        }
+        if (count > s->outCap) {
+            r = growRingFor(s, count);
+            if (r != HS_SUCCESS) {
+                return r;
+            }
+            continue;
+        }
+        matches->resize(count);
+        if (count) {
+            CUDA_TRY(cudaMemcpyAsync(matches->data(), s->d_out, (size_t)count * sizeof(DevMatch),
+                                     cudaMemcpyDeviceToHost, s->stream));
+            CUDA_TRY(cudaStreamSynchronize(s->stream));
+        }
+        t.read = nowMs();
+        return ordered ? postprocessVec(im, matches) : HS_SUCCESS;
+    }
+    return HS_UNKNOWN_ERROR;
+}
+
+/* Lay host blocks out for a corpus handle.  Returns through *direct whether the
  * caller's buffer could be copied as it lies (all starts 16-byte aligned
- * relative to the first block, ascending, disjoint). */
-hs_error_t layoutBlocks(hs_scratch *s, const unsigned long long *offsets,
-                        const unsigned *lengths, size_t nblocks, std::vector<u64> *packed,
-                        u64 *total, u64 *payload, bool *direct, u32 *uniPitch = nullptr,
-                        u32 *uniLen = nullptr) {
-    (void)s;
-    if (uniPitch) {
-        *uniPitch = *uniLen = 0;
-        /* fast path (hsbench-style corpora): equally long blocks at a fixed
-         * 16-byte aligned pitch -- one tight pass, no packed table at all */
-        if (nblocks >= 2 && lengths[0] && offsets[1] > offsets[0]) {
-            const u64 base = offsets[0], pitch = offsets[1] - offsets[0];
-            const u32 len0 = lengths[0];
-            if (pitch % 16 == 0 && pitch <= 0xffffffffu && len0 <= pitch) {
-                /* two simple loops the compiler vectorises */
-                size_t bad = 0;
-                u64 expect = base;
-                for (size_t i = 0; i < nblocks; i++, expect += pitch) {
-                    bad += offsets[i] != expect;
-                }
-                for (size_t i = 0; i < nblocks; i++) {
-                    bad += lengths[i] != len0;
-                }
-                if (!bad) {
-                    packed->clear();
-                    *total = (nblocks - 1) * pitch + len0;
-                    *payload = (u64)nblocks * len0;
-                    *direct = true;
-                    *uniPitch = (u32)pitch;
-                    *uniLen = len0;
-                    return HS_SUCCESS;
-                }
+ * relative to the first block, ascending, disjoint), and through *uniPitch and
+ * *uniLen (or zeros) that it also holds equally long blocks at a fixed pitch. */
+void layoutBlocks(const unsigned long long *offsets, const unsigned *lengths, size_t nblocks,
+                  std::vector<u64> *packed, u64 *total, u64 *payload, bool *direct, u32 *uniPitch, u32 *uniLen) {
+    *uniPitch = *uniLen = 0;
+    /* fast path (hsbench-style corpora): equally long blocks at a fixed
+     * 16-byte aligned pitch -- one tight pass, no packed table at all */
+    if (nblocks >= 2 && lengths[0] && offsets[1] > offsets[0]) {
+        const u64 base = offsets[0], pitch = offsets[1] - offsets[0];
+        const u32 len0 = lengths[0];
+        if (pitch % 16 == 0 && pitch <= 0xffffffffu && len0 <= pitch) {
+            /* two simple loops the compiler vectorises */
+            size_t bad = 0;
+            u64 expect = base;
+            for (size_t i = 0; i < nblocks; i++, expect += pitch) {
+                bad += offsets[i] != expect;
+            }
+            for (size_t i = 0; i < nblocks; i++) {
+                bad += lengths[i] != len0;
+            }
+            if (!bad) {
+                packed->clear();
+                *total = (nblocks - 1) * pitch + len0;
+                *payload = (u64)nblocks * len0;
+                *direct = true;
+                *uniPitch = (u32)pitch;
+                *uniLen = len0;
+                return;
             }
         }
     }
@@ -1207,7 +1280,6 @@ hs_error_t layoutBlocks(hs_scratch *s, const unsigned long long *offsets,
     *total = prevEnd;
     *payload = pay;
     *direct = ok;
-    return HS_SUCCESS;
 }
 
 } // namespace
@@ -1353,7 +1425,7 @@ hs_error_t hs_alloc_scratch(const hs_database_t *db, hs_scratch_t **scratch) {
     }
     hs_scratch *s = *scratch;
     if (s) {
-        if ((uintptr_t)s % 64 || s->magic != SCRATCH_MAGIC) {
+        if (!validScratch(s)) {
             return HS_INVALID;
         }
         if (markInUse(s)) {
@@ -1382,7 +1454,7 @@ hs_error_t hs_alloc_scratch(const hs_database_t *db, hs_scratch_t **scratch) {
 }
 
 hs_error_t hs_clone_scratch(const hs_scratch_t *src, hs_scratch_t **dest) {
-    if (!dest || !src || (uintptr_t)src % 64 || src->magic != SCRATCH_MAGIC) {
+    if (!dest || !validScratch(src)) {
         return HS_INVALID;
     }
     *dest = nullptr;
@@ -1393,21 +1465,17 @@ hs_error_t hs_clone_scratch(const hs_scratch_t *src, hs_scratch_t **dest) {
         return r;
     }
     for (const DevImage *im : *src->images) {
-        const DevImage *mine = nullptr;
         /* rebuild from the source image's own copy of the database: the application may
          * have freed the original (legal in the reference, whose clone never touches it) */
         const hs_database_t *copy = (const hs_database_t *)(im->dbCopy.data() + im->dbCopyShift);
         DevImage *fresh = nullptr;
         r = buildImage(copy, &fresh);
-        if (r == HS_SUCCESS) {
-            fresh->db = im->db; /* keep the identity the application knows */
-            s->images->push_back(fresh);
-            mine = fresh;
-        }
         if (r != HS_SUCCESS) {
             hs_free_scratch(s);
             return r;
         }
+        fresh->db = im->db; /* keep the identity the application knows */
+        s->images->push_back(fresh);
     }
     r = growRing(s, src->outCap);
     if (r != HS_SUCCESS) {
@@ -1419,7 +1487,7 @@ hs_error_t hs_clone_scratch(const hs_scratch_t *src, hs_scratch_t **dest) {
 }
 
 hs_error_t hs_scratch_size(const hs_scratch_t *scratch, size_t *size) {
-    if (!size || !scratch || (uintptr_t)scratch % 64 || scratch->magic != SCRATCH_MAGIC) {
+    if (!size || !validScratch(scratch)) {
         return HS_INVALID;
     }
     size_t n = sizeof(hs_scratch) + 64 + (size_t)scratch->outCap * sizeof(DevMatch);
@@ -1437,7 +1505,7 @@ hs_error_t hs_free_scratch(hs_scratch_t *s) {
     if (!s) {
         return HS_SUCCESS;
     }
-    if ((uintptr_t)s % 64 || s->magic != SCRATCH_MAGIC) {
+    if (!validScratch(s)) {
         return HS_INVALID;
     }
     if (markInUse(s)) {
@@ -1526,7 +1594,7 @@ hs_error_t hs_b200_corpus_upload(const char *data, const unsigned long long *off
     u64 total = 0, payload = 0;
     bool direct = false;
     u32 uniPitch = 0, uniLen = 0;
-    layoutBlocks(nullptr, offsets, lengths, nblocks, &packed, &total, &payload, &direct, &uniPitch, &uniLen);
+    layoutBlocks(offsets, lengths, nblocks, &packed, &total, &payload, &direct, &uniPitch, &uniLen);
     hs_error_t r = reserveCorpus(c, total, nblocks);
     if (r != HS_SUCCESS) {
         freeCorpus(c);
@@ -1641,21 +1709,11 @@ size_t hs_b200_corpus_bytes(const hs_b200_corpus_t *corpus) {
 /* ---- device-resident scan --------------------------------------------------------- */
 
 static hs_error_t checkScanArgs(const hs_database_t *db, hs_scratch_t *scratch) {
-    hs_error_t err = validDb(db);
-    if (err != HS_SUCCESS) {
-        return err;
+    const hs_error_t r = checkDb(db, MODE_BLOCK);
+    if (r != HS_SUCCESS) {
+        return r;
     }
-    const RoseEngine *rose = dbRose(db);
-    if ((uintptr_t)rose % 16) {
-        return HS_INVALID;
-    }
-    if (rose->mode != MODE_BLOCK) {
-        return HS_DB_MODE_ERROR;
-    }
-    if ((uintptr_t)scratch % 64 || scratch->magic != SCRATCH_MAGIC) {
-        return HS_INVALID;
-    }
-    return HS_SUCCESS;
+    return validScratch(scratch) ? HS_SUCCESS : HS_INVALID;
 }
 
 hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corpus_t *corpus,
@@ -1678,8 +1736,6 @@ hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corp
         if (corpus->bytes == 0 || corpus->nblocks == 0) {
             scratch->h_counters[CTR_MATCHES] = 0;
             scratch->h_counters[CTR_ERROR] = 0;
-            scratch->lastImage = im;
-            scratch->lastCorpus = corpus;
             scratch->pending = false;
             scratch->lastCount = 0;
         } else {
@@ -1692,7 +1748,7 @@ hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corp
 
 hs_error_t hs_b200_scan_corpus_finish(hs_scratch_t *scratch, unsigned long long *nrecords,
                                       const void **d_records) {
-    if (!scratch || (uintptr_t)scratch % 64 || scratch->magic != SCRATCH_MAGIC) {
+    if (!validScratch(scratch)) {
         return HS_INVALID;
     }
     DeviceGuard guard(scratch->device);
@@ -1712,11 +1768,7 @@ hs_error_t hs_b200_scan_corpus_finish(hs_scratch_t *scratch, unsigned long long 
     }
     if (count > scratch->outCap) {
         /* ring overflowed: grow so that a re-run succeeds */
-        u64 want = (u64)count + count / 4 + 1024;
-        if (want > 0xfffffff0ull) {
-            want = 0xfffffff0ull;
-        }
-        hs_error_t r = growRing(scratch, (u32)want);
+        hs_error_t r = growRingFor(scratch, count);
         if (r != HS_SUCCESS) {
             return r;
         }
@@ -1781,7 +1833,7 @@ hs_error_t hs_b200_peer_buffer_close(void *d_ptr, int opened) {
 hs_error_t hs_b200_set_peer_exchange(hs_scratch_t *scratch, unsigned int nranks, unsigned int my_rank,
                                      void *const *peer_bases, size_t cap_per_rank,
                                      unsigned int block_base) {
-    if (!scratch || (uintptr_t)scratch % 64 || scratch->magic != SCRATCH_MAGIC || nranks > MAX_PEERS ||
+    if (!validScratch(scratch) || nranks > MAX_PEERS ||
         (nranks && (!peer_bases || my_rank >= nranks || cap_per_rank == 0 || cap_per_rank > 0xfffffff0u))) {
         return HS_INVALID;
     }
@@ -1797,7 +1849,7 @@ hs_error_t hs_b200_set_peer_exchange(hs_scratch_t *scratch, unsigned int nranks,
 
 hs_error_t hs_b200_export_records_async(hs_scratch_t *scratch, void *d_dst, size_t cap,
                                         void *d_count, void *cuda_stream) {
-    if (!scratch || !d_dst || !d_count || (uintptr_t)scratch % 64 || scratch->magic != SCRATCH_MAGIC) {
+    if (!validScratch(scratch) || !d_dst || !d_count) {
         return HS_INVALID;
     }
     DeviceGuard guard(scratch->device);
@@ -1873,17 +1925,12 @@ hs_error_t hs_b200_fetch_matches(const hs_database_t *db, hs_scratch_t *scratch,
 hs_error_t hs_b200_nfa_scan_corpus(const void *nfa, size_t nfa_len, const hs_b200_corpus_t *corpus,
                                    hs_b200_match_t *out, size_t cap, unsigned long long *nmatches,
                                    float *kernel_ms) {
-    if (!nfa || nfa_len < sizeof(NFA) + 64 || !corpus || (cap && !out) || !nmatches) {
-        return HS_INVALID;
-    }
-    NFA hdr;
-    memcpy(&hdr, nfa, sizeof(hdr));
-    if (hdr.length > nfa_len) {
+    if (!corpus || (cap && !out) || !nmatches) {
         return HS_INVALID;
     }
     DfaParams p;
     {
-        const hs_error_t er = engineParams(nfa, nfa_len, &p);
+        const hs_error_t er = engineParams(nfa, nfa_len, &p); /* HS_INVALID for a short or damaged engine */
         if (er != HS_SUCCESS) {
             return er;
         }
@@ -1908,21 +1955,9 @@ hs_error_t hs_b200_nfa_scan_corpus(const void *nfa, size_t nfa_len, const hs_b20
         e = cudaMalloc(&d_out, (size_t)capDev * sizeof(DevMatch));
         if (e != cudaSuccess) break;
         e = cudaMemset(d_ctr, 0, CTR_COUNT * sizeof(u32));
-        p.corpus = corpus->d_data;
-        p.readableEnd = corpus->readableEnd;
-        p.blockOff = corpus->d_off;
-        p.blockLen = corpus->d_len;
-        p.nblocks = (u32)corpus->nblocks;
-        p.uniformPitch = corpus->uniformPitch;
-        p.uniformLen = corpus->uniformLen;
-        p.nfa = d_nfa;
-        p.out = d_out;
-        p.outCap = capDev;
-        p.counters = d_ctr;
         if (e == cudaSuccess) e = cudaEventRecord(ev0, 0);
-        if (e == cudaSuccess) e = launchDfa(p, smCount, maxSmem, 0);
+        if (e == cudaSuccess) e = launchEngine(p, d_nfa, corpus, d_out, capDev, d_ctr, smCount, maxSmem, 0);
         if (e == cudaSuccess) e = cudaEventRecord(ev1, 0);
-        g_launches++;
         u32 ctr[CTR_COUNT] = {0};
         if (e == cudaSuccess) e = cudaMemcpy(ctr, d_ctr, sizeof(ctr), cudaMemcpyDeviceToHost);
         if (e != cudaSuccess) break;
@@ -1969,10 +2004,6 @@ hs_error_t hs_b200_nfa_scan_corpus(const void *nfa, size_t nfa_len, const hs_b20
 
 /* Copy host blocks into the scratch's inline corpus and scan them, with the
  * host->device copy pipelined against the kernel in chunk_mb pieces. */
-static double nowMs() {
-    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
-}
-
 static hs_error_t scanHostBlocks(const DevImage *im, hs_scratch *s, const char *data,
                                  const unsigned long long *offsets, const unsigned *lengths,
                                  size_t nblocks, std::vector<DevMatch> *matches,
@@ -1980,29 +2011,23 @@ static hs_error_t scanHostBlocks(const DevImage *im, hs_scratch *s, const char *
     static const bool trace = getenv("HSB200_TRACE") != nullptr;
     DeviceGuard guard(s->device); /* every host-buffer scan (hs_scan, hs_b200_scan_blocks, streams) ends up here */
     const double t0 = nowMs();
-    double tLayout = 0, tEnq = 0, tWait = 0, tRec = 0;
     hs_b200_corpus *c = s->inlineCorpus;
     std::vector<u64> &packed = *s->tmpOff;
     u64 total = 0, payload = 0;
     bool direct = false;
     u32 uniPitch = 0, uniLen = 0;
-    layoutBlocks(s, offsets, lengths, nblocks, &packed, &total, &payload, &direct, &uniPitch, &uniLen);
+    layoutBlocks(offsets, lengths, nblocks, &packed, &total, &payload, &direct, &uniPitch, &uniLen);
     matches->clear();
     if (total == 0) {
         return HS_SUCCESS;
     }
-    tLayout = nowMs();
+    const double tLayout = nowMs();
     hs_error_t r = reserveCorpus(c, total, nblocks);
     if (r != HS_SUCCESS) {
         return r;
     }
     c->readableEnd = HSB_ROUNDUP(total, 16) + 16;
     r = setBlocks(c, packed.data(), lengths, nblocks, total, payload, s->copyStream, uniPitch, uniLen);
-    if (r != HS_SUCCESS) {
-        return r;
-    }
-    ScanPlan pl;
-    r = planScan(s, im, &pl);
     if (r != HS_SUCCESS) {
         return r;
     }
@@ -2013,125 +2038,94 @@ static hs_error_t scanHostBlocks(const DevImage *im, hs_scratch *s, const char *
         CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
         s->chunkEvents->push_back(ev);
     }
-    /* a second pass after the record ring grew; a third may be needed (the
-     * candidate list can overflow before the ring does) */
-    for (int attempt = 0; attempt < 3; attempt++) {
-        CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), s->stream));
-        CUDA_TRY(cudaEventRecord(s->evStart, s->stream));
-        /* zero the look-ahead bytes after the corpus */
-        CUDA_TRY(cudaMemsetAsync(c->d_data + total, 0, HSB_ROUNDUP(total, 16) + 32 - total,
-                                 s->copyStream));
-        u32 tDone = 0;
-        size_t blk = 0;
-        for (size_t ci = 0; ci < nchunks; ci++) {
-            const u64 from = ci * chunk, to = std::min<u64>(total, from + chunk);
-            if (attempt == 0) {
-                if (direct) {
-                    CUDA_TRY(cudaMemcpyAsync(c->d_data + from, data + offsets[0] + from, to - from,
-                                             cudaMemcpyHostToDevice, s->copyStream));
-                } else {
-                    /* unaligned host layout: pack this chunk's blocks (16-byte
-                     * aligned starts, zero gaps) into a pinned staging buffer and
-                     * send it as one copy; blocks that straddle the chunk edge go
-                     * whole with the chunk they start in.  Two buffers alternate. */
-                    const size_t b0 = blk;
-                    u64 end = from;
-                    while (blk < nblocks && packed[blk] < to) {
-                        end = std::max<u64>(end, packed[blk] + lengths[blk]);
-                        blk++;
-                    }
-                    if (blk > b0) {
-                        const u64 start = packed[b0];
-                        const size_t need = (size_t)(end - start);
-                        u8 *&stage = (ci & 1) ? s->h_stage2 : s->h_stage;
-                        size_t &cap = (ci & 1) ? s->h_stage2Cap : s->h_stageCap;
-                        cudaEvent_t ev = (ci & 1) ? s->evStage2 : s->evStage;
-                        CUDA_TRY(cudaEventSynchronize(ev)); /* previous use of this buffer has been sent */
-                        if (need > cap) {
-                            if (stage) cudaFreeHost(stage);
-                            stage = nullptr;
-                            cap = 0;
-                            CUDA_TRY(cudaMallocHost(&stage, need + need / 4 + 4096));
-                            cap = need + need / 4 + 4096;
-                        }
-                        memset(stage, 0, need);
-                        for (size_t k = b0; k < blk; k++) {
-                            memcpy(stage + (packed[k] - start), data + offsets[k], lengths[k]);
-                        }
-                        CUDA_TRY(cudaMemcpyAsync(c->d_data + start, stage, need, cudaMemcpyHostToDevice,
-                                                 s->copyStream));
-                        CUDA_TRY(cudaEventRecord(ev, s->copyStream));
-                    }
-                }
-                CUDA_TRY(cudaEventRecord((*s->chunkEvents)[ci], s->copyStream));
-                CUDA_TRY(cudaStreamWaitEvent(s->stream, (*s->chunkEvents)[ci], 0));
-            }
-            /* tiles wholly inside the copied prefix (plus look-ahead) */
-            u32 tEnd;
-            if (ci + 1 == nchunks) {
-                tEnd = (u32)((total + pl.tileBytes - 1) / pl.tileBytes);
-            } else {
-                u64 covered = direct ? to : (blk < nblocks ? packed[blk] : total);
-                covered = std::min(covered, to);
-                tEnd = covered > 16 ? (u32)((covered - 16) / pl.tileBytes) : 0;
-            }
-            r = launchRange(s, im, c, pl, tDone, tEnd, s->stream);
-            if (r != HS_SUCCESS) {
-                return r;
-            }
-            tDone = std::max(tDone, tEnd);
+    /* zero the look-ahead bytes after the corpus */
+    CUDA_TRY(cudaMemsetAsync(c->d_data + total, 0, HSB_ROUNDUP(total, 16) + 32 - total, s->copyStream));
+    size_t blk = 0; /* first block of the next chunk (packed layout) */
+    Upload up;
+    up.nchunks = nchunks;
+    up.chunk = [&](size_t ci, u64 *covered) -> hs_error_t {
+        const u64 from = ci * chunk, to = std::min<u64>(total, from + chunk);
+        /* packed layout: blocks that straddle the chunk edge go whole with the chunk they start in */
+        const size_t b0 = blk;
+        u64 end = from;
+        while (!direct && blk < nblocks && packed[blk] < to) {
+            end = std::max<u64>(end, packed[blk] + lengths[blk]);
+            blk++;
         }
-        CUDA_TRY(cudaEventRecord(s->evStop, s->stream));
-        CUDA_TRY(cudaMemcpyAsync(s->h_counters, s->d_counters, CTR_COUNT * sizeof(u32),
-                                 cudaMemcpyDeviceToHost, s->stream));
-        CUDA_TRY(cudaEventRecord(s->evDone, s->stream));
-        s->lastImage = im;
-        s->lastCorpus = c;
-        s->activeStream = s->stream;
-        s->pending = true;
-        u32 count = 0;
-        tEnq = nowMs();
-        r = finishScan(s, &count);
-        tWait = nowMs();
-        if (r != HS_SUCCESS) {
-            return r;
-        }
-        if (count <= s->outCap) {
-            matches->resize(count);
-            if (count) {
-                CUDA_TRY(cudaMemcpyAsync(matches->data(), s->d_out, (size_t)count * sizeof(DevMatch),
-                                         cudaMemcpyDeviceToHost, s->stream));
-                CUDA_TRY(cudaStreamSynchronize(s->stream));
+        *covered = std::min(direct ? to : (blk < nblocks ? packed[blk] : total), to);
+        if (direct) {
+            CUDA_TRY(cudaMemcpyAsync(c->d_data + from, data + offsets[0] + from, to - from,
+                                     cudaMemcpyHostToDevice, s->copyStream));
+        } else if (blk > b0) {
+            /* unaligned host layout: pack this chunk's blocks (16-byte aligned starts,
+             * zero gaps) into a pinned staging buffer and send it as one copy.  Two
+             * buffers alternate. */
+            const u64 start = packed[b0];
+            const size_t need = (size_t)(end - start);
+            u8 *&stage = (ci & 1) ? s->h_stage2 : s->h_stage;
+            size_t &cap = (ci & 1) ? s->h_stage2Cap : s->h_stageCap;
+            cudaEvent_t ev = (ci & 1) ? s->evStage2 : s->evStage;
+            CUDA_TRY(cudaEventSynchronize(ev)); /* previous use of this buffer has been sent */
+            if (need > cap) {
+                if (stage) cudaFreeHost(stage);
+                stage = nullptr;
+                cap = 0;
+                CUDA_TRY(cudaMallocHost(&stage, need + need / 4 + 4096));
+                cap = need + need / 4 + 4096;
             }
-            tRec = nowMs();
-            /* nobody will look at the order, and neither dedupe keys nor
-             * exhaustion keys exist: the raw count IS the delivered count */
-            const bool plain = countOnly && im->exhaustible.empty() && !im->hasDedupe && im->kind != FK_OUTFIX;
-            if (!plain) {
-                r = postprocessVec(im, matches);
-                if (r != HS_SUCCESS) {
-                    return r;
-                }
+            memset(stage, 0, need);
+            for (size_t k = b0; k < blk; k++) {
+                memcpy(stage + (packed[k] - start), data + offsets[k], lengths[k]);
             }
-            if (trace) {
-                fprintf(stderr, "[hs_b200 trace] host scan: layout %.3f ms, enqueue %.3f, wait %.3f, records %.3f, "
-                                "postprocess %.3f (total %.3f, %zu chunks)\n",
-                        tLayout - t0, tEnq - tLayout, tWait - tEnq, tRec - tWait, nowMs() - tRec,
-                        nowMs() - t0, nchunks);
-            }
-            return HS_SUCCESS;
+            CUDA_TRY(cudaMemcpyAsync(c->d_data + start, stage, need, cudaMemcpyHostToDevice, s->copyStream));
+            CUDA_TRY(cudaEventRecord(ev, s->copyStream));
         }
-        /* record ring overflowed: grow it and scan the resident corpus again */
-        u64 want = (u64)count + count / 4 + 1024;
-        if (want > 0xfffffff0ull) {
-            return HS_NOMEM;
+        CUDA_TRY(cudaEventRecord((*s->chunkEvents)[ci], s->copyStream));
+        CUDA_TRY(cudaStreamWaitEvent(s->stream, (*s->chunkEvents)[ci], 0));
+        return HS_SUCCESS;
+    };
+    /* nobody will look at the order, and neither dedupe keys nor
+     * exhaustion keys exist: the raw count IS the delivered count */
+    const bool plain = countOnly && im->exhaustible.empty() && !im->hasDedupe && im->kind != FK_OUTFIX;
+    ScanTimes tm;
+    r = scanRecords(s, im, c, &up, !plain, matches, &tm);
+    if (r == HS_SUCCESS && trace) {
+        fprintf(stderr, "[hs_b200 trace] host scan: layout %.3f ms, enqueue %.3f, wait %.3f, records %.3f, "
+                        "postprocess %.3f (total %.3f, %zu chunks)\n",
+                tLayout - t0, tm.enqueued - tLayout, tm.waited - tm.enqueued, tm.read - tm.waited,
+                nowMs() - tm.read, nowMs() - t0, nchunks);
+    }
+    return r;
+}
+
+/* hs_scan, hs_b200_scan_blocks and _collect: check the database and the scratch,
+ * mark the scratch in use, scan the blocks and hand the records to deliver() before
+ * the mark is released.  skipShort (hs_scan): a block shorter than any match is not
+ * scanned at all (src/runtime.c:346-350). */
+static hs_error_t blockScan(const hs_database_t *db, hs_scratch *s, const char *data,
+                            const unsigned long long *offsets, const unsigned *lengths, size_t nblocks,
+                            bool countOnly, bool skipShort,
+                            const std::function<hs_error_t(const std::vector<DevMatch> &)> &deliver) {
+    hs_error_t r = checkScanArgs(db, s);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    if (markInUse(s)) {
+        return HS_SCRATCH_IN_USE;
+    }
+    if (!(skipShort && dbRose(db)->minWidth > lengths[0])) {
+        const DevImage *im = nullptr;
+        std::vector<DevMatch> matches;
+        r = findImage(s, db, &im);
+        if (r == HS_SUCCESS) {
+            r = scanHostBlocks(im, s, data, offsets, lengths, nblocks, &matches, countOnly);
         }
-        r = growRing(s, (u32)want);
-        if (r != HS_SUCCESS) {
-            return r;
+        if (r == HS_SUCCESS) {
+            r = deliver(matches);
         }
     }
-    return HS_UNKNOWN_ERROR;
+    unmarkInUse(s);
+    return r;
 }
 
 hs_error_t hs_b200_scan_blocks(const hs_database_t *db, const char *data,
@@ -2142,41 +2136,28 @@ hs_error_t hs_b200_scan_blocks(const hs_database_t *db, const char *data,
     if (!scratch || (nblocks && (!data || !offsets || !lengths)) || nblocks > 0xfffffff0u) {
         return HS_INVALID;
     }
-    hs_error_t r = checkScanArgs(db, scratch);
-    if (r != HS_SUCCESS) {
-        return r;
-    }
-    if (markInUse(scratch)) {
-        return HS_SCRATCH_IN_USE;
-    }
-    const DevImage *im = nullptr;
-    r = findImage(scratch, db, &im);
-    std::vector<DevMatch> matches;
-    if (r == HS_SUCCESS) {
-        r = scanHostBlocks(im, scratch, data, offsets, lengths, nblocks, &matches, onEvent == nullptr);
-    }
-    unsigned long long delivered = 0;
-    if (r == HS_SUCCESS) {
-        if (!onEvent) {
-            delivered = matches.size();
-        } else {
-            u32 stopped = 0xffffffffu;
-            for (const DevMatch &m : matches) {
-                if (m.block == stopped) {
-                    continue;
-                }
-                delivered++;
-                if (onEvent(m.block, m.id, 0, m.to, 0, context)) {
-                    stopped = m.block;
-                }
-            }
-        }
-    }
-    if (nmatches) {
-        *nmatches = delivered;
-    }
-    unmarkInUse(scratch);
-    return r;
+    return blockScan(db, scratch, data, offsets, lengths, nblocks, onEvent == nullptr, false,
+                     [&](const std::vector<DevMatch> &matches) {
+                         unsigned long long delivered = 0;
+                         if (!onEvent) {
+                             delivered = matches.size();
+                         } else {
+                             u32 stopped = 0xffffffffu;
+                             for (const DevMatch &m : matches) {
+                                 if (m.block == stopped) {
+                                     continue;
+                                 }
+                                 delivered++;
+                                 if (onEvent(m.block, m.id, 0, m.to, 0, context)) {
+                                     stopped = m.block;
+                                 }
+                             }
+                         }
+                         if (nmatches) {
+                             *nmatches = delivered;
+                         }
+                         return HS_SUCCESS;
+                     });
 }
 
 hs_error_t hs_b200_scan_blocks_collect(const hs_database_t *db, const char *data,
@@ -2186,31 +2167,15 @@ hs_error_t hs_b200_scan_blocks_collect(const hs_database_t *db, const char *data
     if (!scratch || (nblocks && (!data || !offsets || !lengths)) || nblocks > 0xfffffff0u || (cap && !out)) {
         return HS_INVALID;
     }
-    hs_error_t r = checkScanArgs(db, scratch);
-    if (r != HS_SUCCESS) {
-        return r;
-    }
-    if (markInUse(scratch)) {
-        return HS_SCRATCH_IN_USE;
-    }
-    const DevImage *im = nullptr;
-    r = findImage(scratch, db, &im);
-    std::vector<DevMatch> matches;
-    if (r == HS_SUCCESS) {
-        r = scanHostBlocks(im, scratch, data, offsets, lengths, nblocks, &matches, false);
-    }
-    if (r == HS_SUCCESS) {
-        if (nmatches) {
-            *nmatches = matches.size();
-        }
-        static_assert(sizeof(DevMatch) == sizeof(hs_b200_match_t), "record layout");
-        memcpy(out, matches.data(), std::min(cap, matches.size()) * sizeof(DevMatch));
-        if (matches.size() > cap) {
-            r = HS_INSUFFICIENT_SPACE;
-        }
-    }
-    unmarkInUse(scratch);
-    return r;
+    return blockScan(db, scratch, data, offsets, lengths, nblocks, false, false,
+                     [&](const std::vector<DevMatch> &matches) {
+                         if (nmatches) {
+                             *nmatches = matches.size();
+                         }
+                         static_assert(sizeof(DevMatch) == sizeof(hs_b200_match_t), "record layout");
+                         memcpy(out, matches.data(), std::min(cap, matches.size()) * sizeof(DevMatch));
+                         return matches.size() > cap ? HS_INSUFFICIENT_SPACE : HS_SUCCESS;
+                     });
 }
 
 hs_error_t hs_scan(const hs_database_t *db, const char *data, unsigned int length,
@@ -2220,35 +2185,15 @@ hs_error_t hs_scan(const hs_database_t *db, const char *data, unsigned int lengt
     if (!scratch || !data) {
         return HS_INVALID;
     }
-    hs_error_t r = checkScanArgs(db, scratch);
-    if (r != HS_SUCCESS) {
-        return r;
-    }
-    if (markInUse(scratch)) {
-        return HS_SCRATCH_IN_USE;
-    }
-    const RoseEngine *rose = dbRose(db);
-    if (rose->minWidth > length) { /* src/runtime.c:346-350 */
-        unmarkInUse(scratch);
-        return HS_SUCCESS;
-    }
-    const DevImage *im = nullptr;
-    r = findImage(scratch, db, &im);
-    std::vector<DevMatch> matches;
-    if (r == HS_SUCCESS) {
-        const unsigned long long off = 0;
-        r = scanHostBlocks(im, scratch, data, &off, &length, 1, &matches);
-    }
-    if (r == HS_SUCCESS && onEvent) {
+    const unsigned long long off = 0;
+    return blockScan(db, scratch, data, &off, &length, 1, false, true, [&](const std::vector<DevMatch> &matches) {
         for (const DevMatch &m : matches) {
-            if (onEvent(m.id, 0, m.to, 0, context)) {
-                r = HS_SCAN_TERMINATED; /* src/report.h:324-328 */
-                break;
+            if (onEvent && onEvent(m.id, 0, m.to, 0, context)) {
+                return HS_SCAN_TERMINATED; /* src/report.h:324-328 */
             }
         }
-    }
-    unmarkInUse(scratch);
-    return r;
+        return HS_SUCCESS;
+    });
 }
 
 /* ---- streaming mode (src/runtime.c:542-977, pure-literal databases) ------------------
@@ -2288,17 +2233,11 @@ hs_error_t hs_open_stream(const hs_database_t *db, unsigned int flags, hs_stream
         return HS_INVALID;
     }
     *stream = nullptr;
-    hs_error_t err = validDb(db);
+    hs_error_t err = checkDb(db, MODE_STREAM);
     if (err != HS_SUCCESS) {
         return err;
     }
     const RoseEngine *rose = dbRose(db);
-    if ((uintptr_t)rose % 16) {
-        return HS_INVALID;
-    }
-    if (rose->mode != MODE_STREAM) {
-        return HS_DB_MODE_ERROR;
-    }
     if (rose->runtimeImpl != RUNTIME_PURE_LITERAL || rose->historyRequired > sizeof(((hs_stream *)0)->hist)) {
         return HS_ARCH_ERROR;
     }
@@ -2376,7 +2315,7 @@ static hs_error_t streamWrite(hs_stream *st, const char *data, unsigned int leng
 hs_error_t hs_scan_stream(hs_stream_t *st, const char *data, unsigned int length, unsigned int flags,
                           hs_scratch_t *scratch, match_event_handler onEvent, void *context) {
     (void)flags;
-    if (!validStream(st) || !scratch || !data || (uintptr_t)scratch % 64 || scratch->magic != SCRATCH_MAGIC) {
+    if (!validStream(st) || !data || !validScratch(scratch)) {
         return HS_INVALID;
     }
     if (markInUse(scratch)) {
@@ -2396,20 +2335,14 @@ hs_error_t hs_scan_vector(const hs_database_t *db, const char *const *data, cons
     if (!scratch || !data || !length) {
         return HS_INVALID;
     }
-    hs_error_t err = validDb(db);
+    hs_error_t err = checkDb(db, MODE_VECTORED);
     if (err != HS_SUCCESS) {
         return err;
     }
+    if (!validScratch(scratch)) {
+        return HS_INVALID;
+    }
     const RoseEngine *rose = dbRose(db);
-    if ((uintptr_t)rose % 16) {
-        return HS_INVALID;
-    }
-    if (rose->mode != MODE_VECTORED) {
-        return HS_DB_MODE_ERROR;
-    }
-    if ((uintptr_t)scratch % 64 || scratch->magic != SCRATCH_MAGIC) {
-        return HS_INVALID;
-    }
     if (rose->runtimeImpl != RUNTIME_PURE_LITERAL || rose->historyRequired > sizeof(((hs_stream *)0)->hist)) {
         return HS_ARCH_ERROR;
     }
@@ -2600,7 +2533,7 @@ hs_error_t hs_reset_and_expand_stream(hs_stream_t *to_stream, const char *buf, s
     if (!validStream(to_stream) || !buf) {
         return HS_INVALID;
     }
-    if (onEvent && (!scratch || (uintptr_t)scratch % 64 || scratch->magic != SCRATCH_MAGIC)) {
+    if (onEvent && !validScratch(scratch)) {
         return HS_INVALID; /* pure-literal databases have no end-of-data reports to deliver */
     }
     /* expand into a copy first: a bad buffer must leave the stream as it was */
@@ -2633,8 +2566,7 @@ struct hs_b200_stream_set {
     u8 *d_hist;     /* 8 bytes per stream */
     u64 *d_offset;
     u32 *d_len;     /* per-write lengths when they differ */
-    hs_b200_corpus corpus; /* pitched staging, reused */
-    u32 pitchCap;
+    hs_b200_corpus corpus; /* pitched staging, reused; its block lengths and stream state are the above */
 };
 
 hs_error_t hs_b200_streams_open(const hs_database_t *db, size_t nstreams, int device,
@@ -2643,14 +2575,11 @@ hs_error_t hs_b200_streams_open(const hs_database_t *db, size_t nstreams, int de
         return HS_INVALID;
     }
     *set = nullptr;
-    hs_error_t err = validDb(db);
+    hs_error_t err = checkDb(db, MODE_STREAM);
     if (err != HS_SUCCESS) {
         return err;
     }
     const RoseEngine *rose = dbRose(db);
-    if (rose->mode != MODE_STREAM) {
-        return HS_DB_MODE_ERROR;
-    }
     if (rose->runtimeImpl != RUNTIME_PURE_LITERAL || rose->historyRequired > 7 || rose->ekeyCount) {
         /* HS_FLAG_SINGLEMATCH state per stream is kept only by hs_scan_stream */
         return HS_ARCH_ERROR;
@@ -2669,7 +2598,6 @@ hs_error_t hs_b200_streams_open(const hs_database_t *db, size_t nstreams, int de
     s->d_hist = nullptr;
     s->d_offset = nullptr;
     s->d_len = nullptr;
-    s->pitchCap = 0;
     cudaError_t e = cudaMalloc(&s->d_hist, nstreams * 8);
     if (e == cudaSuccess) e = cudaMalloc(&s->d_offset, nstreams * 8);
     if (e == cudaSuccess) e = cudaMalloc(&s->d_len, nstreams * 4);
@@ -2679,6 +2607,10 @@ hs_error_t hs_b200_streams_open(const hs_database_t *db, size_t nstreams, int de
         hs_b200_streams_close(s);
         return e == cudaErrorMemoryAllocation ? HS_NOMEM : HS_UNKNOWN_ERROR;
     }
+    s->corpus.device = device;
+    s->corpus.d_len = s->d_len;
+    s->corpus.streamHist = s->d_hist;
+    s->corpus.streamOffset = s->d_offset;
     *set = s;
     return HS_SUCCESS;
 }
@@ -2698,122 +2630,104 @@ hs_error_t hs_b200_streams_close(hs_b200_stream_set_t *s) {
 
 size_t hs_b200_streams_state_bytes(const hs_b200_stream_set_t *s) { return s ? s->nstreams * 16 : 0; }
 
+/* Copy one write per stream into the pitched corpus and drop each stream's
+ * look-behind in front of it, scan the corpus, and roll history and offsets
+ * forward once the scan has succeeded. */
 static hs_error_t streamsScanImpl(hs_b200_stream_set_t *set, const char *data,
                                   const unsigned long long *offsets, const unsigned int *lengths,
-                                  hs_scratch_t *scratch, std::vector<DevMatch> &matches) {
-    hs_scratch *s = scratch;
+                                  hs_scratch *s, std::vector<DevMatch> *matches) {
     const size_t n = set->nstreams;
-    hs_error_t r = HS_SUCCESS;
     if (s->device != set->device) {
         return HS_INVALID; /* the set's state and the scratch's ring must share a device */
     }
     DeviceGuard guard(set->device);
-    do {
-        const DevImage *im = nullptr;
-        r = findImage(s, set->db, &im);
-        if (r != HS_SUCCESS) break;
-        /* write lengths: uniform (config 4) or per stream */
-        u32 maxLen = 0, uni = lengths[0];
-        bool contiguous = true;
+    const DevImage *im = nullptr;
+    hs_error_t r = findImage(s, set->db, &im);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    /* write lengths: uniform (config 4) or per stream */
+    u32 maxLen = 0, uni = lengths[0];
+    bool contiguous = true;
+    for (size_t i = 0; i < n; i++) {
+        maxLen = std::max(maxLen, lengths[i]);
+        if (lengths[i] != uni) uni = 0;
+        if (offsets[i] != offsets[0] + (u64)i * lengths[0]) contiguous = false;
+    }
+    if (maxLen == 0) {
+        return HS_SUCCESS;
+    }
+    const u32 pitch = 16 + (u32)HSB_ROUNDUP((u64)maxLen, 16);
+    hs_b200_corpus *c = &set->corpus;
+    const u64 total = (u64)n * pitch;
+    r = reserveCorpus(c, total, 0);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    cudaStream_t st = s->stream;
+    cudaError_t e;
+    if (uni && contiguous) {
+        e = cudaMemcpy2DAsync(c->d_data + 16, pitch, data + offsets[0], uni, uni, n,
+                              cudaMemcpyHostToDevice, st);
+    } else {
+        /* ragged writes: pack on the host, one copy */
+        std::vector<u8> pack((size_t)total, 0);
         for (size_t i = 0; i < n; i++) {
-            maxLen = std::max(maxLen, lengths[i]);
-            if (lengths[i] != uni) uni = 0;
-            if (offsets[i] != offsets[0] + (u64)i * lengths[0]) contiguous = false;
+            memcpy(pack.data() + i * pitch + 16, data + offsets[i], lengths[i]);
         }
-        if (maxLen == 0) break;
-        const u32 pitch = 16 + (u32)HSB_ROUNDUP((u64)maxLen, 16);
-        hs_b200_corpus *c = &set->corpus;
-        const u64 total = (u64)n * pitch;
-        c->device = set->device;
-        r = reserveCorpus(c, total, 0);
-        if (r != HS_SUCCESS) break;
-        cudaStream_t st = s->stream;
-        cudaError_t e;
-        if (uni && contiguous) {
-            e = cudaMemcpy2DAsync(c->d_data + 16, pitch, data + offsets[0], uni, uni, n,
-                                  cudaMemcpyHostToDevice, st);
-        } else {
-            /* ragged writes: pack on the host, one copy */
-            std::vector<u8> pack((size_t)total, 0);
-            for (size_t i = 0; i < n; i++) {
-                memcpy(pack.data() + i * pitch + 16, data + offsets[i], lengths[i]);
-            }
-            e = cudaMemcpyAsync(c->d_data, pack.data(), total, cudaMemcpyHostToDevice, st);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(st); /* `pack` dies at scope end */
-            if (e == cudaSuccess && !uni) {
-                e = cudaMemcpyAsync(set->d_len, lengths, n * 4, cudaMemcpyHostToDevice, st);
-                if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-            }
+        e = cudaMemcpyAsync(c->d_data, pack.data(), total, cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st); /* `pack` dies at scope end */
+        if (e == cudaSuccess && !uni) {
+            e = cudaMemcpyAsync(set->d_len, lengths, n * 4, cudaMemcpyHostToDevice, st);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
         }
-        if (e == cudaSuccess) {
-            e = cudaMemsetAsync(c->d_data + total, 0, 48, st);
-        }
-        if (e == cudaSuccess) e = launchStreamAssemble(c->d_data, set->d_hist, (u32)n, pitch, st);
-        if (e != cudaSuccess) { r = HS_UNKNOWN_ERROR; break; }
-        g_launches++;
-        c->nblocks = n;
-        c->bytes = total;
-        c->readableEnd = HSB_ROUNDUP(total, 16) + 16;
-        c->payload = 0;
-        c->uniformPitch = 0;
-        c->uniformLen = uni;
-        c->d_len = set->d_len;
-        ScanPlan pl;
-        r = planScan(s, im, &pl);
-        if (r != HS_SUCCESS) break;
-        for (int attempt = 0; attempt < 2 && r == HS_SUCCESS; attempt++) {
-            ScanParams p;
-            fillParams(s, im, c, pl, &p);
-            p.streamPitch = pitch;
-            p.streamHist = set->d_hist;
-            p.streamOffset = set->d_offset;
-            p.tileFirst = 0;
-            p.ntiles = (u32)((total + pl.tileBytes - 1) / pl.tileBytes);
-            LaunchCfg cfg = pl.cfg;
-            cfg.grid = (int)std::min<u32>((u32)cfg.grid, (p.ntiles + (u32)cfg.warps - 1) / (u32)cfg.warps);
-            e = cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), st);
-            if (e == cudaSuccess) e = cudaEventRecord(s->evStart, st);
-            if (e == cudaSuccess) e = launchScan(cfg, p, st);
-            if (e == cudaSuccess) {
-                e = launchConfirm(cfg, p, st); /* candidate list -> records (counters were just cleared) */
-                g_launches++;
-            }
-            if (e == cudaSuccess) e = cudaEventRecord(s->evStop, st);
-            if (e == cudaSuccess) {
-                e = cudaMemcpyAsync(s->h_counters, s->d_counters, CTR_COUNT * sizeof(u32),
-                                    cudaMemcpyDeviceToHost, st);
-            }
-            if (e == cudaSuccess) e = cudaEventRecord(s->evDone, st);
-            if (e != cudaSuccess) { r = HS_UNKNOWN_ERROR; break; }
-            g_launches++;
-            s->activeStream = st;
-            s->pending = true;
-            u32 count = 0;
-            r = finishScan(s, &count);
-            if (r != HS_SUCCESS) break;
-            if (count <= s->outCap) {
-                matches.resize(count);
-                if (count) {
-                    e = cudaMemcpyAsync(matches.data(), s->d_out, (size_t)count * sizeof(DevMatch),
-                                        cudaMemcpyDeviceToHost, st);
-                    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-                    if (e != cudaSuccess) { r = HS_UNKNOWN_ERROR; break; }
-                }
-                matches.resize(postprocess(im, matches.data(), count));
-                break;
-            }
-            u64 want = (u64)count + count / 4 + 1024;
-            r = want > 0xfffffff0ull ? HS_NOMEM : growRing(s, (u32)want);
-        }
-        c->d_len = nullptr; /* borrowed */
-        if (r != HS_SUCCESS) break;
-        e = launchStreamAdvance(c->d_data, set->d_hist, set->d_offset, set->d_len, uni, (u32)n, pitch,
-                                set->histReq, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { r = HS_UNKNOWN_ERROR; break; }
-        g_launches++;
-    } while (0);
-    set->corpus.d_len = nullptr;
+    }
+    if (e == cudaSuccess) {
+        e = cudaMemsetAsync(c->d_data + total, 0, 48, st);
+    }
+    if (e == cudaSuccess) e = launchStreamAssemble(c->d_data, set->d_hist, (u32)n, pitch, st);
+    if (e != cudaSuccess) {
+        return HS_UNKNOWN_ERROR;
+    }
+    g_launches++;
+    c->nblocks = n;
+    c->bytes = total;
+    c->readableEnd = HSB_ROUNDUP(total, 16) + 16;
+    c->payload = 0;
+    c->uniformPitch = 0;
+    c->uniformLen = uni;
+    c->streamPitch = pitch;
+    r = scanRecords(s, im, c, nullptr, true, matches); /* a rescan reads the assembled corpus again */
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    e = launchStreamAdvance(c->d_data, set->d_hist, set->d_offset, set->d_len, uni, (u32)n, pitch,
+                            set->histReq, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) {
+        return HS_UNKNOWN_ERROR;
+    }
+    g_launches++;
+    return HS_SUCCESS;
+}
+
+/* hs_b200_streams_scan and _collect: check the arguments, mark the scratch in use,
+ * scan and hand the records to deliver() before the mark is released. */
+static hs_error_t streamSetScan(hs_b200_stream_set_t *set, const char *data, const unsigned long long *offsets,
+                                const unsigned int *lengths, hs_scratch_t *scratch,
+                                const std::function<hs_error_t(const std::vector<DevMatch> &)> &deliver) {
+    if (!set || !data || !offsets || !lengths || !validScratch(scratch)) {
+        return HS_INVALID;
+    }
+    if (markInUse(scratch)) {
+        return HS_SCRATCH_IN_USE;
+    }
+    std::vector<DevMatch> matches;
+    hs_error_t r = streamsScanImpl(set, data, offsets, lengths, scratch, &matches);
+    if (r == HS_SUCCESS) {
+        r = deliver(matches);
+    }
+    unmarkInUse(scratch);
     return r;
 }
 
@@ -2821,29 +2735,17 @@ hs_error_t hs_b200_streams_scan(hs_b200_stream_set_t *set, const char *data,
                                 const unsigned long long *offsets, const unsigned int *lengths,
                                 hs_scratch_t *scratch, hs_b200_block_event_handler onEvent,
                                 void *context, unsigned long long *nmatches) {
-    if (!set || !scratch || !data || !offsets || !lengths || (uintptr_t)scratch % 64 ||
-        scratch->magic != SCRATCH_MAGIC) {
-        return HS_INVALID;
-    }
-    if (markInUse(scratch)) {
-        return HS_SCRATCH_IN_USE;
-    }
-    std::vector<DevMatch> matches;
-    hs_error_t r = streamsScanImpl(set, data, offsets, lengths, scratch, matches);
-    unsigned long long delivered = 0;
-    if (r == HS_SUCCESS) {
-        delivered = matches.size();
+    return streamSetScan(set, data, offsets, lengths, scratch, [&](const std::vector<DevMatch> &matches) {
+        if (nmatches) {
+            *nmatches = matches.size();
+        }
         if (onEvent) {
             for (const DevMatch &m : matches) {
                 onEvent(m.block, m.id, 0, m.to, 0, context);
             }
         }
-    }
-    if (nmatches) {
-        *nmatches = delivered;
-    }
-    unmarkInUse(scratch);
-    return r;
+        return HS_SUCCESS;
+    });
 }
 
 hs_error_t hs_b200_streams_scan_collect(hs_b200_stream_set_t *set, const char *data,
@@ -2851,24 +2753,15 @@ hs_error_t hs_b200_streams_scan_collect(hs_b200_stream_set_t *set, const char *d
                                         const unsigned int *lengths, hs_scratch_t *scratch,
                                         hs_b200_match_t *out, size_t cap,
                                         unsigned long long *nmatches) {
-    if (!set || !scratch || !data || !offsets || !lengths || !nmatches || (cap && !out) ||
-        (uintptr_t)scratch % 64 || scratch->magic != SCRATCH_MAGIC) {
+    if (!nmatches || (cap && !out)) {
         return HS_INVALID;
     }
-    if (markInUse(scratch)) {
-        return HS_SCRATCH_IN_USE;
-    }
-    std::vector<DevMatch> matches;
-    hs_error_t r = streamsScanImpl(set, data, offsets, lengths, scratch, matches);
-    if (r == HS_SUCCESS) {
+    return streamSetScan(set, data, offsets, lengths, scratch, [&](const std::vector<DevMatch> &matches) {
         *nmatches = matches.size();
         memcpy(out, matches.data(), std::min(cap, matches.size()) * sizeof(DevMatch));
-        if (matches.size() > cap) {
-            r = HS_INSUFFICIENT_SPACE; /* the stream state HAS advanced; the first cap records are valid */
-        }
-    }
-    unmarkInUse(scratch);
-    return r;
+        /* the stream state HAS advanced; the first cap records are valid */
+        return matches.size() > cap ? HS_INSUFFICIENT_SPACE : HS_SUCCESS;
+    });
 }
 
 } /* extern "C" */

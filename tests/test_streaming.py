@@ -187,6 +187,46 @@ def test_stream_set_rejects_what_it_cannot_do(hs):
     with pytest.raises(hs.HsError) as e:
         hs.StreamSet(single, 4)
     assert e.value.code == hs.HS_ARCH_ERROR
+    # a database whose bytecode is not 16-byte aligned: its bytes moved 8 bytes off
+    sdb = hs.compile_lit_multi([b"abc"], mode=hs.HS_MODE_STREAM)
+    L = hs.lib()
+    size = C.c_size_t()
+    assert L.hs_database_size(sdb.ptr, C.byref(size)) == 0
+    raw = C.create_string_buffer(size.value + 128)
+    base = (C.addressof(raw) + 63) // 64 * 64 + 8
+    C.memmove(base, sdb.ptr, size.value)
+    p = C.c_void_p()
+    assert L.hs_b200_streams_open(C.c_void_p(base), 4, 0, C.byref(p)) == hs.HS_INVALID
+
+
+@pytest.mark.gpu
+def test_stream_set_survives_ring_overflow(hs):
+    """A stream set whose record ring overflows on the first scan, and again on the
+    rescan (the candidate list fills before the ring does), still returns every
+    record and carries its history on: 16 streams of `abcd` repeated against one
+    literal under 64 ids, three rounds, a 16-record initial ring against the default."""
+    db = hs.compile_lit_multi([b"abcd"] * 64, ids=list(range(64)), mode=hs.HS_MODE_STREAM)
+    nstreams, wlen = 16, 256
+    data = np.frombuffer(b"abcd" * (nstreams * wlen // 4), dtype=np.uint8).copy()
+    off = np.arange(nstreams, dtype=np.uint64) * wlen
+    ln = np.full(nstreams, wlen, dtype=np.uint32)
+
+    def rounds(ring):
+        hs.set_runtime_option("initial_ring", ring)     # read when the scratch is allocated
+        try:
+            scratch = hs.Scratch(db)
+        finally:
+            hs.set_runtime_option("initial_ring", 1 << 20)
+        sset = hs.StreamSet(db, nstreams)
+        got = [sset.scan(data, off, ln, scratch) for _ in range(3)]
+        sset.close()
+        return got
+
+    want = rounds(1 << 20)
+    got = rounds(16)
+    for w, g in zip(want, got):
+        assert w.size == nstreams * (wlen // 4) * 64
+        assert np.array_equal(g, w)
 
 
 @pytest.mark.gpu
