@@ -1181,12 +1181,17 @@ struct ScanTimes {
  * raw when !ordered.  When the record ring overflows, it grows and the corpus, resident
  * by then, is scanned again as one range.  A second pass finds the real record count;
  * a third may be needed, because the candidate list can overflow before the ring does.
- * A third overflow is an error. */
+ * A third overflow is an error.  A first pass that uploads the corpus in several chunks
+ * runs one range per chunk, and each range reports a candidate-list overflow with its own
+ * candidate count only, which is too small to size the ring for one range over the whole
+ * corpus.  So that pass does not count: the rescans then run exactly as for a corpus
+ * that was resident from the start. */
 hs_error_t scanRecords(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c, const Upload *up,
                        bool ordered, std::vector<DevMatch> *matches, ScanTimes *times = nullptr) {
     ScanTimes unused;
     ScanTimes &t = times ? *times : unused;
-    for (int attempt = 0; attempt < 3; attempt++) {
+    const int passes = up && up->nchunks > 1 ? 4 : 3;
+    for (int attempt = 0; attempt < passes; attempt++) {
         hs_error_t r = enqueueScan(s, im, c, s->stream, attempt == 0 ? up : nullptr);
         if (r != HS_SUCCESS) {
             return r;
