@@ -34,7 +34,10 @@ HS_FLAG_MULTILINE = 4
 HS_FLAG_SINGLEMATCH = 8
 HS_FLAG_ALLOWEMPTY = 16
 HS_FLAG_UTF8 = 32
+HS_FLAG_PREFILTER = 128
 HS_FLAG_SOM_LEFTMOST = 256
+HS_FLAG_COMBINATION = 512
+HS_FLAG_QUIET = 1024
 HS_MODE_BLOCK = 1
 HS_MODE_STREAM = 2
 HS_MODE_VECTORED = 4
@@ -139,6 +142,7 @@ def lib():
         L.hs_b200_peer_buffer_read.argtypes = [vp, vp, C.c_size_t]
         L.hs_b200_set_peer_exchange.argtypes = [vp, C.c_uint, C.c_uint, C.POINTER(vp), C.c_size_t, C.c_uint]
         L.hs_b200_postprocess_matches.argtypes = [vp, vp, C.c_size_t, u64p]
+        L.hs_b200_postprocess_blocks.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t, u64p]
         L.hs_b200_fetch_matches.argtypes = [vp, vp, vp, C.c_size_t, u64p]
         L.hs_b200_db_info.argtypes = [vp, C.POINTER(DbInfo)]
         L.hs_b200_set_build_option.argtypes = [cp, C.c_int]
@@ -462,6 +466,24 @@ def postprocess_matches(db, recs):
     n = C.c_ulonglong()
     _check(lib().hs_b200_postprocess_matches(db.ptr, recs.ctypes.data, recs.size, C.byref(n)))
     return recs[: int(n.value)]
+
+
+def postprocess_blocks(db, recs, lengths):
+    """Host-side report rules over the raw records of blocks with the given lengths, for any
+    database: with logical combinations (HS_FLAG_COMBINATION) the raw records hold logical-key
+    records (bit 63 of `to`), which become the combination reports.  No GPU needed."""
+    recs = np.ascontiguousarray(recs, dtype=MATCH_DTYPE)
+    ln = np.ascontiguousarray(lengths, dtype=np.uint32)
+    cap = recs.size + 1024
+    while True:
+        out = np.zeros(cap, dtype=MATCH_DTYPE)
+        n = C.c_ulonglong()
+        rc = lib().hs_b200_postprocess_blocks(db.ptr, recs.ctypes.data, recs.size, ln.ctypes.data, ln.size,
+                                              out.ctypes.data, cap, C.byref(n))
+        if rc != HS_INSUFFICIENT_SPACE:
+            _check(rc, "hs_b200_postprocess_blocks")
+            return out[: int(n.value)]
+        cap = int(n.value)
 
 
 def launch_count():

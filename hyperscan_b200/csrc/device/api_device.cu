@@ -116,6 +116,7 @@ struct DevImage {
     u32 minWidth = 0;
     bool hasDedupe = false;              /* RoseEngine.dkeyCount != 0 */
     mutable std::unordered_set<u32> exhaustible; /* report ids under HS_FLAG_SINGLEMATCH (FK_OUTFIX: found with the programs) */
+    mutable Combinations comb;           /* logical combinations (FK_OUTFIX: lkeyReport found with the programs) */
     size_t deviceBytes = 0;
 };
 
@@ -483,6 +484,9 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
     im->groups = r->initialGroups & r->floating_group_mask;
     im->minWidth = r->minWidth;
     im->hasDedupe = r->dkeyCount != 0;
+    if (r->ckeyCount) {
+        loadCombinations(r, &im->comb);
+    }
     if (soleOutfix) {
         /* hs_scan -> soleOutfixBlockExec (src/runtime.c:245-280): ONE engine over the whole block,
          * its reports are report programs (roseReportAdaptor, src/rose/match.c:611-633).  The
@@ -616,18 +620,19 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
             }
             memcpy(&table[b * 4], &e, 4);
         }
-        programsOk = collectProgramReports(bc, h->length, n.id, &im->exhaustible);
+        programsOk = collectProgramReports(bc, h->length, n.id, &im->exhaustible, nullptr, &im->comb.lkeyReport);
     } else if (hw->type == HWLM_ENGINE_FDR) {
         FDR f;
         memcpy(&f, bc + engOff, sizeof(f));
         im->confirmKind = CK_FDR;
         im->confOff = engOff + f.confOffset;
         if (f.engineID == 0) {
-            programsOk = walkConfirm(bc, h->length, im->confOff, 8, &im->exhaustible, &tails);
+            programsOk = walkConfirm(bc, h->length, im->confOff, 8, &im->exhaustible, &tails, &im->comb.lkeyReport);
             pairStage(true);
         } else if (teddyIdValid(f.engineID)) {
             const u32 oct = teddyNumBuckets(f.engineID) / 8;
-            programsOk = walkConfirm(bc, h->length, im->confOff, 8 * oct, &im->exhaustible, &tails);
+            programsOk = walkConfirm(bc, h->length, im->confOff, 8 * oct, &im->exhaustible, &tails,
+                                     &im->comb.lkeyReport);
             if (oct == 2) {
                 /* fat Teddy (49..96 literals): the class-pair kernel with 8 bucket bits that
                  * carry buckets i and i + 8 (confirmKernel unfolds them) */
@@ -726,6 +731,7 @@ struct hs_b200_corpus {
     u32 streamPitch = 0;
     const u8 *streamHist = nullptr;
     const u64 *streamOffset = nullptr;
+    std::vector<u32> h_len;  /* block lengths, for the end-of-block evaluation of logical combinations */
 };
 
 /* ---- scratch ------------------------------------------------------------------ */
@@ -745,6 +751,7 @@ struct hs_scratch {
     u32 *d_counters;
     u32 *h_counters;         /* pinned */
     hs_b200_corpus *inlineCorpus; /* staging for hs_scan / hs_b200_scan_blocks */
+    const hs_b200_corpus *lastCorpus; /* of the last resident scan: its block lengths, for hs_b200_fetch_matches */
     u8 *h_stage, *h_stage2;  /* pinned pack buffers (unaligned host blocks), alternating */
     size_t h_stageCap, h_stage2Cap;
     cudaEvent_t evStage, evStage2;
@@ -1056,13 +1063,33 @@ size_t postprocess(const DevImage *im, DevMatch *m, size_t n) {
     return postprocessRecords(im->exhaustible, (MatchRec *)m, n);
 }
 
+/* Records of a database with logical combinations, in delivery order with the combination
+ * reports added (postprocessCombinations); lengths[i] is the length of block i. */
+void postprocessComb(const DevImage *im, std::vector<DevMatch> *v, const u32 *lengths, size_t nblocks) {
+    static_assert(sizeof(MatchRec) == sizeof(DevMatch), "record layout");
+    std::vector<MatchRec> recs(v->size());
+    memcpy(recs.data(), v->data(), v->size() * sizeof(DevMatch));
+    postprocessCombinations(im->comb, im->exhaustible, &recs, lengths, nblocks);
+    v->resize(recs.size());
+    memcpy(v->data(), recs.data(), recs.size() * sizeof(DevMatch));
+}
+
 /* Records of a scan, ordered and with the order-dependent report rules applied (see
  * postprocessRecords).  Single-outfix databases: the kernel's records carry report PROGRAM
  * offsets (and the padding of the lanes' reserved slots); each is replaced by the reports its
- * program raises -- roseReportAdaptor -> roseRunProgram (src/rose/match.c:611-633) -- first. */
-hs_error_t postprocessVec(const DevImage *im, std::vector<DevMatch> *v) {
+ * program raises -- roseReportAdaptor -> roseRunProgram (src/rose/match.c:611-633) -- first.
+ * Databases with logical combinations need the block lengths (lengths[0, nblocks)). */
+hs_error_t postprocessVec(const DevImage *im, std::vector<DevMatch> *v, const u32 *lengths = nullptr,
+                          size_t nblocks = 0) {
+    if (im->comb.any() && !lengths && nblocks) {
+        return HS_INVALID;
+    }
     if (im->kind != FK_OUTFIX) {
-        v->resize(postprocess(im, v->data(), v->size()));
+        if (im->comb.any()) {
+            postprocessComb(im, v, lengths, nblocks);
+        } else {
+            v->resize(postprocess(im, v->data(), v->size()));
+        }
         return HS_SUCCESS;
     }
     const u8 *bc = (const u8 *)dbRose((const hs_database_t *)(im->dbCopy.data() + im->dbCopyShift));
@@ -1076,7 +1103,7 @@ hs_error_t postprocessVec(const DevImage *im, std::vector<DevMatch> *v) {
         if (it == im->progReports.end()) {
             std::vector<ProgReport> reps;
             if (m.id % INSTR_ALIGN || m.id < sizeof(RoseEngine) || m.id >= im->length ||
-                !collectProgramReports(bc, im->length, m.id, &im->exhaustible, &reps)) {
+                !collectProgramReports(bc, im->length, m.id, &im->exhaustible, &reps, &im->comb.lkeyReport)) {
                 return HS_UNKNOWN_ERROR; /* a program with a state-carrying opcode (or a corrupt record) */
             }
             it = im->progReports.emplace(m.id, std::move(reps)).first;
@@ -1087,11 +1114,15 @@ hs_error_t postprocessVec(const DevImage *im, std::vector<DevMatch> *v) {
             }
             DevMatch o = m;
             o.id = rp.onmatch;
-            o.to = (u64)((long long)m.to + rp.offset_adjust);
+            o.to = (u64)((long long)m.to + rp.offset_adjust) | (rp.logical ? LKEY_RECORD : 0);
             outv.push_back(o);
         }
     }
-    outv.resize(postprocess(im, outv.data(), outv.size()));
+    if (im->comb.any()) {
+        postprocessComb(im, &outv, lengths, nblocks);
+    } else {
+        outv.resize(postprocess(im, outv.data(), outv.size()));
+    }
     v->swap(outv);
     return HS_SUCCESS;
 }
@@ -1187,7 +1218,8 @@ struct ScanTimes {
  * corpus.  So that pass does not count: the rescans then run exactly as for a corpus
  * that was resident from the start. */
 hs_error_t scanRecords(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c, const Upload *up,
-                       bool ordered, std::vector<DevMatch> *matches, ScanTimes *times = nullptr) {
+                       bool ordered, std::vector<DevMatch> *matches, ScanTimes *times = nullptr,
+                       const u32 *lengths = nullptr) {
     ScanTimes unused;
     ScanTimes &t = times ? *times : unused;
     const int passes = up && up->nchunks > 1 ? 4 : 3;
@@ -1217,7 +1249,7 @@ hs_error_t scanRecords(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
             CUDA_TRY(cudaStreamSynchronize(s->stream));
         }
         t.read = nowMs();
-        return ordered ? postprocessVec(im, matches) : HS_SUCCESS;
+        return ordered ? postprocessVec(im, matches, lengths, c->nblocks) : HS_SUCCESS;
     }
     return HS_UNKNOWN_ERROR;
 }
@@ -1557,6 +1589,7 @@ static hs_error_t setBlocks(hs_b200_corpus *c, const u64 *packed, const unsigned
     c->nblocks = nblocks;
     c->bytes = total;
     c->payload = payload;
+    c->h_len.assign(lengths, lengths + nblocks);
     if (uniPitch && uniLen) { /* layoutBlocks already proved uniformity: no tables */
         c->uniformPitch = uniPitch;
         c->uniformLen = uniLen;
@@ -1746,6 +1779,7 @@ hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corp
         } else {
             r = enqueueScan(scratch, im, corpus, st);
         }
+        scratch->lastCorpus = corpus;
     }
     unmarkInUse(scratch);
     return r;
@@ -1904,7 +1938,13 @@ hs_error_t hs_b200_fetch_matches(const hs_database_t *db, hs_scratch_t *scratch,
                                  cudaMemcpyDeviceToHost, scratch->copyStream));
         CUDA_TRY(cudaStreamSynchronize(scratch->copyStream));
     }
-    r = postprocessVec(im, &tmp);
+    if (im->comb.any()) {
+        /* the combinations are evaluated per block, over the blocks of the corpus last scanned */
+        const hs_b200_corpus *c = scratch->lastCorpus;
+        r = c ? postprocessVec(im, &tmp, c->h_len.data(), c->h_len.size()) : HS_INVALID;
+    } else {
+        r = postprocessVec(im, &tmp);
+    }
     if (r != HS_SUCCESS) {
         return r;
     }
@@ -2091,9 +2131,9 @@ static hs_error_t scanHostBlocks(const DevImage *im, hs_scratch *s, const char *
     };
     /* nobody will look at the order, and neither dedupe keys nor
      * exhaustion keys exist: the raw count IS the delivered count */
-    const bool plain = countOnly && im->exhaustible.empty() && !im->hasDedupe && im->kind != FK_OUTFIX;
+    const bool plain = countOnly && im->exhaustible.empty() && !im->hasDedupe && im->kind != FK_OUTFIX && !im->comb.any();
     ScanTimes tm;
-    r = scanRecords(s, im, c, &up, !plain, matches, &tm);
+    r = scanRecords(s, im, c, &up, !plain, matches, &tm, lengths);
     if (r == HS_SUCCESS && trace) {
         fprintf(stderr, "[hs_b200 trace] host scan: layout %.3f ms, enqueue %.3f, wait %.3f, records %.3f, "
                         "postprocess %.3f (total %.3f, %zu chunks)\n",

@@ -385,6 +385,20 @@ __device__ void runProgram(const ScanParams &p, const BlockRef &blk, u32 prog, u
         case OP_INCLUDED_JUMP: /* the child literal is confirmed on its own */
             NEXT(InstrIncludedJump);
             break;
+        case OP_SET_LOGICAL: {
+            /* a logical-key record (id = lkey, bit 63 of `to` set): the combinations are
+             * evaluated on the host when the records are ordered (postprocessCombinations) */
+            const InstrSetLogical in = loadInstr<InstrSetLogical>(pc);
+            emitMatch(p, in.lkey, blk.index, (blk.toBase + to + in.offset_adjust) | (1ull << 63));
+            NEXT(InstrSetLogical);
+            break;
+        }
+        case OP_SET_COMBINATION: /* follows from the lkey on the host */
+            NEXT(InstrSetCombination);
+            break;
+        case OP_FLUSH_COMBINATION:
+            NEXT(InstrFlushCombination);
+            break;
         default:
             atomicExch(p.counters + CTR_ERROR, (u32)ERR_BAD_OPCODE);
             return;

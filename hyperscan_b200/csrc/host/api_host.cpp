@@ -788,6 +788,46 @@ static std::vector<std::string> regexToLiterals(const char *re, unsigned flags, 
     return FiniteRegex(re, flags, idx).expand();
 }
 
+static hs_error_t exprInfo(const char *expression, unsigned flags, const hs_expr_ext_t *ext,
+                           hs_expr_info_t **info, hs_compile_error_t **error);
+
+/* What a combination may name (validateSubIDs, src/parser/logical_combination.cpp:116-159): the
+ * first expression with each named id is an ordinary one, without SOM or PREFILTER, whose matches
+ * arrive in order. */
+static void checkSubExpressions(const LogicalSet &logic, const char *const *expressions, const unsigned *flags,
+                                const unsigned *ids, unsigned elements) {
+    for (const auto &lk : logic.lkeyOf) {
+        unsigned i = 0;
+        while (i < elements && (ids ? ids[i] : 0) != lk.first) {
+            i++;
+        }
+        if (i == elements) {
+            throw CompileError{"Unknown sub-expression id.", -1};
+        }
+        if (logic.ckeyOf.count(lk.first)) {
+            throw CompileError{"Have combination of combination.", -1};
+        }
+        const unsigned f = flags ? flags[i] : 0;
+        if (f & HS_FLAG_SOM_LEFTMOST) {
+            throw CompileError{"Have SOM flag in sub-expression.", -1};
+        }
+        if (f & HS_FLAG_PREFILTER) {
+            throw CompileError{"Have PREFILTER flag in sub-expression.", -1};
+        }
+        hs_expr_info_t *info = nullptr;
+        hs_compile_error_t *err = nullptr;
+        if (exprInfo(expressions[i], f, nullptr, &info, &err) != HS_SUCCESS) {
+            hs_free_compile_error(err);
+            throw CompileError{"Run hs_expression_info() failed.", -1};
+        }
+        const bool unordered = info->unordered_matches;
+        g_misc_free(info);
+        if (unordered) {
+            throw CompileError{"Have unordered match in sub-expressions.", -1};
+        }
+    }
+}
+
 static hs_error_t compileCommon(const char *const *expressions,
                                 const unsigned *flags, const unsigned *ids,
                                 const hs_expr_ext_t *const *ext,
@@ -828,12 +868,51 @@ static hs_error_t compileCommon(const char *const *expressions,
         pats.reserve(elements);
         std::vector<RegexPattern> rpats; /* every expression, for the NFA route */
         bool needNfa = false;
+        LogicalSet logic; /* HS_FLAG_COMBINATION expressions */
         for (unsigned i = 0; i < elements; i++) {
             const unsigned f = flags ? flags[i] : 0;
             if (!expressions[i]) {
                 throw CompileError{"Invalid parameter: expression is NULL", (int)i};
             }
             const hs_expr_ext_t *xp = ext && ext[i] && ext[i]->flags != 0 ? ext[i] : nullptr;
+            if ((f & HS_FLAG_COMBINATION) && !litApi) {
+                /* src/compiler/compiler.cpp:286-322: a combination is no pattern of its own; a quiet one
+                 * is dropped unparsed */
+                if (f & ~(HS_FLAG_COMBINATION | HS_FLAG_QUIET | HS_FLAG_SINGLEMATCH)) {
+                    throw CompileError{"only HS_FLAG_QUIET and HS_FLAG_SINGLEMATCH are supported in combination "
+                                       "with HS_FLAG_COMBINATION.", (int)i};
+                }
+                if (f & HS_FLAG_QUIET) {
+                    continue;
+                }
+                if (mode & (HS_MODE_STREAM | HS_MODE_VECTORED)) {
+                    /* the stream state would have to carry the logical and combination multibits */
+                    throw CompileError{"Logical combinations (HS_FLAG_COMBINATION) are supported in block mode "
+                                       "only in this build.", (int)i};
+                }
+                u64 lo = 0, hi = MAX_OFFSET;
+                if (xp) {
+                    if (xp->flags & ~(HS_EXT_FLAG_MIN_OFFSET | HS_EXT_FLAG_MAX_OFFSET)) {
+                        throw CompileError{"only HS_EXT_FLAG_MIN_OFFSET and HS_EXT_FLAG_MAX_OFFSET extra flags are "
+                                           "supported in combination with HS_FLAG_COMBINATION.", (int)i};
+                    }
+                    if ((xp->flags & HS_EXT_FLAG_MIN_OFFSET) && (xp->flags & HS_EXT_FLAG_MAX_OFFSET) &&
+                        xp->min_offset > xp->max_offset) {
+                        throw CompileError{"In hs_expr_ext, min_offset must be less than or equal to max_offset.",
+                                           (int)i};
+                    }
+                    lo = (xp->flags & HS_EXT_FLAG_MIN_OFFSET) ? xp->min_offset : 0;
+                    hi = (xp->flags & HS_EXT_FLAG_MAX_OFFSET) ? xp->max_offset : MAX_OFFSET;
+                }
+                try {
+                    /* (the ekey is a placeholder until the route numbers the exhaustion keys) */
+                    logic.add(ids ? ids[i] : 0, expressions[i], (f & HS_FLAG_SINGLEMATCH) ? 0 : INVALID_EKEY, lo, hi);
+                } catch (CompileError &e) {
+                    e.index = (int)i;
+                    throw;
+                }
+                continue;
+            }
             if (xp) {
                 /* validation as src/compiler/compiler.cpp:80-110 */
                 if (litApi) {
@@ -883,11 +962,13 @@ static hs_error_t compileCommon(const char *const *expressions,
                 }
                 p.s.assign(expressions[i], lens[i]);
             } else {
-                if (f & (HS_FLAG_COMBINATION | HS_FLAG_QUIET)) {
-                    throw CompileError{"HS_FLAG_COMBINATION / HS_FLAG_QUIET need the regex "
-                                       "back end; this build compiles literal patterns only.",
-                                       (int)i};
+                if ((f & HS_FLAG_QUIET) && (f & HS_FLAG_SINGLEMATCH)) {
+                    /* the reference raises SET_EXHAUST for such a report, a state-carrying opcode the
+                     * device interpreter does not run */
+                    throw CompileError{"HS_FLAG_QUIET together with HS_FLAG_SINGLEMATCH is only supported on a "
+                                       "logical combination (HS_FLAG_COMBINATION) in this build.", (int)i};
                 }
+                p.quiet = (f & HS_FLAG_QUIET) != 0;
                 if (f & HS_FLAG_SOM_LEFTMOST) {
                     throw CompileError{"HS_FLAG_SOM_LEFTMOST is not supported by the H100 "
                                        "literal compiler yet.", (int)i};
@@ -943,6 +1024,10 @@ static hs_error_t compileCommon(const char *const *expressions,
             }
             pats.push_back(p);
         }
+        if (!logic.empty()) {
+            checkSubExpressions(logic, expressions, flags, ids, elements);
+            logic.renumber();
+        }
         CompileOpts opts;
         opts.pureLiteralApi = litApi;
         opts.streaming = (mode & (HS_MODE_STREAM | HS_MODE_VECTORED)) != 0; /* isStreaming || isVectored: src/hs.cpp, util/compile_context.h:47-48 */
@@ -966,7 +1051,8 @@ static hs_error_t compileCommon(const char *const *expressions,
         if (opts.hwlm.allowFatTeddy) {
             opts.platform &= ~PLATFORM_NOAVX2; /* 16-bucket Teddy needs AVX2 on CPUs */
         }
-        std::vector<u8> bc = needNfa ? buildRegexRose(rpats, opts) : buildLiteralRose(pats, opts, nullptr);
+        LogicalSet *ls = logic.empty() ? nullptr : &logic;
+        std::vector<u8> bc = needNfa ? buildRegexRose(rpats, opts, ls) : buildLiteralRose(pats, opts, nullptr, ls);
         hs_error_t aerr;
         hs_database_t *out = dbCreate(bc, opts.platform, &aerr);
         if (!out) {

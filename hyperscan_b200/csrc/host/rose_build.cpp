@@ -64,11 +64,55 @@ struct PatInfo {
     u32 ekey, dkey;
 };
 
-u32 blockSize(const PatInfo &pi) {
-    u32 sz = 0;
-    if (pi.p->s.size() > 8) {
-        sz += instrSize<InstrCheckLit>();
+/* Combination bookkeeping of a report block (makeReport, src/rose/rose_build_program.cpp:568-626): when
+ * the database has combinations, FLUSH_COMBINATION before the report; when the report's id is a
+ * sub-expression of one, SET_LOGICAL and one SET_COMBINATION per combination that names it after it. */
+u32 flushSize(const LogicalSet *ls) { return ls && !ls->empty() ? instrSize<InstrFlushCombination>() : 0; }
+
+u32 logicalSize(const LogicalSet *ls, u32 report) {
+    const u32 lk = ls ? ls->lkey(report) : INVALID_LKEY;
+    if (lk == INVALID_LKEY) {
+        return 0;
     }
+    return instrSize<InstrSetLogical>() + (u32)ls->ckeysOfLkey.at(lk).size() * instrSize<InstrSetCombination>();
+}
+
+u32 writeFlush(Blob &blob, u32 pc, const LogicalSet *ls) {
+    if (flushSize(ls)) {
+        InstrFlushCombination f;
+        f.code = OP_FLUSH_COMBINATION;
+        memcpy(blob.at(pc), &f, sizeof(f));
+        pc += instrSize<InstrFlushCombination>();
+    }
+    return pc;
+}
+
+u32 writeLogical(Blob &blob, u32 pc, const LogicalSet *ls, u32 report, s32 adjust) {
+    const u32 lk = ls ? ls->lkey(report) : INVALID_LKEY;
+    if (lk == INVALID_LKEY) {
+        return pc;
+    }
+    InstrSetLogical sl;
+    memset(&sl, 0, sizeof(sl));
+    sl.code = OP_SET_LOGICAL;
+    sl.lkey = lk;
+    sl.offset_adjust = adjust;
+    memcpy(blob.at(pc), &sl, sizeof(sl));
+    pc += instrSize<InstrSetLogical>();
+    for (u32 ck : ls->ckeysOfLkey.at(lk)) {
+        InstrSetCombination sc;
+        memset(&sc, 0, sizeof(sc));
+        sc.code = OP_SET_COMBINATION;
+        sc.ckey = ck;
+        memcpy(blob.at(pc), &sc, sizeof(sc));
+        pc += instrSize<InstrSetCombination>();
+    }
+    return pc;
+}
+
+/* the report block of one pattern, without its literal check */
+u32 reportSize(const PatInfo &pi, const LogicalSet *ls) {
+    u32 sz = flushSize(ls) + logicalSize(ls, pi.p->report);
     if (pi.ekey != INVALID_EKEY) {
         sz += instrSize<InstrCheckExhausted>();
         if (pi.dkey != INVALID_DKEY) {
@@ -76,11 +120,125 @@ u32 blockSize(const PatInfo &pi) {
         }
         sz += instrSize<InstrReportExhaust>();
     } else if (pi.dkey != INVALID_DKEY) {
-        sz += instrSize<InstrDedupeAndReport>();
-    } else {
+        sz += pi.p->quiet ? instrSize<InstrDedupe>() : instrSize<InstrDedupeAndReport>();
+    } else if (!pi.p->quiet) {
         sz += instrSize<InstrReport>();
     }
     return sz;
+}
+
+u32 blockSize(const PatInfo &pi, const LogicalSet *ls) {
+    return (pi.p->s.size() > 8 ? instrSize<InstrCheckLit>() : 0) + reportSize(pi, ls);
+}
+
+/* Write the report block of pattern pi at pc; a failed check jumps to `failTo`. */
+void writeReport(Blob &blob, u32 pc, const PatInfo &pi, u32 failTo, const LogicalSet *ls) {
+    const u32 report = pi.p->report;
+    if (pi.ekey != INVALID_EKEY) {
+        InstrCheckExhausted ce;
+        memset(&ce, 0, sizeof(ce));
+        ce.code = OP_CHECK_EXHAUSTED;
+        ce.ekey = pi.ekey;
+        ce.fail_jump = failTo - pc;
+        memcpy(blob.at(pc), &ce, sizeof(ce));
+        pc += instrSize<InstrCheckExhausted>();
+        pc = writeFlush(blob, pc, ls);
+        if (pi.dkey != INVALID_DKEY) {
+            InstrDedupe d;
+            memset(&d, 0, sizeof(d));
+            d.code = OP_DEDUPE;
+            d.dkey = pi.dkey;
+            d.fail_jump = failTo - pc;
+            memcpy(blob.at(pc), &d, sizeof(d));
+            pc += instrSize<InstrDedupe>();
+        }
+        InstrReportExhaust re;
+        memset(&re, 0, sizeof(re));
+        re.code = OP_REPORT_EXHAUST;
+        re.onmatch = report;
+        re.ekey = pi.ekey;
+        memcpy(blob.at(pc), &re, sizeof(re));
+        pc += instrSize<InstrReportExhaust>();
+    } else if (pi.dkey != INVALID_DKEY) {
+        pc = writeFlush(blob, pc, ls);
+        if (pi.p->quiet) {
+            InstrDedupe d;
+            memset(&d, 0, sizeof(d));
+            d.code = OP_DEDUPE;
+            d.dkey = pi.dkey;
+            d.fail_jump = failTo - pc;
+            memcpy(blob.at(pc), &d, sizeof(d));
+            pc += instrSize<InstrDedupe>();
+        } else {
+            InstrDedupeAndReport dr;
+            memset(&dr, 0, sizeof(dr));
+            dr.code = OP_DEDUPE_AND_REPORT;
+            dr.dkey = pi.dkey;
+            dr.onmatch = report;
+            dr.fail_jump = failTo - pc;
+            memcpy(blob.at(pc), &dr, sizeof(dr));
+            pc += instrSize<InstrDedupeAndReport>();
+        }
+    } else {
+        pc = writeFlush(blob, pc, ls);
+        if (!pi.p->quiet) {
+            InstrReport r;
+            memset(&r, 0, sizeof(r));
+            r.code = OP_REPORT;
+            r.onmatch = report;
+            memcpy(blob.at(pc), &r, sizeof(r));
+            pc += instrSize<InstrReport>();
+        }
+    }
+    writeLogical(blob, pc, ls, report, 0);
+}
+
+/* The combination tables (src/rose/rose_build_bytecode.cpp:2497-2506 writeLogicalInfo) and the
+ * LAST_FLUSH_COMBINATION program run at the end of a block (:3362-3369), added to the blob. */
+void writeLogicalInfo(Blob &blob, const LogicalSet *ls, RoseEngine *r) {
+    if (!ls || ls->empty()) {
+        return;
+    }
+    if (!ls->tree.empty()) {
+        r->logicalTreeOffset = blob.add(ls->tree.data(), ls->tree.size() * sizeof(LogicalOp), alignof(LogicalOp));
+    }
+    r->combInfoMapOffset = blob.add(ls->combs.data(), ls->combs.size() * sizeof(CombInfo), alignof(CombInfo));
+    r->lkeyCount = (u32)ls->lkeyOf.size();
+    r->lopCount = (u32)ls->tree.size();
+    r->ckeyCount = (u32)ls->combs.size();
+    const u32 prog = blob.reserve(instrSize<InstrLastFlushCombination>() + instrSize<InstrEnd>(), INSTR_ALIGN);
+    *blob.at(prog) = OP_LAST_FLUSH_COMBINATION;
+    *blob.at(prog + instrSize<InstrLastFlushCombination>()) = OP_END;
+    r->lastFlushCombProgramOffset = prog;
+}
+
+/* A combination with HS_FLAG_SINGLEMATCH takes the exhaustion key of its id (compiler.cpp:297-299
+ * getExhaustibleKey), after those of the expressions. */
+void assignCombinationEkeys(LogicalSet *ls, std::map<u32, u32> *ekeys) {
+    if (!ls) {
+        return;
+    }
+    for (CombInfo &ci : ls->combs) {
+        if (ci.ekey != INVALID_EKEY) {
+            ci.ekey = ekeys->emplace(ci.id, (u32)ekeys->size()).first->second;
+        }
+    }
+}
+
+/* the logical and combination multibits in the state, after the exhaustion vector (fillStateOffsets,
+ * src/rose/rose_build_bytecode.cpp:429-438); returns the offset after them */
+u32 layoutLogicalState(const RoseEngine &r, StateOffsets *so, u32 cur) {
+    so->logicalVec = cur;
+    if (r.ckeyCount) {
+        so->logicalVec_size = mmbitSize(r.lkeyCount + r.lopCount);
+        cur += so->logicalVec_size;
+    }
+    so->combVec = cur;
+    if (r.ckeyCount) {
+        so->combVec_size = mmbitSize(r.ckeyCount);
+        cur += so->combVec_size;
+    }
+    return cur;
 }
 
 /* What the header needs to know about the literal set. */
@@ -88,6 +246,7 @@ struct RoseTail {
     u32 minLen, maxLen, ekeyCount, dkeyCount, invDkeyOffset;
     bool canExhaust;
     u32 smallWriteOffset = 0;
+    const LogicalSet *logic = nullptr;
 };
 
 /* A database whose only matcher is ONE engine run as an outfix over the whole block
@@ -101,6 +260,7 @@ std::vector<u8> finishOutfixRose(Blob &blob, const std::vector<u8> &nfa, const R
     const u32 nfaOffset = blob.add(nfa.data(), nfa.size(), 64);
     RoseEngine r;
     memset(&r, 0, sizeof(r));
+    writeLogicalInfo(blob, t.logic, &r);
     r.pureLiteral = 0;
     r.runtimeImpl = RUNTIME_SINGLE_OUTFIX;
     r.canExhaust = t.canExhaust ? 1 : 0;
@@ -138,7 +298,7 @@ std::vector<u8> finishOutfixRose(Blob &blob, const std::vector<u8> &nfa, const R
     so.exhausted = cur;
     so.exhausted_size = mmbitSize(r.ekeyCount);
     cur += so.exhausted_size;
-    so.logicalVec = so.combVec = cur;
+    cur = layoutLogicalState(r, &so, cur);
     so.nfaStateBegin = cur;
     NfaInfo ni;
     memset(&ni, 0, sizeof(ni));
@@ -168,11 +328,12 @@ std::vector<u8> finishRose(Blob &blob, const std::vector<HwlmLit> &hl, const Ros
         throw CompileError{std::string("Unable to build literal matcher: ") + e.what(), -1};
     }
     const u32 fmatcherOffset = blob.add(hwlm.data(), hwlm.size(), 64);
+    RoseEngine r;
+    memset(&r, 0, sizeof(r));
+    writeLogicalInfo(blob, t.logic, &r);
     const u32 total = (u32)HSB_ROUNDUP(blob.base + blob.bytes.size(), 64);
 
     /* --- header --- */
-    RoseEngine r;
-    memset(&r, 0, sizeof(r));
     r.pureLiteral = opts.pureLiteralApi ? 1 : 0;
     r.runtimeImpl = RUNTIME_PURE_LITERAL;
     r.canExhaust = t.canExhaust ? 1 : 0;
@@ -216,7 +377,7 @@ std::vector<u8> finishRose(Blob &blob, const std::vector<HwlmLit> &hl, const Ros
     so.exhausted = cur;
     so.exhausted_size = mmbitSize(r.ekeyCount);
     cur += so.exhausted_size;
-    so.logicalVec = so.combVec = cur;
+    cur = layoutLogicalState(r, &so, cur);
     so.nfaStateBegin = so.end = cur;
 
     std::vector<u8> out(total, 0);
@@ -228,7 +389,7 @@ std::vector<u8> finishRose(Blob &blob, const std::vector<HwlmLit> &hl, const Ros
 } // namespace
 
 std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
-                                 const CompileOpts &opts, HwlmBuildInfo *info) {
+                                 const CompileOpts &opts, HwlmBuildInfo *info, LogicalSet *logic) {
     if (patsIn.empty()) {
         throw CompileError{"Invalid parameter: elements is zero", -1};
     }
@@ -313,6 +474,7 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
             pi.dkey = it->second;
         }
     }
+    assignCombinationEkeys(logic, &ekeys);
 
     if (opts.outfixKind) {
         /* --- single-outfix database: report programs ([CHECK_EXHAUSTED] [DEDUPE] REPORT_EXHAUST |
@@ -327,47 +489,9 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
         for (const PatInfo &pi : pats) {
             minLen = std::min<u32>(minLen, (u32)pi.p->s.size());
             maxLen = std::max<u32>(maxLen, (u32)pi.p->s.size());
-            const u32 sz = blockSize(pi) - (pi.p->s.size() > 8 ? instrSize<InstrCheckLit>() : 0) + instrSize<InstrEnd>();
-            u32 pc = blob.reserve(sz, INSTR_ALIGN);
-            const u32 prog = pc, endAt = pc + sz - instrSize<InstrEnd>();
-            if (pi.ekey != INVALID_EKEY) {
-                InstrCheckExhausted ce;
-                memset(&ce, 0, sizeof(ce));
-                ce.code = OP_CHECK_EXHAUSTED;
-                ce.ekey = pi.ekey;
-                ce.fail_jump = endAt - pc;
-                memcpy(blob.at(pc), &ce, sizeof(ce));
-                pc += instrSize<InstrCheckExhausted>();
-                if (pi.dkey != INVALID_DKEY) {
-                    InstrDedupe dd;
-                    memset(&dd, 0, sizeof(dd));
-                    dd.code = OP_DEDUPE;
-                    dd.dkey = pi.dkey;
-                    dd.fail_jump = endAt - pc;
-                    memcpy(blob.at(pc), &dd, sizeof(dd));
-                    pc += instrSize<InstrDedupe>();
-                }
-                InstrReportExhaust re;
-                memset(&re, 0, sizeof(re));
-                re.code = OP_REPORT_EXHAUST;
-                re.onmatch = pi.p->report;
-                re.ekey = pi.ekey;
-                memcpy(blob.at(pc), &re, sizeof(re));
-            } else if (pi.dkey != INVALID_DKEY) {
-                InstrDedupeAndReport dr;
-                memset(&dr, 0, sizeof(dr));
-                dr.code = OP_DEDUPE_AND_REPORT;
-                dr.dkey = pi.dkey;
-                dr.onmatch = pi.p->report;
-                dr.fail_jump = endAt - pc;
-                memcpy(blob.at(pc), &dr, sizeof(dr));
-            } else {
-                InstrReport rr;
-                memset(&rr, 0, sizeof(rr));
-                rr.code = OP_REPORT;
-                rr.onmatch = pi.p->report;
-                memcpy(blob.at(pc), &rr, sizeof(rr));
-            }
+            const u32 sz = reportSize(pi, logic) + instrSize<InstrEnd>();
+            const u32 prog = blob.reserve(sz, INSTR_ALIGN), endAt = prog + sz - instrSize<InstrEnd>();
+            writeReport(blob, prog, pi, endAt, logic);
             InstrEnd e;
             e.code = OP_END;
             memcpy(blob.at(endAt), &e, sizeof(e));
@@ -391,6 +515,7 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
             t.invDkeyOffset = blob.add(inv.data(), inv.size() * sizeof(u32), 4);
         }
         t.canExhaust = allHighlander;
+        t.logic = logic;
         std::vector<u8> nfa;
         try {
             if (opts.outfixKind == OUTFIX_LIMEX32) {
@@ -451,15 +576,14 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
     for (Fragment &fr : frags) {
         u32 total = instrSize<InstrEnd>();
         for (u32 pi : fr.pats) {
-            total += blockSize(pats[pi]);
+            total += blockSize(pats[pi], logic);
         }
         const u32 start = blob.reserve(total, INSTR_ALIGN);
         fr.program = start;
         u32 pc = start;
         for (size_t k = 0; k < fr.pats.size(); k++) {
             const PatInfo &pi = pats[fr.pats[k]];
-            const u32 next = pc + blockSize(pi); /* next pattern's block or END */
-            const u32 report = pi.p->report;
+            const u32 next = pc + blockSize(pi, logic); /* next pattern's block or END */
             if (pi.p->s.size() > 8) {
                 InstrCheckLit in;
                 memset(&in, 0, sizeof(in));
@@ -471,47 +595,8 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
                 pendingLits.push_back({pc, pi.folded});
                 pc += instrSize<InstrCheckLit>();
             }
-            if (pi.ekey != INVALID_EKEY) {
-                InstrCheckExhausted ce;
-                memset(&ce, 0, sizeof(ce));
-                ce.code = OP_CHECK_EXHAUSTED;
-                ce.ekey = pi.ekey;
-                ce.fail_jump = next - pc;
-                memcpy(blob.at(pc), &ce, sizeof(ce));
-                pc += instrSize<InstrCheckExhausted>();
-                if (pi.dkey != INVALID_DKEY) {
-                    InstrDedupe d;
-                    memset(&d, 0, sizeof(d));
-                    d.code = OP_DEDUPE;
-                    d.dkey = pi.dkey;
-                    d.fail_jump = next - pc;
-                    memcpy(blob.at(pc), &d, sizeof(d));
-                    pc += instrSize<InstrDedupe>();
-                }
-                InstrReportExhaust re;
-                memset(&re, 0, sizeof(re));
-                re.code = OP_REPORT_EXHAUST;
-                re.onmatch = report;
-                re.ekey = pi.ekey;
-                memcpy(blob.at(pc), &re, sizeof(re));
-                pc += instrSize<InstrReportExhaust>();
-            } else if (pi.dkey != INVALID_DKEY) {
-                InstrDedupeAndReport dr;
-                memset(&dr, 0, sizeof(dr));
-                dr.code = OP_DEDUPE_AND_REPORT;
-                dr.dkey = pi.dkey;
-                dr.onmatch = report;
-                dr.fail_jump = next - pc;
-                memcpy(blob.at(pc), &dr, sizeof(dr));
-                pc += instrSize<InstrDedupeAndReport>();
-            } else {
-                InstrReport r;
-                memset(&r, 0, sizeof(r));
-                r.code = OP_REPORT;
-                r.onmatch = report;
-                memcpy(blob.at(pc), &r, sizeof(r));
-                pc += instrSize<InstrReport>();
-            }
+            writeReport(blob, pc, pi, next, logic);
+            pc = next;
         }
         InstrEnd e;
         e.code = OP_END;
@@ -557,6 +642,7 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
     t.dkeyCount = (u32)dkeys.size();
     t.invDkeyOffset = invDkeyOffset;
     t.canExhaust = allHighlander;
+    t.logic = logic;
 
     /* --- small-write engine (src/smallwrite/smallwrite_build.cpp; used by hs_scan for
      * buffers shorter than largestBuffer, src/runtime.c:401-413): one DFA over the WHOLE
@@ -581,47 +667,9 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
                 break;
             }
             /* report program: [CHECK_EXHAUSTED] [DEDUPE] REPORT_EXHAUST | DEDUPE_AND_REPORT | REPORT, END */
-            const u32 sz = blockSize(pi) - (pi.p->s.size() > 8 ? instrSize<InstrCheckLit>() : 0) + instrSize<InstrEnd>();
-            u32 pc = blob.reserve(sz, INSTR_ALIGN);
-            const u32 prog = pc, endAt = pc + sz - instrSize<InstrEnd>();
-            if (pi.ekey != INVALID_EKEY) {
-                InstrCheckExhausted ce;
-                memset(&ce, 0, sizeof(ce));
-                ce.code = OP_CHECK_EXHAUSTED;
-                ce.ekey = pi.ekey;
-                ce.fail_jump = endAt - pc;
-                memcpy(blob.at(pc), &ce, sizeof(ce));
-                pc += instrSize<InstrCheckExhausted>();
-                if (pi.dkey != INVALID_DKEY) {
-                    InstrDedupe dd;
-                    memset(&dd, 0, sizeof(dd));
-                    dd.code = OP_DEDUPE;
-                    dd.dkey = pi.dkey;
-                    dd.fail_jump = endAt - pc;
-                    memcpy(blob.at(pc), &dd, sizeof(dd));
-                    pc += instrSize<InstrDedupe>();
-                }
-                InstrReportExhaust re;
-                memset(&re, 0, sizeof(re));
-                re.code = OP_REPORT_EXHAUST;
-                re.onmatch = pi.p->report;
-                re.ekey = pi.ekey;
-                memcpy(blob.at(pc), &re, sizeof(re));
-            } else if (pi.dkey != INVALID_DKEY) {
-                InstrDedupeAndReport dr;
-                memset(&dr, 0, sizeof(dr));
-                dr.code = OP_DEDUPE_AND_REPORT;
-                dr.dkey = pi.dkey;
-                dr.onmatch = pi.p->report;
-                dr.fail_jump = endAt - pc;
-                memcpy(blob.at(pc), &dr, sizeof(dr));
-            } else {
-                InstrReport rr;
-                memset(&rr, 0, sizeof(rr));
-                rr.code = OP_REPORT;
-                rr.onmatch = pi.p->report;
-                memcpy(blob.at(pc), &rr, sizeof(rr));
-            }
+            const u32 sz = reportSize(pi, logic) + instrSize<InstrEnd>();
+            const u32 prog = blob.reserve(sz, INSTR_ALIGN), endAt = prog + sz - instrSize<InstrEnd>();
+            writeReport(blob, prog, pi, endAt, logic);
             InstrEnd e;
             e.code = OP_END;
             memcpy(blob.at(endAt), &e, sizeof(e));
@@ -649,7 +697,7 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
     return finishRose(blob, hl, t, opts, info);
 }
 
-std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const CompileOpts &opts) {
+std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const CompileOpts &opts, LogicalSet *logic) {
     if (pats.empty()) {
         throw CompileError{"Invalid parameter: elements is zero", -1};
     }
@@ -683,6 +731,7 @@ std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const Comp
         }
         dkeys.emplace(p.report, (u32)dkeys.size());
     }
+    assignCombinationEkeys(logic, &ekeys);
     Blob blob((u32)HSB_ROUNDUP(sizeof(RoseEngine), 64));
     RawNfa nfa;
     regexNfaInit(&nfa);
@@ -695,10 +744,12 @@ std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const Comp
             return pit->second;
         }
         const bool single = (p.flags & HS_FLAG_SINGLEMATCH) != 0;
+        const bool quiet = (p.flags & HS_FLAG_QUIET) != 0;
         const bool bounded = p.minOffset > 0 || p.maxOffset != ~0ull;
-        u32 sz = instrSize<InstrEnd>() + (bounded ? instrSize<InstrCheckBounds>() : 0);
+        u32 sz = instrSize<InstrEnd>() + (bounded ? instrSize<InstrCheckBounds>() : 0) + flushSize(logic) +
+                 logicalSize(logic, p.report);
         sz += single ? instrSize<InstrCheckExhausted>() + instrSize<InstrDedupe>() + instrSize<InstrReportExhaust>()
-                     : instrSize<InstrDedupeAndReport>();
+                     : quiet ? instrSize<InstrDedupe>() : instrSize<InstrDedupeAndReport>();
         u32 pc = blob.reserve(sz, INSTR_ALIGN);
         const u32 prog = pc;
         const u32 endAt = pc + sz - instrSize<InstrEnd>();
@@ -722,6 +773,7 @@ std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const Comp
             ce.fail_jump = endAt - pc;
             memcpy(blob.at(pc), &ce, sizeof(ce));
             pc += instrSize<InstrCheckExhausted>();
+            pc = writeFlush(blob, pc, logic);
             InstrDedupe dd;
             memset(&dd, 0, sizeof(dd));
             dd.code = OP_DEDUPE;
@@ -737,7 +789,19 @@ std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const Comp
             re.offset_adjust = adjust;
             re.ekey = ekeys[p.report];
             memcpy(blob.at(pc), &re, sizeof(re));
+            pc += instrSize<InstrReportExhaust>();
+        } else if (quiet) {
+            pc = writeFlush(blob, pc, logic);
+            InstrDedupe dd;
+            memset(&dd, 0, sizeof(dd));
+            dd.code = OP_DEDUPE;
+            dd.dkey = dkeys[p.report];
+            dd.offset_adjust = adjust;
+            dd.fail_jump = endAt - pc;
+            memcpy(blob.at(pc), &dd, sizeof(dd));
+            pc += instrSize<InstrDedupe>();
         } else {
+            pc = writeFlush(blob, pc, logic);
             InstrDedupeAndReport dr;
             memset(&dr, 0, sizeof(dr));
             dr.code = OP_DEDUPE_AND_REPORT;
@@ -746,7 +810,9 @@ std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const Comp
             dr.offset_adjust = adjust;
             dr.fail_jump = endAt - pc;
             memcpy(blob.at(pc), &dr, sizeof(dr));
+            pc += instrSize<InstrDedupeAndReport>();
         }
+        writeLogical(blob, pc, logic, p.report, adjust);
         InstrEnd e;
         e.code = OP_END;
         memcpy(blob.at(endAt), &e, sizeof(e));
@@ -814,6 +880,7 @@ std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const Comp
     }
     t.invDkeyOffset = blob.add(inv.data(), inv.size() * sizeof(u32), 4);
     t.canExhaust = allHighlander;
+    t.logic = logic;
     std::vector<u8> eng;
     try {
         /* small automata run as DFAs, as in the reference (ng_mcclellan before LimEx); the report programs are

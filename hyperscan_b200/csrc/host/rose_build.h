@@ -20,10 +20,17 @@ struct CompileError {
     int index; /* expression index or -1 */
 };
 
+} // namespace hsb
+
+#include "logical.h"
+
+namespace hsb {
+
 struct LitPattern {
     std::string s;      /* raw bytes of the literal */
     bool caseless = false;
     bool singlematch = false;
+    bool quiet = false; /* HS_FLAG_QUIET: no report, only its part in combinations */
     u32 report = 0;     /* user-visible id */
     u32 index = 0;      /* position in the caller's expression array */
 };
@@ -51,9 +58,10 @@ static const size_t LIMIT_PATTERN_LENGTH = 16000;
 static const size_t LIMIT_LITERAL_LENGTH = 1600;
 static const size_t LIMIT_LITERAL_COUNT = 8000000;
 
-/** Build the RoseEngine bytecode for a set of literal patterns. */
+/** Build the RoseEngine bytecode for a set of literal patterns.  `logic` (may be null): the
+ * logical combinations over them; combinations with HS_FLAG_SINGLEMATCH get their ekeys here. */
 std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &pats,
-                                 const CompileOpts &opts, HwlmBuildInfo *info);
+                                 const CompileOpts &opts, HwlmBuildInfo *info, LogicalSet *logic = nullptr);
 
 /** Expressions that need an NFA (regex_nfa.h): ONE LimEx-32 engine over all of them, run as the
  * database's single outfix (ROSE_RUNTIME_SINGLE_OUTFIX).  Block mode only.  Throws CompileError. */
@@ -65,7 +73,8 @@ struct RegexPattern {
     u64 minOffset = 0, maxOffset = ~0ull; /* hs_expr_ext: bounds on the match end (CHECK_BOUNDS in the report programs) */
     u64 minLength = 0;                    /* hs_expr_ext: shortest match that counts (regex_nfa.cpp) */
 };
-std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const CompileOpts &opts);
+std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const CompileOpts &opts,
+                               LogicalSet *logic = nullptr);
 
 /** Test hook: pure-literal block database from raw literal programs (`area`
  * is placed at programAreaBase(); lits[i].id = its program's offset in area). */

@@ -328,7 +328,11 @@ enum RoseOp {
     OP_CHECK_MED_LIT_NOCASE = 54,
     OP_CLEAR_WORK_DONE = 55,
     OP_INCLUDED_JUMP = 61,
+    OP_SET_LOGICAL = 62,
+    OP_SET_COMBINATION = 63,
+    OP_FLUSH_COMBINATION = 64,
     OP_SET_EXHAUST = 65,
+    OP_LAST_FLUSH_COMBINATION = 66,
     OP_CHECK_MASK_64 = 69,
     OP_LAST = 69
 };
@@ -354,6 +358,34 @@ struct InstrSquashGroups { u8 code; u64 groups; };
 struct InstrCheckLit { u8 code; u32 lit_offset; u32 lit_length; u32 fail_jump; }; /* MED + LONG */
 struct InstrIncludedJump { u8 code, squash; u32 child_offset; };
 struct InstrSetExhaust { u8 code; u32 ekey; };
+struct InstrSetLogical { u8 code; u32 lkey; s32 offset_adjust; };
+struct InstrSetCombination { u8 code; u32 ckey; };
+struct InstrFlushCombination { u8 code; };
+struct InstrLastFlushCombination { u8 code; };
+
+/* ---- logical combinations: src/util/logical.h:42-72 -------------------- */
+
+static const u32 INVALID_LKEY = 0xffffffffu;
+static const u64 MAX_OFFSET = ~0ull;
+enum LogicalOpType { LOGICAL_OP_NOT = 0, LOGICAL_OP_AND = 1, LOGICAL_OP_OR = 2 };
+
+/* one operation of the tree at logicalTreeOffset; its id is lkeyCount + its index */
+struct LogicalOp {
+    u32 id;
+    u32 op; /* LogicalOpType */
+    u32 lo; /* left operand (unused for NOT) */
+    u32 ro; /* right operand */
+};
+
+/* one combination (ckey = index) at combInfoMapOffset: operations start..result of the tree */
+struct CombInfo {
+    u32 id;
+    u32 ekey; /* INVALID_EKEY unless HS_FLAG_SINGLEMATCH */
+    u32 start;
+    u32 result;
+    u64 min_offset;
+    u64 max_offset;
+};
 
 /* ---- NFA engines (DFA subset): src/nfa/nfa_internal.h:53-126,
  *      src/nfa/mcclellan_internal.h:36-106 -------------------------------- */

@@ -138,7 +138,11 @@ typedef int (*match_event_handler)(unsigned int id, unsigned long long from,
  * (ROSE_RUNTIME_SINGLE_OUTFIX) when its positions fit -- DESIGN.md section 10b.
  * Anything else (look-around, back-references, UTF-8 / UCP, larger sets, ...) yields
  * HS_COMPILER_ERROR with an explanatory hs_compile_error_t, exactly as the
- * reference reports unsupported constructs. */
+ * reference reports unsupported constructs.
+ * Logical combinations (HS_FLAG_COMBINATION, with HS_FLAG_QUIET on any expression) are
+ * compiled in block mode, over either kind of database (DESIGN.md section 10c); in
+ * streaming and vectored mode they are a compile error, and so is HS_FLAG_QUIET
+ * together with HS_FLAG_SINGLEMATCH on an expression that is not a combination. */
 hs_error_t hs_compile(const char *expression, unsigned int flags,
                       unsigned int mode, const hs_platform_info_t *platform,
                       hs_database_t **db, hs_compile_error_t **error);
@@ -259,7 +263,13 @@ hs_error_t hs_scan_vector(const hs_database_t *db, const char *const *data,
  * Part 2: H100 batch / device-resident extension
  * ---------------------------------------------------------------------- */
 
-/* One match record as the device writes it (16 bytes; SURVEY.md section 8d). */
+/* One match record as the device writes it (16 bytes; SURVEY.md section 8d).
+ * Raw records of a database with logical combinations (HS_FLAG_COMBINATION) also
+ * hold logical-key records: bit 63 of `to` set, `id` = the logical key of a
+ * sub-expression that matched, `to` & ~(1 << 63) = where.  No match offset reaches
+ * 2^63, and every id is a valid user id, so the bit is what tells them apart.  The
+ * ordered forms (callbacks, _collect, hs_b200_fetch_matches,
+ * hs_b200_postprocess_blocks) replace them with the combination reports. */
 typedef struct hs_b200_match {
     unsigned int id;             /* report id the user registered */
     unsigned int block;          /* index of the block in the batch */
@@ -289,7 +299,9 @@ hs_error_t hs_b200_scan_blocks(const hs_database_t *db, const char *data,
 
 /* Same, the delivered matches written to `out` in (block, to, id) order (the order
  * the callbacks would fire in, all report rules applied) instead of one callback
- * per match.  HS_INSUFFICIENT_SPACE: more than `cap` matches (*nmatches tells; the
+ * per match.  With logical combinations the order within one (block, to) is the
+ * reference's: the expressions' reports by id, then the combination reports the
+ * offset completes, by combination (in the order the combinations were given).  HS_INSUFFICIENT_SPACE: more than `cap` matches (*nmatches tells; the
  * first cap are valid). */
 hs_error_t hs_b200_scan_blocks_collect(const hs_database_t *db, const char *data,
                                        const unsigned long long *offsets,
@@ -362,14 +374,29 @@ hs_error_t hs_b200_set_peer_exchange(hs_scratch_t *scratch, unsigned int nranks,
  * (in place; e.g. the concatenation of all ranks' records after the
  * all-gather): sort by (block, to, id), one record per (block, id, to),
  * HS_FLAG_SINGLEMATCH reports keep their first match per block.  Host only
- * (needs no CUDA device). */
+ * (needs no CUDA device).  A database with logical combinations is refused
+ * (HS_INVALID): its reports depend on the block lengths, see below. */
 hs_error_t hs_b200_postprocess_matches(const hs_database_t *db,
                                        hs_b200_match_t *recs, size_t n,
                                        unsigned long long *nout);
+/* The same for the raw records of blocks 0 .. nblocks-1 whose lengths are given,
+ * for any database, written to `out`: with logical combinations, the logical-key
+ * records are evaluated block by block as hs_scan would (a combination that is
+ * true with none of its sub-expressions matched reports at the block's end), and
+ * the order within one (block, to) is as for hs_b200_scan_blocks_collect.  Records
+ * of blocks >= nblocks are dropped.  HS_INSUFFICIENT_SPACE: more than `cap` records
+ * (*nout tells).  Host only. */
+hs_error_t hs_b200_postprocess_blocks(const hs_database_t *db,
+                                      const hs_b200_match_t *recs, size_t n,
+                                      const unsigned int *lengths, size_t nblocks,
+                                      hs_b200_match_t *out, size_t cap,
+                                      unsigned long long *nout);
 /* Copy the records of the last finished scan to the host, apply the
  * host-side report rules (dedupe per (id,to); HS_FLAG_SINGLEMATCH keeps the
  * first match per id and block), sort by (block, to, id).  `out` may be NULL
- * to query the count. */
+ * to query the count.  With logical combinations the combination reports are
+ * added (order as for hs_b200_scan_blocks_collect); they need the block lengths
+ * of the corpus last scanned, which must not have been freed. */
 hs_error_t hs_b200_fetch_matches(const hs_database_t *db, hs_scratch_t *scratch,
                                  hs_b200_match_t *out, size_t cap,
                                  unsigned long long *nmatches);
