@@ -101,9 +101,10 @@ struct DevImage {
     u32 bitmapBytes = 0, bitmapShift = 0, keyBytes = 0;
     u32 pairBytes = 0, bitmapBits = 0; /* FK_PAIR32 layout (kernels.h) */
     u32 bucketFold = 0;
-    u32 nfaOffset = 0, nfaLength = 0;   /* FK_OUTFIX: the sole engine (bytecode offset, NFA.length) */
+    u32 nfaOffset = 0, nfaLength = 0;   /* the outfix engine (bytecode offset, NFA.length), alone (FK_OUTFIX) or
+                                         * beside the literal matcher; nfaLength == 0: none */
     DfaParams nfaParams;                /* ... and what launchDfa needs to know about it */
-    /* FK_OUTFIX: report program offset -> its (onmatch, offset_adjust) list, filled as programs are met */
+    /* the outfix's report program offset -> its (onmatch, offset_adjust) list, filled as programs are met */
     mutable std::unordered_map<u32, std::vector<ProgReport>> progReports;
     double pairRate = 0;     /* FK_PAIR32: modelled first-stage candidates per byte (printable ASCII) */
     u8 *d_bitmap2 = nullptr; /* second level (HBM / L2) for large literal sets */
@@ -461,9 +462,26 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
     const bool soleOutfix = r->runtimeImpl == RUNTIME_SINGLE_OUTFIX && r->mode == MODE_BLOCK && r->queueCount == 1 &&
                             r->outfixBeginQueue == 0 && r->outfixEndQueue == 1 && r->nfaInfoOffset &&
                             !r->amatcherOffset && !r->ematcherOffset && !r->fmatcherOffset && !r->hasSom;
-    if (!soleOutfix && (r->runtimeImpl != RUNTIME_PURE_LITERAL || !r->fmatcherOffset)) {
-        /* FULL_ROSE databases need the full rose interpreter and the catch-up machinery
-         * (SURVEY.md section 8f rank 1): not in this build */
+    /* the one FULL_ROSE shape run here: the floating literal matcher, whose role-less programs report
+     * directly, and one outfix on queue 0 (DESIGN.md section 10d) -- no anchored, EOD or small-block
+     * matcher, no roles, leftfixes, suffixes, delayed literals, MPV, SOM or long-literal table, and an
+     * EOD program that at most checks the engines' EOD accepts */
+    const bool mixed = r->runtimeImpl == RUNTIME_FULL_ROSE && r->mode == MODE_BLOCK && r->fmatcherOffset &&
+                       !r->amatcherOffset && !r->ematcherOffset && !r->sbmatcherOffset && !r->drmatcherOffset &&
+                       r->queueCount == 1 && r->activeArrayCount == 1 && r->outfixBeginQueue == 0 &&
+                       r->outfixEndQueue == 1 && r->leftfixBeginQueue == 1 && r->nfaInfoOffset &&
+                       !r->activeLeftCount && !r->rosePrefixCount && !r->rolesWithStateCount && !r->delay_count &&
+                       !r->anchored_count && r->initMpvNfa == MO_INVALID_IDX && !r->hasSom &&
+                       !r->longLitTableOffset && !r->ckeyCount && !r->eagerIterOffset && !r->delayProgramOffset &&
+                       !r->anchoredProgramOffset && !r->boundary.reportEodOffset && !r->boundary.reportZeroOffset &&
+                       !r->boundary.reportZeroEodOffset && !r->lastByteHistoryIterOffset &&
+                       (!r->eodProgramOffset ||
+                        ((size_t)r->eodProgramOffset + 16 <= h->length && r->eodProgramOffset % INSTR_ALIGN == 0 &&
+                         bc[r->eodProgramOffset] == OP_ENGINES_EOD &&
+                         bc[r->eodProgramOffset + HSB_ROUNDUP(sizeof(InstrEnginesEod), INSTR_ALIGN)] == OP_END));
+    if (!soleOutfix && !mixed && (r->runtimeImpl != RUNTIME_PURE_LITERAL || !r->fmatcherOffset)) {
+        /* other FULL_ROSE databases need the full rose interpreter (SURVEY.md section 8f rank 1):
+         * not in this build */
         return HS_ARCH_ERROR;
     }
     DevImage *im = new (std::nothrow) DevImage();
@@ -487,11 +505,13 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
     if (r->ckeyCount) {
         loadCombinations(r, &im->comb);
     }
-    if (soleOutfix) {
+    if (soleOutfix || mixed) {
         /* hs_scan -> soleOutfixBlockExec (src/runtime.c:245-280): ONE engine over the whole block,
          * its reports are report programs (roseReportAdaptor, src/rose/match.c:611-633).  The
          * engine runs on the DFA / NFA kernels (dfa_kernels.cu) straight from the bytecode copy;
-         * the programs are resolved on the host when the records are ordered (postprocess). */
+         * the programs are resolved on the host when the records are ordered (postprocess).  With
+         * a literal matcher beside it (roseBlockExec's outfix), the engine's records are tagged so
+         * that the host can tell them from the literals' */
         if ((size_t)r->nfaInfoOffset + sizeof(NfaInfo) > h->length) {
             delete im;
             return HS_INVALID;
@@ -513,9 +533,12 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
             delete im;
             return er;
         }
-        im->kind = FK_OUTFIX;
         im->nfaOffset = ni.nfaOffset;
         im->nfaLength = nh.length;
+        im->nfaParams.toTag = mixed ? ENGINE_RECORD : 0;
+    }
+    if (soleOutfix) {
+        im->kind = FK_OUTFIX;
         im->groups = 0;
         cudaError_t e = cudaMalloc(&im->d_bc, HSB_ROUNDUP(h->length, 16));
         if (e == cudaSuccess) {
@@ -620,19 +643,19 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
             }
             memcpy(&table[b * 4], &e, 4);
         }
-        programsOk = collectProgramReports(bc, h->length, n.id, &im->exhaustible, nullptr, &im->comb.lkeyReport);
+        programsOk = collectProgramReports(bc, h->length, n.id, &im->exhaustible, nullptr, &im->comb.lkeyReport, mixed);
     } else if (hw->type == HWLM_ENGINE_FDR) {
         FDR f;
         memcpy(&f, bc + engOff, sizeof(f));
         im->confirmKind = CK_FDR;
         im->confOff = engOff + f.confOffset;
         if (f.engineID == 0) {
-            programsOk = walkConfirm(bc, h->length, im->confOff, 8, &im->exhaustible, &tails, &im->comb.lkeyReport);
+            programsOk = walkConfirm(bc, h->length, im->confOff, 8, &im->exhaustible, &tails, &im->comb.lkeyReport, mixed);
             pairStage(true);
         } else if (teddyIdValid(f.engineID)) {
             const u32 oct = teddyNumBuckets(f.engineID) / 8;
             programsOk = walkConfirm(bc, h->length, im->confOff, 8 * oct, &im->exhaustible, &tails,
-                                     &im->comb.lkeyReport);
+                                     &im->comb.lkeyReport, mixed);
             if (oct == 2) {
                 /* fat Teddy (49..96 literals): the class-pair kernel with 8 bucket bits that
                  * carry buckets i and i + 8 (confirmKernel unfolds them) */
@@ -1031,31 +1054,31 @@ hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
     if (t1 <= t0) {
         return HS_SUCCESS;
     }
-    if (im->kind == FK_OUTFIX) {
-        /* a block is one thread's walk from its first byte: wait for the last range of the
-         * corpus, then run the engine over every block */
-        const u32 ntiles = (u32)((c->bytes + pl.tileBytes - 1) / pl.tileBytes);
-        if (t1 < ntiles) {
-            return HS_SUCCESS;
+    if (im->kind != FK_OUTFIX) {
+        ScanParams p;
+        fillParams(s, im, c, pl, &p);
+        p.tileFirst = t0;
+        p.ntiles = t1 - t0;
+        LaunchCfg cfg = pl.cfg;
+        const u32 perCta = (u32)cfg.warps;
+        cfg.grid = (int)std::min<u32>((u32)cfg.grid, (p.ntiles + perCta - 1) / perCta);
+        if (t0 > 0) {
+            CUDA_TRY(cudaMemsetAsync(s->d_counters + CTR_CANDQ, 0, sizeof(u32), stream));
         }
-        CUDA_TRY(launchEngine(im->nfaParams, im->d_bc + im->nfaOffset, c, s->d_out, s->outCap, s->d_counters,
-                              s->smCount, s->maxSmem, stream));
-        return HS_SUCCESS;
+        CUDA_TRY(launchScan(cfg, p, stream));
+        g_launches++;
+        CUDA_TRY(launchConfirm(cfg, p, stream));
+        g_launches++;
     }
-    ScanParams p;
-    fillParams(s, im, c, pl, &p);
-    p.tileFirst = t0;
-    p.ntiles = t1 - t0;
-    LaunchCfg cfg = pl.cfg;
-    const u32 perCta = (u32)cfg.warps;
-    cfg.grid = (int)std::min<u32>((u32)cfg.grid, (p.ntiles + perCta - 1) / perCta);
-    if (t0 > 0) {
-        CUDA_TRY(cudaMemsetAsync(s->d_counters + CTR_CANDQ, 0, sizeof(u32), stream));
+    if (im->nfaLength) {
+        /* a block is one thread's walk from its first byte: after the last range of the corpus,
+         * the engine runs over every block, into the same record ring */
+        const u32 ntiles = (u32)((c->bytes + pl.tileBytes - 1) / pl.tileBytes);
+        if (t1 >= ntiles) {
+            CUDA_TRY(launchEngine(im->nfaParams, im->d_bc + im->nfaOffset, c, s->d_out, s->outCap, s->d_counters,
+                                  s->smCount, s->maxSmem, stream));
+        }
     }
-    CUDA_TRY(launchScan(cfg, p, stream));
-    g_launches++;
-    CUDA_TRY(launchConfirm(cfg, p, stream));
-    g_launches++;
     return HS_SUCCESS;
 }
 
@@ -1075,16 +1098,18 @@ void postprocessComb(const DevImage *im, std::vector<DevMatch> *v, const u32 *le
 }
 
 /* Records of a scan, ordered and with the order-dependent report rules applied (see
- * postprocessRecords).  Single-outfix databases: the kernel's records carry report PROGRAM
- * offsets (and the padding of the lanes' reserved slots); each is replaced by the reports its
- * program raises -- roseReportAdaptor -> roseRunProgram (src/rose/match.c:611-633) -- first.
- * Databases with logical combinations need the block lengths (lengths[0, nblocks)). */
+ * postprocessRecords).  Databases with an outfix: the engine kernel's records carry report PROGRAM
+ * offsets (and the padding of the lanes' reserved slots) -- all of a single-outfix database's
+ * records, and those tagged ENGINE_RECORD beside a literal matcher; each is replaced by the reports
+ * its program raises -- roseReportAdaptor -> roseRunProgram (src/rose/match.c:611-633) -- first,
+ * and the literals' records join them as they are.  Databases with logical combinations need the
+ * block lengths (lengths[0, nblocks)). */
 hs_error_t postprocessVec(const DevImage *im, std::vector<DevMatch> *v, const u32 *lengths = nullptr,
                           size_t nblocks = 0) {
     if (im->comb.any() && !lengths && nblocks) {
         return HS_INVALID;
     }
-    if (im->kind != FK_OUTFIX) {
+    if (!im->nfaLength) {
         if (im->comb.any()) {
             postprocessComb(im, v, lengths, nblocks);
         } else {
@@ -1095,7 +1120,15 @@ hs_error_t postprocessVec(const DevImage *im, std::vector<DevMatch> *v, const u3
     const u8 *bc = (const u8 *)dbRose((const hs_database_t *)(im->dbCopy.data() + im->dbCopyShift));
     std::vector<DevMatch> outv;
     outv.reserve(v->size());
-    for (const DevMatch &m : *v) {
+    const bool tagged = im->kind != FK_OUTFIX;
+    for (DevMatch m : *v) {
+        if (tagged) {
+            if (!(m.to & ENGINE_RECORD)) {
+                outv.push_back(m); /* a literal's record */
+                continue;
+            }
+            m.to &= ~ENGINE_RECORD;
+        }
         if (m.id == 0xffffffffu) {
             continue; /* a slot some lane reserved and did not fill */
         }
@@ -1158,6 +1191,11 @@ struct Upload {
  * ranges, read the counters back.  The only place a scan's stream sequence is issued. */
 hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
                        cudaStream_t stream, const Upload *up = nullptr) {
+    if (s->nPeers && im->nfaLength && im->kind != FK_OUTFIX) {
+        /* the engine kernel stores no records into the peers' exchange buffers, and the count it
+         * publishes would cover them: an exchange of both halves' records is not built */
+        return HS_ARCH_ERROR;
+    }
     ScanPlan pl;
     hs_error_t r = planScan(s, im, &pl);
     if (r != HS_SUCCESS) {
@@ -2131,7 +2169,7 @@ static hs_error_t scanHostBlocks(const DevImage *im, hs_scratch *s, const char *
     };
     /* nobody will look at the order, and neither dedupe keys nor
      * exhaustion keys exist: the raw count IS the delivered count */
-    const bool plain = countOnly && im->exhaustible.empty() && !im->hasDedupe && im->kind != FK_OUTFIX && !im->comb.any();
+    const bool plain = countOnly && im->exhaustible.empty() && !im->hasDedupe && !im->nfaLength && !im->comb.any();
     ScanTimes tm;
     r = scanRecords(s, im, c, &up, !plain, matches, &tm, lengths);
     if (r == HS_SUCCESS && trace) {

@@ -50,7 +50,7 @@ __device__ __forceinline__ u32 emitDfaMatch(const DfaParams &p, u32 cursor, u32 
         DevMatch m;
         m.id = id;
         m.block = block;
-        m.to = to;
+        m.to = to | p.toTag;
         *reinterpret_cast<uint4 *>(p.out + cursor) = *reinterpret_cast<const uint4 *>(&m);
     }
     return cursor + 1;
@@ -260,7 +260,7 @@ __device__ void padReserved(const DfaParams &p, u32 cursor) {
             DevMatch m;
             m.id = DFA_NO_RECORD;
             m.block = 0;
-            m.to = 0;
+            m.to = p.toTag;
             *reinterpret_cast<uint4 *>(p.out + cursor) = *reinterpret_cast<const uint4 *>(&m);
         }
     }
@@ -841,9 +841,33 @@ cudaError_t launchStaged(const DfaParams &p, int smCount, size_t tableBytes, cud
 
 } // namespace
 
+/* The lanes reserve record slots eight at a time and take a count that is not a multiple of eight
+ * for slots they already hold (emitDfaMatch).  In a ring that a literal matcher has written to
+ * first (p.toTag != 0), round the count up to a multiple of eight before the engine runs, and fill
+ * the slots in between with no-records. */
+__global__ void alignSharedRing(const DfaParams p) {
+    const u32 n = p.counters[CTR_MATCHES];
+    const u32 up = (u32)HSB_ROUNDUP((u64)n, DFA_SLOTS);
+    for (u32 i = n; i < up && i < p.outCap; i++) {
+        DevMatch m;
+        m.id = DFA_NO_RECORD;
+        m.block = 0;
+        m.to = p.toTag;
+        *reinterpret_cast<uint4 *>(p.out + i) = *reinterpret_cast<const uint4 *>(&m);
+    }
+    p.counters[CTR_MATCHES] = up;
+}
+
 cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t stream) {
     if (!p.nblocks) {
         return cudaSuccess;
+    }
+    if (p.toTag) {
+        HSB_LAUNCH(alignSharedRing, 1, 1, 0, stream, p);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) {
+            return e;
+        }
     }
     const size_t tilesMax = 32 * 2 * DfaTile<64>::WARP_BYTES;
     if (p.kind == NFA_SHENG) {

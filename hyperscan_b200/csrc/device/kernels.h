@@ -187,6 +187,8 @@ struct DfaParams {
     DevMatch *out;   /* {report, block, offset after the last byte} */
     u32 outCap;
     u32 *counters;   /* CTR_MATCHES */
+    u64 toTag;       /* ORed into every record's offset: ENGINE_RECORD (db_walk.h) when the engine's records
+                      * share the ring with a literal matcher's, else 0 */
 };
 cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t stream);
 

@@ -399,6 +399,9 @@ __device__ void runProgram(const ScanParams &p, const BlockRef &blk, u32 prog, u
         case OP_FLUSH_COMBINATION:
             NEXT(InstrFlushCombination);
             break;
+        case OP_CATCH_UP: /* (databases with an outfix only: the host orders its records among these) */
+            NEXT(InstrCatchUp);
+            break;
         default:
             atomicExch(p.counters + CTR_ERROR, (u32)ERR_BAD_OPCODE);
             return;

@@ -868,6 +868,7 @@ static hs_error_t compileCommon(const char *const *expressions,
         pats.reserve(elements);
         std::vector<RegexPattern> rpats; /* every expression, for the NFA route */
         bool needNfa = false;
+        bool anyCombination = false;
         LogicalSet logic; /* HS_FLAG_COMBINATION expressions */
         for (unsigned i = 0; i < elements; i++) {
             const unsigned f = flags ? flags[i] : 0;
@@ -878,6 +879,7 @@ static hs_error_t compileCommon(const char *const *expressions,
             if ((f & HS_FLAG_COMBINATION) && !litApi) {
                 /* src/compiler/compiler.cpp:286-322: a combination is no pattern of its own; a quiet one
                  * is dropped unparsed */
+                anyCombination = true;
                 if (f & ~(HS_FLAG_COMBINATION | HS_FLAG_QUIET | HS_FLAG_SINGLEMATCH)) {
                     throw CompileError{"only HS_FLAG_QUIET and HS_FLAG_SINGLEMATCH are supported in combination "
                                        "with HS_FLAG_COMBINATION.", (int)i};
@@ -1052,7 +1054,41 @@ static hs_error_t compileCommon(const char *const *expressions,
             opts.platform &= ~PLATFORM_NOAVX2; /* 16-bucket Teddy needs AVX2 on CPUs */
         }
         LogicalSet *ls = logic.empty() ? nullptr : &logic;
-        std::vector<u8> bc = needNfa ? buildRegexRose(rpats, opts, ls) : buildLiteralRose(pats, opts, nullptr, ls);
+        std::vector<u8> bc;
+        if (!needNfa) {
+            bc = buildLiteralRose(pats, opts, nullptr, ls);
+        } else {
+            /* the expressions that did not become literals: the engine half of a split set */
+            std::set<u32> litIndex;
+            for (const LitPattern &p : pats) {
+                litIndex.insert(p.index);
+            }
+            std::vector<RegexPattern> engineHalf;
+            for (const RegexPattern &rp : rpats) {
+                if (!litIndex.count(rp.index)) {
+                    engineHalf.push_back(rp);
+                }
+            }
+            const bool canSplit = !pats.empty() && !engineHalf.empty() && !anyCombination && !opts.streaming;
+            if (canSplit && mixedRoseOption()) {
+                bc = buildMixedRose(pats, engineHalf, opts, nullptr);
+            } else {
+                try {
+                    bc = buildRegexRose(rpats, opts, ls);
+                } catch (const CompileError &e) {
+                    /* the literals' character positions overflow the one automaton: the literals go to
+                     * a literal matcher and the rest to the engine; if that fails too, the error stays */
+                    if (!canSplit || e.msg.rfind("Pattern set is too large", 0) != 0) {
+                        throw;
+                    }
+                    try {
+                        bc = buildMixedRose(pats, engineHalf, opts, nullptr);
+                    } catch (const CompileError &) {
+                        throw e;
+                    }
+                }
+            }
+        }
         hs_error_t aerr;
         hs_database_t *out = dbCreate(bc, opts.platform, &aerr);
         if (!out) {
@@ -1246,14 +1282,18 @@ hs_error_t hs_expression_ext_info(const char *expression, unsigned int flags,
  * matchers as usual; 1 DFA chosen by size, 2 McClellan-8, 3 McClellan-16, 4 Sheng,
  * 5 LimEx-32: block-mode literal sets are compiled to a database whose only matcher is
  * that engine run as an outfix, ROSE_RUNTIME_SINGLE_OUTFIX); "regex_dfa" (1: regular expressions whose
- * determinised automaton stays small run as a McClellan DFA, 0: always as a LimEx NFA). */
+ * determinised automaton stays small run as a McClellan DFA, 0: always as a LimEx NFA); "mixed_rose" (0: a
+ * set of literals and regular expressions is split into a literal matcher and one engine only when the
+ * expressions' one automaton would be too large, 1: whenever it has both). */
 namespace hsb {
 static HwlmBuildOpts g_tunables;
 static bool g_tun_set[8];
 static int g_outfixEngine = 0; /* "outfix_engine": see enum OutfixKind (rose_build.h) */
 static int g_regexDfa = 1;     /* "regex_dfa": 0 = expressions always become a LimEx NFA */
+static int g_mixedRose = 0;    /* "mixed_rose": 1 = split literals from regexes whenever a set has both */
 int outfixEngineOption() { return g_outfixEngine; }
 int regexDfaOption() { return g_regexDfa; }
+int mixedRoseOption() { return g_mixedRose; }
 void applyBuildOptions(HwlmBuildOpts *o) {
     if (g_tun_set[0]) o->forceEngine = g_tunables.forceEngine;
     if (g_tun_set[1]) o->forceDomain = g_tunables.forceDomain;
@@ -1276,6 +1316,11 @@ extern "C" hs_error_t hs_b200_set_build_option(const char *key, int value) {
         g_tunables = HwlmBuildOpts();
         hsb::g_outfixEngine = 0;
         hsb::g_regexDfa = 1;
+        hsb::g_mixedRose = 0;
+        return HS_SUCCESS;
+    }
+    if (k == "mixed_rose") {
+        hsb::g_mixedRose = value != 0;
         return HS_SUCCESS;
     }
     if (k == "regex_dfa") {

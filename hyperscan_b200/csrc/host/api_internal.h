@@ -23,6 +23,7 @@ static inline const RoseEngine *dbRose(const hs_database_t *db) {
 void applyBuildOptions(HwlmBuildOpts *o);
 int outfixEngineOption(); /* build option "outfix_engine" (api_host.cpp) */
 int regexDfaOption();     /* build option "regex_dfa" (api_host.cpp) */
+int mixedRoseOption();    /* build option "mixed_rose" (api_host.cpp) */
 
 } // namespace hsb
 #endif

@@ -14,11 +14,11 @@ namespace hsb {
  * the walk continues past a terminator while a jump target lies beyond it.
  * Returns false on an opcode the device interpreter (scan_kernels.cu
  * runProgram) does not implement -- the state-carrying ones of
- * roseRunProgram_l: PUSH_DELAYED, CATCH_UP*, SOM_*, TRIGGER_SUFFIX, REPORT_CHAIN,
+ * roseRunProgram_l: PUSH_DELAYED, CATCH_UP* (CATCH_UP is accepted on request), SOM_*, TRIGGER_SUFFIX, REPORT_CHAIN,
  * REPORT_SOM*, SET_EXHAUST.  SET_LOGICAL is a report of its own here (a logical-key record
  * on the device); FLUSH_COMBINATION and SET_COMBINATION follow from it on the host. */
 bool collectProgramReports(const u8 *bc, u32 bcLen, u32 prog, std::unordered_set<u32> *ex,
-                           std::vector<ProgReport> *reports, LkeyReports *lkeys) {
+                           std::vector<ProgReport> *reports, LkeyReports *lkeys, bool catchUp) {
     u32 pc = prog, furthest = prog;
     u32 lastReport = INVALID_EKEY; /* the report of the current report block, for SET_LOGICAL */
     /* CHECK_BOUNDS guards the instructions up to its fail_jump target */
@@ -137,6 +137,12 @@ bool collectProgramReports(const u8 *bc, u32 bcLen, u32 prog, std::unordered_set
         case OP_SQUASH_GROUPS: STEP(InstrSquashGroups); break;
         case OP_CLEAR_WORK_DONE: pc += INSTR_ALIGN; break;
         case OP_INCLUDED_JUMP: STEP(InstrIncludedJump); break;
+        case OP_CATCH_UP:
+            if (!catchUp) {
+                return false;
+            }
+            STEP(InstrCatchUp);
+            break;
         default:
             return false;
         }
@@ -149,7 +155,7 @@ bool collectProgramReports(const u8 *bc, u32 bcLen, u32 prog, std::unordered_set
 /* Walk the hash-confirm structures to enumerate literal programs
  * (src/fdr/fdr_confirm.h:36-94). */
 bool walkConfirm(const u8 *bc, u32 bcLen, u32 confOff, u32 nBuckets,
-                 std::unordered_set<u32> *ex, std::vector<LitTail> *tails, LkeyReports *lkeys) {
+                 std::unordered_set<u32> *ex, std::vector<LitTail> *tails, LkeyReports *lkeys, bool catchUp) {
     bool ok = true;
     const u8 *confBase = bc + confOff;
     for (u32 b = 0; b < nBuckets; b++) {
@@ -172,7 +178,7 @@ bool walkConfirm(const u8 *bc, u32 bcLen, u32 confOff, u32 nBuckets,
             for (;;) {
                 LitInfo x;
                 memcpy(&x, li, sizeof(x));
-                ok &= collectProgramReports(bc, bcLen, x.id, ex, nullptr, lkeys);
+                ok &= collectProgramReports(bc, bcLen, x.id, ex, nullptr, lkeys, catchUp);
                 tails->push_back({x.v, x.msk, x.size, b});
                 if (!x.next) {
                     break;

@@ -44,12 +44,15 @@ struct ProgReport {
 /* lkey -> the report id whose report block sets it (a SET_LOGICAL after a report instruction; a quiet
  * sub-expression has none) */
 typedef std::unordered_map<u32, u32> LkeyReports;
+/* catchUp: the program belongs to a database with an outfix, where CATCH_UP only orders the outfix's
+ * reports before the literal's -- which the host's ordering does -- and is accepted */
 bool collectProgramReports(const u8 *bc, u32 bcLen, u32 prog, std::unordered_set<u32> *ex,
                            std::vector<ProgReport> *reports = nullptr, /* every report instruction, in program order */
-                           LkeyReports *lkeys = nullptr);
+                           LkeyReports *lkeys = nullptr, bool catchUp = false);
 
 bool walkConfirm(const u8 *bc, u32 bcLen, u32 confOff, u32 nBuckets,
-                 std::unordered_set<u32> *ex, std::vector<LitTail> *tails, LkeyReports *lkeys = nullptr);
+                 std::unordered_set<u32> *ex, std::vector<LitTail> *tails, LkeyReports *lkeys = nullptr,
+                 bool catchUp = false);
 
 /* Logical combinations of a database (RoseEngine.ckeyCount != 0): the tables the reference evaluates
  * per block (src/rose/program_runtime.c:2026-2120, src/report.h:190-245), copied from the bytecode. */
@@ -67,6 +70,9 @@ void loadCombinations(const RoseEngine *r, Combinations *cb);
 /* The bit of MatchRec.to that marks a logical-key record (id = lkey): written by SET_LOGICAL, consumed by
  * postprocessCombinations.  No match offset reaches 2^63. */
 static const u64 LKEY_RECORD = 1ull << 63;
+/* The bit of MatchRec.to that marks an engine's record in a database with a literal matcher and an
+ * outfix: its id is a report PROGRAM offset, resolved on the host; the literal records carry report ids. */
+static const u64 ENGINE_RECORD = 1ull << 62;
 
 /** Reports compiled with HS_FLAG_SINGLEMATCH in a pure-literal database. */
 hs_error_t collectExhaustible(const hs_database_t *db, std::unordered_set<u32> *ex, LkeyReports *lkeys = nullptr);

@@ -15,6 +15,7 @@
  *     shared report id   DEDUPE_AND_REPORT
  *     otherwise          REPORT
  *   END
+ * (beside an outfix, CATCH_UP before each report block: buildMixedRose)
  *
  * Literals longer than 8 bytes reach the literal matcher as their 8-byte
  * suffix (src/rose/rose_build_matchers.cpp:717-720); patterns with equal
@@ -249,157 +250,211 @@ struct RoseTail {
     const LogicalSet *logic = nullptr;
 };
 
-/* A database whose only matcher is ONE engine run as an outfix over the whole block
- * (ROSE_RUNTIME_SINGLE_OUTFIX: hs_scan -> soleOutfixBlockExec, src/runtime.c:245-280): queue 0,
- * no literal matchers.  What the reference's compiler emits for a pattern set that is all
- * engine and no literal (rose_build_bytecode.cpp:3672-3690 pickRuntimeImpl); here it is built
- * for literal sets on request, so that the DFA / NFA engines run inside a real database. */
-std::vector<u8> finishOutfixRose(Blob &blob, const std::vector<u8> &nfa, const RoseTail &t, const CompileOpts &opts) {
-    NFA hdr;
-    memcpy(&hdr, nfa.data(), sizeof(hdr));
-    const u32 nfaOffset = blob.add(nfa.data(), nfa.size(), 64);
-    RoseEngine r;
-    memset(&r, 0, sizeof(r));
-    writeLogicalInfo(blob, t.logic, &r);
-    r.pureLiteral = 0;
-    r.runtimeImpl = RUNTIME_SINGLE_OUTFIX;
-    r.canExhaust = t.canExhaust ? 1 : 0;
-    r.mode = MODE_BLOCK;
-    r.ekeyCount = t.ekeyCount;
-    r.dkeyCount = t.dkeyCount;
-    r.dkeyLogSize = fatbitSize(r.dkeyCount);
-    r.invDkeyOffset = t.invDkeyOffset;
-    r.somLocationFatbitSize = fatbitSize(0);
-    r.activeArrayCount = 1;
-    r.queueCount = 1;
-    r.activeQueueArraySize = fatbitSize(1);
-    r.handledKeyFatbitSize = fatbitSize(0);
-    r.minWidth = t.minLen;
-    r.minWidthExcludingBoundaries = t.minLen;
-    r.maxBiAnchoredWidth = ROSE_BOUND_INF;
-    r.floatingDistance = ROSE_BOUND_INF;
-    r.initialGroups = 0;
-    r.delay_fatbit_size = fatbitSize(0);
-    r.anchored_fatbit_size = fatbitSize(0);
-    r.outfixBeginQueue = 0;
-    r.outfixEndQueue = 1;
-    r.leftfixBeginQueue = 1;
-    r.initMpvNfa = 0xffffffffu;
-    r.scratchStateSize = (u32)HSB_ROUNDUP(hdr.scratchStateSize, 64); /* the queue's full state, in scratch */
-    StateOffsets &so = r.stateOffsets;
-    u32 cur = 1; /* status byte; no roles */
+/* Header fields that every route sets alike: report keys, widths, and the sizes of the
+ * runtime's (empty) delay / anchored / SOM / handled-key structures. */
+void commonHeader(RoseEngine *r, const RoseTail &t) {
+    r->canExhaust = t.canExhaust ? 1 : 0;
+    r->ekeyCount = t.ekeyCount;
+    r->dkeyCount = t.dkeyCount;
+    r->dkeyLogSize = fatbitSize(r->dkeyCount);
+    r->invDkeyOffset = t.invDkeyOffset;
+    r->somLocationFatbitSize = fatbitSize(0);
+    r->handledKeyFatbitSize = fatbitSize(0);
+    r->minWidth = t.minLen;
+    r->minWidthExcludingBoundaries = t.minLen;
+    r->maxBiAnchoredWidth = ROSE_BOUND_INF;
+    r->floatingDistance = ROSE_BOUND_INF;
+    r->delay_fatbit_size = fatbitSize(0);
+    r->anchored_fatbit_size = fatbitSize(0);
+    r->initMpvNfa = 0xffffffffu; /* MO_INVALID_IDX: no MPV outfix */
+}
+
+/* The state layout (fillStateOffsets, src/rose/rose_build_bytecode.cpp:382-465): the status byte
+ * (no roles), the active leaf array of `leafCount` engines, `groupsSize` bytes of literal groups,
+ * `history` bytes, then the exhaustion, logical and combination vectors.  Returns nfaStateBegin,
+ * where the engines' stream state goes. */
+u32 layoutState(RoseEngine *r, u32 leafCount, u32 groupsSize, u32 history) {
+    StateOffsets &so = r->stateOffsets;
+    u32 cur = 1;
     so.activeLeafArray = cur;
-    so.activeLeafArray_size = mmbitSize(1);
+    so.activeLeafArray_size = leafCount ? mmbitSize(leafCount) : 0;
     cur += so.activeLeafArray_size;
     so.activeLeftArray = so.longLitState = so.leftfixLagTable = so.anchorState = cur;
     so.groups = cur;
-    so.groups_size = 0;
+    so.groups_size = groupsSize;
+    cur += groupsSize;
     so.history = cur;
+    cur += history;
     so.exhausted = cur;
-    so.exhausted_size = mmbitSize(r.ekeyCount);
+    so.exhausted_size = mmbitSize(r->ekeyCount);
     cur += so.exhausted_size;
-    cur = layoutLogicalState(r, &so, cur);
-    so.nfaStateBegin = cur;
-    NfaInfo ni;
-    memset(&ni, 0, sizeof(ni));
-    ni.nfaOffset = nfaOffset;
-    ni.stateOffset = cur;
-    ni.fullStateOffset = 0;
-    cur += hdr.streamStateSize;
-    so.end = cur;
-    r.stateSize = cur;
-    r.nfaInfoOffset = blob.add(&ni, sizeof(ni), 4);
-    const u32 total = (u32)HSB_ROUNDUP(blob.base + blob.bytes.size(), 64);
-    r.size = total;
-    (void)opts;
-    std::vector<u8> out(total, 0);
-    memcpy(out.data(), &r, sizeof(r));
-    memcpy(out.data() + blob.base, blob.bytes.data(), blob.bytes.size());
-    return out;
+    cur = layoutLogicalState(*r, &so, cur);
+    so.nfaStateBegin = so.end = cur;
+    return cur;
 }
 
-/* Floating literal matcher + RoseEngine header around a finished program blob. */
-std::vector<u8> finishRose(Blob &blob, const std::vector<HwlmLit> &hl, const RoseTail &t,
-                           const CompileOpts &opts, HwlmBuildInfo *info) {
+/* The floating literal matcher (HWLM over `hl`), added to the blob; the header fields that
+ * describe it.  minLen: the shortest literal. */
+void addFloatingMatcher(Blob &blob, RoseEngine *r, const std::vector<HwlmLit> &hl, u32 minLen,
+                        const CompileOpts &opts, HwlmBuildInfo *info) {
     std::vector<u8> hwlm;
     try {
         hwlm = buildHwlm(hl, opts.hwlm, info);
     } catch (const std::runtime_error &e) {
         throw CompileError{std::string("Unable to build literal matcher: ") + e.what(), -1};
     }
-    const u32 fmatcherOffset = blob.add(hwlm.data(), hwlm.size(), 64);
-    RoseEngine r;
-    memset(&r, 0, sizeof(r));
-    writeLogicalInfo(blob, t.logic, &r);
+    r->fmatcherOffset = blob.add(hwlm.data(), hwlm.size(), 64);
+    r->fmatcherMinWidth = minLen;
+    r->floatingMinLiteralMatchOffset = minLen;
+    r->initialGroups = 1;
+    r->floating_group_mask = 1;
+    r->totalNumLiterals = (u32)hl.size();
+}
+
+/* Queue 0 holds the engine at nfaOffset (header hdr) as the database's only outfix: its NfaInfo,
+ * the queue counts, its full state in scratch and its stream state at `cur` (nfaStateBegin). */
+void addOutfixQueue(Blob &blob, RoseEngine *r, u32 nfaOffset, const NFA &hdr, u32 cur) {
+    r->activeArrayCount = 1;
+    r->queueCount = 1;
+    r->activeQueueArraySize = fatbitSize(1);
+    r->outfixBeginQueue = 0;
+    r->outfixEndQueue = 1;
+    r->leftfixBeginQueue = 1;
+    r->scratchStateSize = (u32)HSB_ROUNDUP(hdr.scratchStateSize, 64); /* the queue's full state, in scratch */
+    NfaInfo ni;
+    memset(&ni, 0, sizeof(ni));
+    ni.nfaOffset = nfaOffset;
+    ni.stateOffset = cur;
+    ni.fullStateOffset = 0;
+    cur += hdr.streamStateSize;
+    r->stateOffsets.end = cur;
+    r->stateSize = cur;
+    r->nfaInfoOffset = blob.add(&ni, sizeof(ni), 4);
+}
+
+/* header + blob, the header's size field set */
+std::vector<u8> emitRose(const Blob &blob, RoseEngine *r) {
     const u32 total = (u32)HSB_ROUNDUP(blob.base + blob.bytes.size(), 64);
-
-    /* --- header --- */
-    r.pureLiteral = opts.pureLiteralApi ? 1 : 0;
-    r.runtimeImpl = RUNTIME_PURE_LITERAL;
-    r.canExhaust = t.canExhaust ? 1 : 0;
-    /* src/rose/rose_build_bytecode.cpp:3615-3622 */
-    r.mode = !opts.streaming ? MODE_BLOCK : opts.vectored ? MODE_VECTORED : MODE_STREAM;
-    /* matches may start in earlier writes: keep the last maxLen-1 bytes
-     * (calcHistoryRequired, src/rose/rose_build_misc.cpp; updated by HWLM) */
-    const u32 historyRequired = opts.streaming && t.maxLen > 1 ? t.maxLen - 1 : 0;
-    r.historyRequired = historyRequired;
-    r.ekeyCount = t.ekeyCount;
-    r.dkeyCount = t.dkeyCount;
-    r.dkeyLogSize = fatbitSize(r.dkeyCount);
-    r.invDkeyOffset = t.invDkeyOffset;
-    r.somLocationFatbitSize = fatbitSize(0);
-    r.fmatcherOffset = fmatcherOffset;
-    r.smallWriteOffset = t.smallWriteOffset;
-    r.fmatcherMinWidth = t.minLen;
-    r.activeQueueArraySize = fatbitSize(0);
-    r.handledKeyFatbitSize = fatbitSize(0);
-    r.minWidth = t.minLen;
-    r.minWidthExcludingBoundaries = t.minLen;
-    r.maxBiAnchoredWidth = ROSE_BOUND_INF;
-    r.floatingDistance = ROSE_BOUND_INF;
-    r.floatingMinLiteralMatchOffset = t.minLen;
-    r.initialGroups = 1;
-    r.floating_group_mask = 1;
-    r.size = total;
-    r.delay_fatbit_size = fatbitSize(0);
-    r.anchored_fatbit_size = fatbitSize(0);
-    r.totalNumLiterals = (u32)hl.size();
-    r.initMpvNfa = 0xffffffffu; /* MO_INVALID_IDX: no MPV outfix */
-    StateOffsets &so = r.stateOffsets;
-    u32 cur = 1;                 /* status byte; role multibit is empty */
-    so.activeLeafArray = so.activeLeftArray = so.longLitState = cur;
-    so.leftfixLagTable = so.anchorState = cur;
-    so.groups = cur;
-    so.groups_size = 1;
-    cur += so.groups_size;
-    so.history = cur;
-    cur += historyRequired;
-    so.exhausted = cur;
-    so.exhausted_size = mmbitSize(r.ekeyCount);
-    cur += so.exhausted_size;
-    cur = layoutLogicalState(r, &so, cur);
-    so.nfaStateBegin = so.end = cur;
-
+    r->size = total;
     std::vector<u8> out(total, 0);
-    memcpy(out.data(), &r, sizeof(r));
+    memcpy(out.data(), r, sizeof(*r));
     memcpy(out.data() + blob.base, blob.bytes.data(), blob.bytes.size());
     return out;
 }
 
-} // namespace
+/* A database whose only matcher is ONE engine run as an outfix over the whole block
+ * (ROSE_RUNTIME_SINGLE_OUTFIX: hs_scan -> soleOutfixBlockExec, src/runtime.c:245-280): queue 0,
+ * no literal matchers.  What the reference's compiler emits for a pattern set that is all
+ * engine and no literal (rose_build_bytecode.cpp:3672-3690 pickRuntimeImpl); here it is built
+ * for literal sets on request, so that the DFA / NFA engines run inside a real database. */
+std::vector<u8> finishOutfixRose(Blob &blob, const std::vector<u8> &nfa, const RoseTail &t) {
+    NFA hdr;
+    memcpy(&hdr, nfa.data(), sizeof(hdr));
+    const u32 nfaOffset = blob.add(nfa.data(), nfa.size(), 64);
+    RoseEngine r;
+    memset(&r, 0, sizeof(r));
+    writeLogicalInfo(blob, t.logic, &r);
+    commonHeader(&r, t);
+    r.runtimeImpl = RUNTIME_SINGLE_OUTFIX;
+    r.mode = MODE_BLOCK;
+    addOutfixQueue(blob, &r, nfaOffset, hdr, layoutState(&r, 1, 0, 0));
+    return emitRose(blob, &r);
+}
 
-std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
-                                 const CompileOpts &opts, HwlmBuildInfo *info, LogicalSet *logic) {
+/* Floating literal matcher + RoseEngine header around a finished program blob. */
+std::vector<u8> finishRose(Blob &blob, const std::vector<HwlmLit> &hl, const RoseTail &t,
+                           const CompileOpts &opts, HwlmBuildInfo *info) {
+    RoseEngine r;
+    memset(&r, 0, sizeof(r));
+    addFloatingMatcher(blob, &r, hl, t.minLen, opts, info);
+    writeLogicalInfo(blob, t.logic, &r);
+    commonHeader(&r, t);
+    r.pureLiteral = opts.pureLiteralApi ? 1 : 0;
+    r.runtimeImpl = RUNTIME_PURE_LITERAL;
+    /* src/rose/rose_build_bytecode.cpp:3615-3622 */
+    r.mode = !opts.streaming ? MODE_BLOCK : opts.vectored ? MODE_VECTORED : MODE_STREAM;
+    /* matches may start in earlier writes: keep the last maxLen-1 bytes
+     * (calcHistoryRequired, src/rose/rose_build_misc.cpp; updated by HWLM) */
+    r.historyRequired = opts.streaming && t.maxLen > 1 ? t.maxLen - 1 : 0;
+    r.smallWriteOffset = t.smallWriteOffset;
+    r.activeQueueArraySize = fatbitSize(0);
+    layoutState(&r, 0, 1, r.historyRequired);
+    return emitRose(blob, &r);
+}
+
+/* A database with the floating literal matcher over `hl` AND one engine (`nfa`) as the outfix on
+ * queue 0 (ROSE_RUNTIME_FULL_ROSE; hs_scan -> roseBlockExec, src/rose/block.c:345-422):
+ * init_for_block clears the active leaf array through the state scatter plan, blockInitSufPQ
+ * starts the outfix, the literal programs' CATCH_UP and roseCatchUpTo(length) run it, and when it
+ * accepts at end of data the EOD program's ENGINES_EOD checks its final state (roseBlockEodExec).
+ * litMinLen: the shortest literal; t.minLen: the shortest match of either half. */
+std::vector<u8> finishMixedRose(Blob &blob, const std::vector<HwlmLit> &hl, u32 litMinLen, const std::vector<u8> &nfa,
+                                const RoseTail &t, const CompileOpts &opts, HwlmBuildInfo *info) {
+    RoseEngine r;
+    memset(&r, 0, sizeof(r));
+    addFloatingMatcher(blob, &r, hl, litMinLen, opts, info);
+    NFA hdr;
+    memcpy(&hdr, nfa.data(), sizeof(hdr));
+    const u32 nfaOffset = blob.add(nfa.data(), nfa.size(), 64);
+    commonHeader(&r, t);
+    r.runtimeImpl = RUNTIME_FULL_ROSE;
+    r.mode = MODE_BLOCK;
+    /* no bi-anchored patterns (findMaxBAWidth): roseBlockFloating scans blocks of any length */
+    r.amatcherMaxBiAnchoredWidth = ROSE_BOUND_INF;
+    r.fmatcherMaxBiAnchoredWidth = ROSE_BOUND_INF;
+    const u32 cur = layoutState(&r, 1, 1, 0);
+    if (hdr.flags & NFA_ACCEPTS_EOD) {
+        /* makeEodProgram (rose_build_bytecode.cpp:3334-3350) with only addEnginesEodProgram: ENGINES_EOD over
+         * a sparse iterator of the queues that accept at EOD (buildEodNfaIterator: queue 0 of 1) */
+        const MmbSparseIter it = {1, 0};
+        const u32 iter = blob.add(&it, sizeof(it), alignof(MmbSparseIter));
+        const u32 prog = blob.reserve(instrSize<InstrEnginesEod>() + instrSize<InstrEnd>(), INSTR_ALIGN);
+        InstrEnginesEod ee;
+        memset(&ee, 0, sizeof(ee));
+        ee.code = OP_ENGINES_EOD;
+        ee.iter_offset = iter;
+        memcpy(blob.at(prog), &ee, sizeof(ee));
+        *blob.at(prog + instrSize<InstrEnginesEod>()) = OP_END;
+        r.eodProgramOffset = prog;
+        r.requiresEodCheck = 1; /* hasEodAnchors (:2446-2475): an outfix accepts at EOD */
+    }
+    /* the state scatter plan of a block-mode database (buildStateScatterPlan, rose_build_scatter.cpp:66-97):
+     * no roles and no leftfixes, so one byte that clears the one-bit active leaf array */
+    const ScatterUnitU8 clearLeaf = {r.stateOffsets.activeLeafArray, 0};
+    r.state_init.s_u8_offset = blob.add(&clearLeaf, sizeof(clearLeaf), alignof(ScatterUnitU8));
+    r.state_init.s_u8_count = 1;
+    addOutfixQueue(blob, &r, nfaOffset, hdr, cur);
+    return emitRose(blob, &r);
+}
+
+/* report id -> (HS_FLAG_SINGLEMATCH, index of the first expression with it) */
+typedef std::map<u32, std::pair<bool, u32>> HighlanderMap;
+
+/* Every expression with one report id must agree on HS_FLAG_SINGLEMATCH (src/compiler/compiler.cpp). */
+void checkHighlander(HighlanderMap *seen, u32 report, bool single, u32 index) {
+    auto it = seen->find(report);
+    if (it == seen->end()) {
+        (*seen)[report] = {single, index};
+    } else if (it->second.first != single) {
+        std::string m = "Expression (index " + std::to_string(index) + ") with match ID " + std::to_string(report) + " ";
+        m += single ? "specified " : "did not specify ";
+        m += "HS_FLAG_SINGLEMATCH whereas previous expression (index " + std::to_string(it->second.second) +
+             ") with the same match ID did";
+        m += single ? " not." : ".";
+        throw CompileError{m, (int)index};
+    }
+}
+
+/* The literal set validated, case-folded and without exact duplicates; keys not yet assigned. */
+std::vector<PatInfo> prepareLiterals(const std::vector<LitPattern> &patsIn, const CompileOpts &opts,
+                                     HighlanderMap *idHighlander) {
     if (patsIn.empty()) {
         throw CompileError{"Invalid parameter: elements is zero", -1};
     }
     if (patsIn.size() > LIMIT_LITERAL_COUNT) {
         throw CompileError{"Number of patterns too large", -1};
     }
-
-    /* --- validate, fold case, drop exact duplicates, assign ekeys/dkeys --- */
     std::vector<PatInfo> pats;
-    std::map<u32, std::pair<bool, u32>> idHighlander; /* report -> (flag, first index) */
     std::set<std::tuple<std::string, bool, u32>> seen;
     for (const LitPattern &p : patsIn) {
         if (p.s.empty()) {
@@ -418,18 +473,7 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
             throw CompileError{"Streaming and vectored modes in this build support literals of up to 8 "
                                "bytes; longer literals need the long literal table.", (int)p.index};
         }
-        auto it = idHighlander.find(p.report);
-        if (it == idHighlander.end()) {
-            idHighlander[p.report] = {p.singlematch, p.index};
-        } else if (it->second.first != p.singlematch) {
-            std::string m = "Expression (index " + std::to_string(p.index) +
-                            ") with match ID " + std::to_string(p.report) + " ";
-            m += p.singlematch ? "specified " : "did not specify ";
-            m += "HS_FLAG_SINGLEMATCH whereas previous expression (index " +
-                 std::to_string(it->second.second) + ") with the same match ID did";
-            m += p.singlematch ? " not." : ".";
-            throw CompileError{m, (int)p.index};
-        }
+        checkHighlander(idHighlander, p.report, p.singlematch, p.index);
         PatInfo pi;
         pi.p = &p;
         pi.folded = p.s;
@@ -449,11 +493,23 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
         pi.ekey = pi.dkey = INVALID_EKEY;
         pats.push_back(pi);
     }
+    return pats;
+}
+
+/* Exhaustion keys for the HS_FLAG_SINGLEMATCH ids, dedupe keys for ids that more than one pattern
+ * raises -- or that `engineIds` (the ids an engine raises too) holds.  Returns whether every
+ * pattern is single-match. */
+bool assignLiteralKeys(std::vector<PatInfo> *patsIo, const std::set<u32> &engineIds, std::map<u32, u32> *ekeysOut,
+                       std::map<u32, u32> *dkeysOut) {
+    std::vector<PatInfo> &pats = *patsIo;
+    std::map<u32, u32> &ekeys = *ekeysOut, &dkeys = *dkeysOut;
     std::map<u32, u32> perReport;
     for (const auto &pi : pats) {
         perReport[pi.p->report]++;
     }
-    std::map<u32, u32> ekeys, dkeys;
+    for (u32 id : engineIds) {
+        perReport[id]++;
+    }
     bool allHighlander = true;
     for (auto &pi : pats) {
         const u32 r = pi.p->report;
@@ -474,68 +530,16 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
             pi.dkey = it->second;
         }
     }
-    assignCombinationEkeys(logic, &ekeys);
+    return allHighlander;
+}
 
-    if (opts.outfixKind) {
-        /* --- single-outfix database: report programs ([CHECK_EXHAUSTED] [DEDUPE] REPORT_EXHAUST |
-         * DEDUPE_AND_REPORT | REPORT, END -- run by roseReportAdaptor / roseRunProgram), one engine
-         * over the whole literals whose reports are those programs' offsets --- */
-        if (opts.streaming) {
-            throw CompileError{"Single-engine databases are built for block mode only.", -1};
-        }
-        Blob blob((u32)HSB_ROUNDUP(sizeof(RoseEngine), 64));
-        std::vector<DfaLiteral> dl;
-        u32 minLen = ~0u, maxLen = 0;
-        for (const PatInfo &pi : pats) {
-            minLen = std::min<u32>(minLen, (u32)pi.p->s.size());
-            maxLen = std::max<u32>(maxLen, (u32)pi.p->s.size());
-            const u32 sz = reportSize(pi, logic) + instrSize<InstrEnd>();
-            const u32 prog = blob.reserve(sz, INSTR_ALIGN), endAt = prog + sz - instrSize<InstrEnd>();
-            writeReport(blob, prog, pi, endAt, logic);
-            InstrEnd e;
-            e.code = OP_END;
-            memcpy(blob.at(endAt), &e, sizeof(e));
-            DfaLiteral l;
-            l.s = pi.p->s;
-            l.caseless = pi.p->caseless && pi.anyAlpha;
-            l.report = prog;
-            dl.push_back(l);
-        }
-        RoseTail t;
-        t.minLen = minLen;
-        t.maxLen = maxLen;
-        t.ekeyCount = (u32)ekeys.size();
-        t.dkeyCount = (u32)dkeys.size();
-        t.invDkeyOffset = 0;
-        if (!dkeys.empty()) {
-            std::vector<u32> inv(dkeys.size());
-            for (const auto &d : dkeys) {
-                inv[d.second] = d.first;
-            }
-            t.invDkeyOffset = blob.add(inv.data(), inv.size() * sizeof(u32), 4);
-        }
-        t.canExhaust = allHighlander;
-        t.logic = logic;
-        std::vector<u8> nfa;
-        try {
-            if (opts.outfixKind == OUTFIX_LIMEX32) {
-                nfa = emitLimEx(nfaFromLiterals(dl));
-            } else {
-                const DfaKind k = opts.outfixKind == OUTFIX_MCCLELLAN8    ? DFA_MCCLELLAN8
-                                  : opts.outfixKind == OUTFIX_MCCLELLAN16 ? DFA_MCCLELLAN16
-                                  : opts.outfixKind == OUTFIX_SHENG       ? DFA_SHENG
-                                                                          : DFA_AUTO;
-                nfa = emitDfa(dfaFromLiterals(dl, false), k, false);
-            }
-        } catch (const std::runtime_error &e) {
-            throw CompileError{std::string("Unable to build the engine: ") + e.what(), -1};
-        }
-        if (info) {
-            memset(info, 0, sizeof(*info));
-        }
-        return finishOutfixRose(blob, nfa, t, opts);
-    }
-
+/* The literal programs, one per fragment (literals grouped by their 8-byte suffix and effective
+ * case), added to the blob; returns the floating matcher's literals (ids = program offsets).
+ * catchUp: each report block starts with CATCH_UP (makeCatchup, src/rose/rose_build_program.cpp:412-434),
+ * as in a database with an outfix (needsCatchup, src/rose/rose_build_bytecode.cpp:226). */
+std::vector<HwlmLit> writeLiteralPrograms(Blob &blob, const std::vector<PatInfo> &pats, const LogicalSet *logic,
+                                          bool catchUp, u32 *minLen, u32 *maxLen) {
+    const u32 catchUpSize = catchUp ? instrSize<InstrCatchUp>() : 0;
     /* --- group into fragments by (8-byte suffix, effective nocase) --- */
     struct Fragment {
         std::string suffix;
@@ -545,10 +549,8 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
     };
     std::vector<Fragment> frags;
     std::map<std::pair<std::string, bool>, u32> fragIndex;
-    u32 minLen = ~0u;
     for (u32 i = 0; i < pats.size(); i++) {
         const std::string &f = pats[i].folded;
-        minLen = std::min<u32>(minLen, (u32)f.size());
         std::string suf = f.size() > 8 ? f.substr(f.size() - 8) : f;
         bool nc = false;
         if (pats[i].p->caseless) {
@@ -566,8 +568,6 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
     }
 
     /* --- programs --- */
-    const u32 blobBase = (u32)HSB_ROUNDUP(sizeof(RoseEngine), 64);
-    Blob blob(blobBase);
     struct PendingLit {
         u32 instrOff;
         std::string bytes;
@@ -576,14 +576,14 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
     for (Fragment &fr : frags) {
         u32 total = instrSize<InstrEnd>();
         for (u32 pi : fr.pats) {
-            total += blockSize(pats[pi], logic);
+            total += blockSize(pats[pi], logic) + catchUpSize;
         }
         const u32 start = blob.reserve(total, INSTR_ALIGN);
         fr.program = start;
         u32 pc = start;
         for (size_t k = 0; k < fr.pats.size(); k++) {
             const PatInfo &pi = pats[fr.pats[k]];
-            const u32 next = pc + blockSize(pi, logic); /* next pattern's block or END */
+            const u32 next = pc + blockSize(pi, logic) + catchUpSize; /* next pattern's block or END */
             if (pi.p->s.size() > 8) {
                 InstrCheckLit in;
                 memset(&in, 0, sizeof(in));
@@ -594,6 +594,10 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
                 memcpy(blob.at(pc), &in, sizeof(in));
                 pendingLits.push_back({pc, pi.folded});
                 pc += instrSize<InstrCheckLit>();
+            }
+            if (catchUp) {
+                *blob.at(pc) = OP_CATCH_UP;
+                pc += catchUpSize;
             }
             writeReport(blob, pc, pi, next, logic);
             pc = next;
@@ -610,18 +614,8 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
         memcpy(blob.at(pl.instrOff), &in, sizeof(in));
     }
 
-    /* --- dkey -> external report id table (rose_internal.h:354) --- */
-    u32 invDkeyOffset = 0;
-    if (!dkeys.empty()) {
-        std::vector<u32> inv(dkeys.size());
-        for (const auto &d : dkeys) {
-            inv[d.second] = d.first;
-        }
-        invDkeyOffset = blob.add(inv.data(), inv.size() * sizeof(u32), 4);
-    }
-
-    /* --- floating literal matcher --- */
     std::vector<HwlmLit> hl;
+    /* --- the floating matcher's literals --- */
     for (const Fragment &fr : frags) {
         HwlmLit l;
         l.s = fr.suffix;
@@ -631,111 +625,55 @@ std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
         l.groups = 1;
         hl.push_back(l);
     }
-    u32 maxLen = 0;
+    *minLen = ~0u;
+    *maxLen = 0;
     for (const auto &pi : pats) {
-        maxLen = std::max<u32>(maxLen, (u32)pi.folded.size());
+        *minLen = std::min<u32>(*minLen, (u32)pi.folded.size());
+        *maxLen = std::max<u32>(*maxLen, (u32)pi.folded.size());
     }
-    RoseTail t;
-    t.minLen = minLen;
-    t.maxLen = maxLen;
-    t.ekeyCount = (u32)ekeys.size();
-    t.dkeyCount = (u32)dkeys.size();
-    t.invDkeyOffset = invDkeyOffset;
-    t.canExhaust = allHighlander;
-    t.logic = logic;
-
-    /* --- small-write engine (src/smallwrite/smallwrite_build.cpp; used by hs_scan for
-     * buffers shorter than largestBuffer, src/runtime.c:401-413): one DFA over the WHOLE
-     * literals whose reports are the offsets of report programs -- the literal's program
-     * without the literal check, which the DFA has already done -- run through
-     * roseReportAdaptor (src/rose/match.c:611-633).  Only while the automaton stays small
-     * (12 000 literal bytes, 16 K states); otherwise no engine, like the reference when its
-     * DFA limits are exceeded. --- */
-    if (opts.smallWrite && !opts.streaming) {
-        const u32 LARGEST_BUFFER = 70; /* Grey::smallWriteLargestBuffer, src/grey.cpp:135 */
-        std::vector<DfaLiteral> dl;
-        size_t budget = 0;
-        bool ok = true;
-        for (const PatInfo &pi : pats) {
-            if (pi.p->s.size() >= LARGEST_BUFFER) {
-                continue; /* cannot match in a buffer that short */
-            }
-            const bool nc = pi.p->caseless && pi.anyAlpha;
-            budget += pi.p->s.size();
-            if (budget > 12000) { /* positions of the automaton; it may still grow past 16 K states */
-                ok = false;
-                break;
-            }
-            /* report program: [CHECK_EXHAUSTED] [DEDUPE] REPORT_EXHAUST | DEDUPE_AND_REPORT | REPORT, END */
-            const u32 sz = reportSize(pi, logic) + instrSize<InstrEnd>();
-            const u32 prog = blob.reserve(sz, INSTR_ALIGN), endAt = prog + sz - instrSize<InstrEnd>();
-            writeReport(blob, prog, pi, endAt, logic);
-            InstrEnd e;
-            e.code = OP_END;
-            memcpy(blob.at(endAt), &e, sizeof(e));
-            DfaLiteral l;
-            l.s = pi.p->s;
-            l.caseless = nc;
-            l.report = prog;
-            dl.push_back(l);
-        }
-        if (ok && !dl.empty()) {
-            try {
-                const std::vector<u8> nfa = emitDfa(dfaFromLiterals(dl, false), DFA_AUTO, false);
-                SmallWriteEngine sw;
-                memset(&sw, 0, sizeof(sw));
-                sw.largestBuffer = LARGEST_BUFFER;
-                sw.start_offset = 0;
-                sw.size = (u32)(sizeof(SmallWriteEngine) + nfa.size());
-                t.smallWriteOffset = blob.add(&sw, sizeof(sw), 64);
-                blob.add(nfa.data(), nfa.size(), 64);
-            } catch (const std::runtime_error &) {
-                /* automaton too large: no small-write engine */
-            }
-        }
-    }
-    return finishRose(blob, hl, t, opts, info);
+    return hl;
 }
 
-std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const CompileOpts &opts, LogicalSet *logic) {
-    if (pats.empty()) {
-        throw CompileError{"Invalid parameter: elements is zero", -1};
+/* the dkey -> external report id table (rose_internal.h:354), or 0 without dedupe keys */
+u32 addInvDkeys(Blob &blob, const std::map<u32, u32> &dkeys) {
+    if (dkeys.empty()) {
+        return 0;
     }
-    if (opts.streaming) {
-        throw CompileError{"Expressions that need an NFA engine are compiled for block mode only in this build.", -1};
+    std::vector<u32> inv(dkeys.size());
+    for (const auto &d : dkeys) {
+        inv[d.second] = d.first;
     }
-    /* report keys: one exhaustion key per HS_FLAG_SINGLEMATCH report id; one dedupe key per report
-     * id, always -- several accepting positions (or expressions) may raise one id at one offset and
-     * the reference delivers a report once (dedupe, src/report.h:55-119) */
-    std::map<u32, std::pair<bool, u32>> highlander;
-    std::map<u32, u32> ekeys, dkeys;
+    return blob.add(inv.data(), inv.size() * sizeof(u32), 4);
+}
+
+/* Report keys of the expressions: one exhaustion key per HS_FLAG_SINGLEMATCH report id; one dedupe key per report
+ * id, always -- several accepting positions (or expressions) may raise one id at one offset and
+ * the reference delivers a report once (dedupe, src/report.h:55-119) */
+bool assignRegexKeys(const std::vector<RegexPattern> &pats, HighlanderMap *highlander, std::map<u32, u32> *ekeys,
+                     std::map<u32, u32> *dkeys) {
     bool allHighlander = true;
     for (const RegexPattern &p : pats) {
         const bool single = (p.flags & HS_FLAG_SINGLEMATCH) != 0;
-        auto it = highlander.find(p.report);
-        if (it == highlander.end()) {
-            highlander[p.report] = {single, p.index};
-        } else if (it->second.first != single) {
-            std::string m = "Expression (index " + std::to_string(p.index) + ") with match ID " +
-                            std::to_string(p.report) + " ";
-            m += single ? "specified " : "did not specify ";
-            m += "HS_FLAG_SINGLEMATCH whereas previous expression (index " + std::to_string(it->second.second) +
-                 ") with the same match ID did";
-            m += single ? " not." : ".";
-            throw CompileError{m, (int)p.index};
-        }
+        checkHighlander(highlander, p.report, single, p.index);
         if (single) {
-            ekeys.emplace(p.report, (u32)ekeys.size());
+            ekeys->emplace(p.report, (u32)ekeys->size());
         } else {
             allHighlander = false;
         }
-        dkeys.emplace(p.report, (u32)dkeys.size());
+        dkeys->emplace(p.report, (u32)dkeys->size());
     }
-    assignCombinationEkeys(logic, &ekeys);
-    Blob blob((u32)HSB_ROUNDUP(sizeof(RoseEngine), 64));
+    return allHighlander;
+}
+
+/* The report programs of the expressions (added to the blob) and ONE engine over all of them, whose
+ * reports are those programs' offsets: McClellan-8 / 16 when the determinised automaton stays small
+ * and `opts.regexDfa`, else LimEx.  *minLen: the shortest match. */
+std::vector<u8> buildRegexEngine(Blob &blob, const std::vector<RegexPattern> &pats, std::map<u32, u32> &ekeys,
+                                 std::map<u32, u32> &dkeys, const LogicalSet *logic, const CompileOpts &opts,
+                                 u32 *minLen) {
     RawNfa nfa;
     regexNfaInit(&nfa);
-    u32 minLen = ~0u;
+    *minLen = ~0u;
     std::map<std::tuple<u32, int, u64, u64>, u32> progOf; /* (report id, offset_adjust, bounds) -> its report program */
     auto program = [&](const RegexPattern &p, int adjust) -> u32 {
         const auto key = std::make_tuple(p.report, adjust, p.minOffset, p.maxOffset);
@@ -863,12 +801,175 @@ std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const Comp
                     }
                 }
             }
-            minLen = std::min<u32>(minLen, (u32)std::max<u64>(ri.minLen, std::min<u64>(p.minLength, 0xffffffffu)));
+            *minLen = std::min<u32>(*minLen, (u32)std::max<u64>(ri.minLen, std::min<u64>(p.minLength, 0xffffffffu)));
             regexNfaAdd(&nfa, p.re.c_str(), p.flags, program(p, 0), ri.needsAdjust ? program(p, -1) : 0, p.minLength);
         } catch (const RegexError &e) {
             throw CompileError{e.msg, (int)p.index};
         }
     }
+    try {
+        /* small automata run as DFAs, as in the reference (ng_mcclellan before LimEx); the report programs are
+         * the same either way */
+        RawDfa dfa;
+        bool asDfa = opts.regexDfa && determinize(nfa, 1024, &dfa);
+        if (asDfa) {
+            minimizeDfa(&dfa);
+            /* (nothing left but the dead state: an expression set that cannot match; it stays an NFA) */
+            asDfa = dfa.size() >= 2 && dfa.size() <= 1024;
+        }
+        if (asDfa) {
+            return emitDfa(dfa, dfa.size() <= 256 ? DFA_MCCLELLAN8 : DFA_MCCLELLAN16, true);
+        } else {
+            return emitLimEx(nfa);
+        }
+    } catch (const std::runtime_error &e) {
+        throw CompileError{std::string("Unable to build the NFA: ") + e.what(), -1};
+    }
+}
+
+} // namespace
+
+std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
+                                 const CompileOpts &opts, HwlmBuildInfo *info, LogicalSet *logic) {
+    HighlanderMap highlander;
+    std::vector<PatInfo> pats = prepareLiterals(patsIn, opts, &highlander);
+    std::map<u32, u32> ekeys, dkeys;
+    const bool allHighlander = assignLiteralKeys(&pats, std::set<u32>(), &ekeys, &dkeys);
+    assignCombinationEkeys(logic, &ekeys);
+
+    if (opts.outfixKind) {
+        /* --- single-outfix database: report programs ([CHECK_EXHAUSTED] [DEDUPE] REPORT_EXHAUST |
+         * DEDUPE_AND_REPORT | REPORT, END -- run by roseReportAdaptor / roseRunProgram), one engine
+         * over the whole literals whose reports are those programs' offsets --- */
+        if (opts.streaming) {
+            throw CompileError{"Single-engine databases are built for block mode only.", -1};
+        }
+        Blob blob((u32)HSB_ROUNDUP(sizeof(RoseEngine), 64));
+        std::vector<DfaLiteral> dl;
+        u32 minLen = ~0u, maxLen = 0;
+        for (const PatInfo &pi : pats) {
+            minLen = std::min<u32>(minLen, (u32)pi.p->s.size());
+            maxLen = std::max<u32>(maxLen, (u32)pi.p->s.size());
+            const u32 sz = reportSize(pi, logic) + instrSize<InstrEnd>();
+            const u32 prog = blob.reserve(sz, INSTR_ALIGN), endAt = prog + sz - instrSize<InstrEnd>();
+            writeReport(blob, prog, pi, endAt, logic);
+            InstrEnd e;
+            e.code = OP_END;
+            memcpy(blob.at(endAt), &e, sizeof(e));
+            DfaLiteral l;
+            l.s = pi.p->s;
+            l.caseless = pi.p->caseless && pi.anyAlpha;
+            l.report = prog;
+            dl.push_back(l);
+        }
+        RoseTail t;
+        t.minLen = minLen;
+        t.maxLen = maxLen;
+        t.ekeyCount = (u32)ekeys.size();
+        t.dkeyCount = (u32)dkeys.size();
+        t.invDkeyOffset = addInvDkeys(blob, dkeys);
+        t.canExhaust = allHighlander;
+        t.logic = logic;
+        std::vector<u8> nfa;
+        try {
+            if (opts.outfixKind == OUTFIX_LIMEX32) {
+                nfa = emitLimEx(nfaFromLiterals(dl));
+            } else {
+                const DfaKind k = opts.outfixKind == OUTFIX_MCCLELLAN8    ? DFA_MCCLELLAN8
+                                  : opts.outfixKind == OUTFIX_MCCLELLAN16 ? DFA_MCCLELLAN16
+                                  : opts.outfixKind == OUTFIX_SHENG       ? DFA_SHENG
+                                                                          : DFA_AUTO;
+                nfa = emitDfa(dfaFromLiterals(dl, false), k, false);
+            }
+        } catch (const std::runtime_error &e) {
+            throw CompileError{std::string("Unable to build the engine: ") + e.what(), -1};
+        }
+        if (info) {
+            memset(info, 0, sizeof(*info));
+        }
+        return finishOutfixRose(blob, nfa, t);
+    }
+
+    Blob blob((u32)HSB_ROUNDUP(sizeof(RoseEngine), 64));
+    u32 minLen = 0, maxLen = 0;
+    const std::vector<HwlmLit> hl = writeLiteralPrograms(blob, pats, logic, false, &minLen, &maxLen);
+    const u32 invDkeyOffset = addInvDkeys(blob, dkeys);
+    RoseTail t;
+    t.minLen = minLen;
+    t.maxLen = maxLen;
+    t.ekeyCount = (u32)ekeys.size();
+    t.dkeyCount = (u32)dkeys.size();
+    t.invDkeyOffset = invDkeyOffset;
+    t.canExhaust = allHighlander;
+    t.logic = logic;
+
+    /* --- small-write engine (src/smallwrite/smallwrite_build.cpp; used by hs_scan for
+     * buffers shorter than largestBuffer, src/runtime.c:401-413): one DFA over the WHOLE
+     * literals whose reports are the offsets of report programs -- the literal's program
+     * without the literal check, which the DFA has already done -- run through
+     * roseReportAdaptor (src/rose/match.c:611-633).  Only while the automaton stays small
+     * (12 000 literal bytes, 16 K states); otherwise no engine, like the reference when its
+     * DFA limits are exceeded. --- */
+    if (opts.smallWrite && !opts.streaming) {
+        const u32 LARGEST_BUFFER = 70; /* Grey::smallWriteLargestBuffer, src/grey.cpp:135 */
+        std::vector<DfaLiteral> dl;
+        size_t budget = 0;
+        bool ok = true;
+        for (const PatInfo &pi : pats) {
+            if (pi.p->s.size() >= LARGEST_BUFFER) {
+                continue; /* cannot match in a buffer that short */
+            }
+            const bool nc = pi.p->caseless && pi.anyAlpha;
+            budget += pi.p->s.size();
+            if (budget > 12000) { /* positions of the automaton; it may still grow past 16 K states */
+                ok = false;
+                break;
+            }
+            /* report program: [CHECK_EXHAUSTED] [DEDUPE] REPORT_EXHAUST | DEDUPE_AND_REPORT | REPORT, END */
+            const u32 sz = reportSize(pi, logic) + instrSize<InstrEnd>();
+            const u32 prog = blob.reserve(sz, INSTR_ALIGN), endAt = prog + sz - instrSize<InstrEnd>();
+            writeReport(blob, prog, pi, endAt, logic);
+            InstrEnd e;
+            e.code = OP_END;
+            memcpy(blob.at(endAt), &e, sizeof(e));
+            DfaLiteral l;
+            l.s = pi.p->s;
+            l.caseless = nc;
+            l.report = prog;
+            dl.push_back(l);
+        }
+        if (ok && !dl.empty()) {
+            try {
+                const std::vector<u8> nfa = emitDfa(dfaFromLiterals(dl, false), DFA_AUTO, false);
+                SmallWriteEngine sw;
+                memset(&sw, 0, sizeof(sw));
+                sw.largestBuffer = LARGEST_BUFFER;
+                sw.start_offset = 0;
+                sw.size = (u32)(sizeof(SmallWriteEngine) + nfa.size());
+                t.smallWriteOffset = blob.add(&sw, sizeof(sw), 64);
+                blob.add(nfa.data(), nfa.size(), 64);
+            } catch (const std::runtime_error &) {
+                /* automaton too large: no small-write engine */
+            }
+        }
+    }
+    return finishRose(blob, hl, t, opts, info);
+}
+
+std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const CompileOpts &opts, LogicalSet *logic) {
+    if (pats.empty()) {
+        throw CompileError{"Invalid parameter: elements is zero", -1};
+    }
+    if (opts.streaming) {
+        throw CompileError{"Expressions that need an NFA engine are compiled for block mode only in this build.", -1};
+    }
+    HighlanderMap highlander;
+    std::map<u32, u32> ekeys, dkeys;
+    const bool allHighlander = assignRegexKeys(pats, &highlander, &ekeys, &dkeys);
+    assignCombinationEkeys(logic, &ekeys);
+    Blob blob((u32)HSB_ROUNDUP(sizeof(RoseEngine), 64));
+    u32 minLen = 0;
+    const std::vector<u8> eng = buildRegexEngine(blob, pats, ekeys, dkeys, logic, opts, &minLen);
     RoseTail t;
     t.minLen = minLen;
     t.maxLen = 0;
@@ -881,26 +982,36 @@ std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const Comp
     t.invDkeyOffset = blob.add(inv.data(), inv.size() * sizeof(u32), 4);
     t.canExhaust = allHighlander;
     t.logic = logic;
-    std::vector<u8> eng;
-    try {
-        /* small automata run as DFAs, as in the reference (ng_mcclellan before LimEx); the report programs are
-         * the same either way */
-        RawDfa dfa;
-        bool asDfa = opts.regexDfa && determinize(nfa, 1024, &dfa);
-        if (asDfa) {
-            minimizeDfa(&dfa);
-            /* (nothing left but the dead state: an expression set that cannot match; it stays an NFA) */
-            asDfa = dfa.size() >= 2 && dfa.size() <= 1024;
-        }
-        if (asDfa) {
-            eng = emitDfa(dfa, dfa.size() <= 256 ? DFA_MCCLELLAN8 : DFA_MCCLELLAN16, true);
-        } else {
-            eng = emitLimEx(nfa);
-        }
-    } catch (const std::runtime_error &e) {
-        throw CompileError{std::string("Unable to build the NFA: ") + e.what(), -1};
+    return finishOutfixRose(blob, eng, t);
+}
+
+std::vector<u8> buildMixedRose(const std::vector<LitPattern> &lits, const std::vector<RegexPattern> &regexes,
+                               const CompileOpts &opts, HwlmBuildInfo *info) {
+    if (regexes.empty() || opts.streaming) {
+        throw CompileError{"A literal matcher with an engine is built for block mode only.", -1};
     }
-    return finishOutfixRose(blob, eng, t, opts);
+    /* one report id is one exhaustion key and one dedupe key, whichever half raises it */
+    HighlanderMap highlander;
+    std::vector<PatInfo> pats = prepareLiterals(lits, opts, &highlander);
+    std::set<u32> engineIds;
+    for (const RegexPattern &p : regexes) {
+        engineIds.insert(p.report);
+    }
+    std::map<u32, u32> ekeys, dkeys;
+    const bool litHighlander = assignLiteralKeys(&pats, engineIds, &ekeys, &dkeys);
+    const bool regexHighlander = assignRegexKeys(regexes, &highlander, &ekeys, &dkeys);
+    Blob blob((u32)HSB_ROUNDUP(sizeof(RoseEngine), 64));
+    u32 litMin = 0, litMax = 0, regexMin = 0;
+    const std::vector<HwlmLit> hl = writeLiteralPrograms(blob, pats, nullptr, true, &litMin, &litMax);
+    const std::vector<u8> eng = buildRegexEngine(blob, regexes, ekeys, dkeys, nullptr, opts, &regexMin);
+    RoseTail t;
+    t.minLen = std::min(litMin, regexMin);
+    t.maxLen = litMax;
+    t.ekeyCount = (u32)ekeys.size();
+    t.dkeyCount = (u32)dkeys.size();
+    t.invDkeyOffset = addInvDkeys(blob, dkeys);
+    t.canExhaust = litHighlander && regexHighlander;
+    return finishMixedRose(blob, hl, litMin, eng, t, opts, info);
 }
 
 /* Test hook (hs_b200_test_compile_programs): a pure-literal block database whose

@@ -3,7 +3,9 @@
  * (programs + floating literal matcher) and the hs_database container.
  * Stands where the reference's RoseBuildImpl::buildFinalEngine + dbCreate stand
  * (src/rose/rose_build_bytecode.cpp:3609-3888, src/compiler/compiler.cpp:476-
- * 536), restricted to databases whose runtimeImpl is ROSE_RUNTIME_PURE_LITERAL.
+ * 536), restricted to databases whose runtimeImpl is ROSE_RUNTIME_PURE_LITERAL,
+ * ROSE_RUNTIME_SINGLE_OUTFIX, or ROSE_RUNTIME_FULL_ROSE with only the floating
+ * literal matcher and one outfix.
  */
 #ifndef HSB200_ROSE_BUILD_H
 #define HSB200_ROSE_BUILD_H
@@ -75,6 +77,13 @@ struct RegexPattern {
 };
 std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const CompileOpts &opts,
                                LogicalSet *logic = nullptr);
+
+/** A set of literals AND expressions that need an engine (ROSE_RUNTIME_FULL_ROSE): the floating
+ * literal matcher over `lits`, whose programs catch the outfix up before they report, and ONE
+ * engine over `regexes` as the outfix on queue 0.  Report ids share their exhaustion and dedupe
+ * keys across both halves.  Block mode only; no logical combinations.  Throws CompileError. */
+std::vector<u8> buildMixedRose(const std::vector<LitPattern> &lits, const std::vector<RegexPattern> &regexes,
+                               const CompileOpts &opts, HwlmBuildInfo *info);
 
 /** Test hook: pure-literal block database from raw literal programs (`area`
  * is placed at programAreaBase(); lits[i].id = its program's offset in area). */

@@ -315,6 +315,7 @@ enum RoseOp {
     OP_CHECK_MASK = 9,
     OP_CHECK_MASK_32 = 10,
     OP_CHECK_BYTE = 11,
+    OP_CATCH_UP = 20,
     OP_DEDUPE = 28,
     OP_REPORT = 33,
     OP_REPORT_EXHAUST = 34,
@@ -322,6 +323,7 @@ enum RoseOp {
     OP_FINAL_REPORT = 38,
     OP_CHECK_EXHAUSTED = 39,
     OP_SQUASH_GROUPS = 43,
+    OP_ENGINES_EOD = 48,
     OP_CHECK_LONG_LIT = 51,
     OP_CHECK_LONG_LIT_NOCASE = 52,
     OP_CHECK_MED_LIT = 53,
@@ -362,6 +364,13 @@ struct InstrSetLogical { u8 code; u32 lkey; s32 offset_adjust; };
 struct InstrSetCombination { u8 code; u32 ckey; };
 struct InstrFlushCombination { u8 code; };
 struct InstrLastFlushCombination { u8 code; };
+struct InstrCatchUp { u8 code; };
+struct InstrEnginesEod { u8 code; u32 iter_offset; }; /* iter_offset: an MmbSparseIter over the queues */
+
+/* one record of a sparse multibit iterator (struct mmbit_sparse_iter, src/util/multibit_internal.h:59-62) */
+struct MmbSparseIter { u64 mask; u32 val; };
+/* one byte of a state scatter plan (struct scatter_unit_u8, src/util/scatter.h) */
+struct ScatterUnitU8 { u32 offset; u8 val; };
 
 /* ---- logical combinations: src/util/logical.h:42-72 -------------------- */
 

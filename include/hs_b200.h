@@ -136,6 +136,9 @@ typedef int (*match_event_handler)(unsigned int id, unsigned long long from,
  * mode, to ONE engine -- a McClellan DFA when the determinised automaton is small, else a LimEx NFA (32- to
  * 512-state model) -- inside a single-outfix database
  * (ROSE_RUNTIME_SINGLE_OUTFIX) when its positions fit -- DESIGN.md section 10b.
+ * Where they do not fit only because of expressions that are finite sets of
+ * literals, those go to a literal matcher beside that engine instead
+ * (ROSE_RUNTIME_FULL_ROSE, block mode) -- DESIGN.md section 10d.
  * Anything else (look-around, back-references, UTF-8 / UCP, larger sets, ...) yields
  * HS_COMPILER_ERROR with an explanatory hs_compile_error_t, exactly as the
  * reference reports unsupported constructs.
@@ -269,7 +272,10 @@ hs_error_t hs_scan_vector(const hs_database_t *db, const char *const *data,
  * sub-expression that matched, `to` & ~(1 << 63) = where.  No match offset reaches
  * 2^63, and every id is a valid user id, so the bit is what tells them apart.  The
  * ordered forms (callbacks, _collect, hs_b200_fetch_matches,
- * hs_b200_postprocess_blocks) replace them with the combination reports. */
+ * hs_b200_postprocess_blocks) replace them with the combination reports.  Raw
+ * records of a database with a literal matcher beside an engine (DESIGN.md
+ * section 10d) hold the engine's records with bit 62 of `to` set and `id` = a
+ * report program's offset; the ordered forms resolve them into reports. */
 typedef struct hs_b200_match {
     unsigned int id;             /* report id the user registered */
     unsigned int block;          /* index of the block in the batch */
