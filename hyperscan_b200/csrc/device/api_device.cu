@@ -25,8 +25,8 @@
 #include <cstdlib>
 #include <cstring>
 #include <functional>
+#include <memory>
 #include <new>
-#include <unordered_map>
 #include <unordered_set>
 #include <vector>
 
@@ -104,8 +104,6 @@ struct DevImage {
     u32 nfaOffset = 0, nfaLength = 0;   /* the outfix engine (bytecode offset, NFA.length), alone (FK_OUTFIX) or
                                          * beside the literal matcher; nfaLength == 0: none */
     DfaParams nfaParams;                /* ... and what launchDfa needs to know about it */
-    /* the outfix's report program offset -> its (onmatch, offset_adjust) list, filled as programs are met */
-    mutable std::unordered_map<u32, std::vector<ProgReport>> progReports;
     double pairRate = 0;     /* FK_PAIR32: modelled first-stage candidates per byte (printable ASCII) */
     u8 *d_bitmap2 = nullptr; /* second level (HBM / L2) for large literal sets */
     u32 bitmap2Shift = 0;
@@ -115,9 +113,7 @@ struct DevImage {
     u32 confirmKind = CK_FDR;
     u64 groups = 0;
     u32 minWidth = 0;
-    bool hasDedupe = false;              /* RoseEngine.dkeyCount != 0 */
-    mutable std::unordered_set<u32> exhaustible; /* report ids under HS_FLAG_SINGLEMATCH (FK_OUTFIX: found with the programs) */
-    mutable Combinations comb;           /* logical combinations (FK_OUTFIX: lkeyReport found with the programs) */
+    ReportRules rules;                   /* how its records are delivered (borrows dbCopy) */
     size_t deviceBytes = 0;
 };
 
@@ -459,32 +455,11 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
     const DbHeader *h = (const DbHeader *)db;
     const RoseEngine *r = dbRose(db);
     const u8 *bc = (const u8 *)r;
-    const bool soleOutfix = r->runtimeImpl == RUNTIME_SINGLE_OUTFIX && r->mode == MODE_BLOCK && r->queueCount == 1 &&
-                            r->outfixBeginQueue == 0 && r->outfixEndQueue == 1 && r->nfaInfoOffset &&
-                            !r->amatcherOffset && !r->ematcherOffset && !r->fmatcherOffset && !r->hasSom;
-    /* the one FULL_ROSE shape run here: the floating literal matcher, whose role-less programs report
-     * directly, and one outfix on queue 0 (DESIGN.md section 10d) -- no anchored, EOD or small-block
-     * matcher, no roles, leftfixes, suffixes, delayed literals, MPV, SOM or long-literal table, and an
-     * EOD program that at most checks the engines' EOD accepts */
-    const bool mixed = r->runtimeImpl == RUNTIME_FULL_ROSE && r->mode == MODE_BLOCK && r->fmatcherOffset &&
-                       !r->amatcherOffset && !r->ematcherOffset && !r->sbmatcherOffset && !r->drmatcherOffset &&
-                       r->queueCount == 1 && r->activeArrayCount == 1 && r->outfixBeginQueue == 0 &&
-                       r->outfixEndQueue == 1 && r->leftfixBeginQueue == 1 && r->nfaInfoOffset &&
-                       !r->activeLeftCount && !r->rosePrefixCount && !r->rolesWithStateCount && !r->delay_count &&
-                       !r->anchored_count && r->initMpvNfa == MO_INVALID_IDX && !r->hasSom &&
-                       !r->longLitTableOffset && !r->ckeyCount && !r->eagerIterOffset && !r->delayProgramOffset &&
-                       !r->anchoredProgramOffset && !r->boundary.reportEodOffset && !r->boundary.reportZeroOffset &&
-                       !r->boundary.reportZeroEodOffset && !r->lastByteHistoryIterOffset &&
-                       (!r->eodProgramOffset ||
-                        ((size_t)r->eodProgramOffset + 16 <= h->length && r->eodProgramOffset % INSTR_ALIGN == 0 &&
-                         bc[r->eodProgramOffset] == OP_ENGINES_EOD &&
-                         bc[r->eodProgramOffset + HSB_ROUNDUP(sizeof(InstrEnginesEod), INSTR_ALIGN)] == OP_END));
-    if (!soleOutfix && !mixed && (r->runtimeImpl != RUNTIME_PURE_LITERAL || !r->fmatcherOffset)) {
-        /* other FULL_ROSE databases need the full rose interpreter (SURVEY.md section 8f rank 1):
-         * not in this build */
+    const DbShape shape = dbShape(db);
+    if (shape == SHAPE_UNSUPPORTED) {
         return HS_ARCH_ERROR;
     }
-    DevImage *im = new (std::nothrow) DevImage();
+    std::unique_ptr<DevImage, void (*)(DevImage *)> im(new (std::nothrow) DevImage(), freeImage);
     if (!im) {
         return HS_NOMEM;
     }
@@ -501,62 +476,46 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
     im->length = h->length;
     im->groups = r->initialGroups & r->floating_group_mask;
     im->minWidth = r->minWidth;
-    im->hasDedupe = r->dkeyCount != 0;
-    if (r->ckeyCount) {
-        loadCombinations(r, &im->comb);
-    }
-    if (soleOutfix || mixed) {
+    if (shape != SHAPE_PURE_LITERAL) {
         /* hs_scan -> soleOutfixBlockExec (src/runtime.c:245-280): ONE engine over the whole block,
          * its reports are report programs (roseReportAdaptor, src/rose/match.c:611-633).  The
          * engine runs on the DFA / NFA kernels (dfa_kernels.cu) straight from the bytecode copy;
-         * the programs are resolved on the host when the records are ordered (postprocess).  With
+         * the programs are resolved on the host when the records are delivered (ReportRules).  With
          * a literal matcher beside it (roseBlockExec's outfix), the engine's records are tagged so
          * that the host can tell them from the literals' */
         if ((size_t)r->nfaInfoOffset + sizeof(NfaInfo) > h->length) {
-            delete im;
             return HS_INVALID;
         }
         NfaInfo ni;
         memcpy(&ni, bc + r->nfaInfoOffset, sizeof(ni));
         if (ni.nfaOffset % 64 || (size_t)ni.nfaOffset + sizeof(NFA) > h->length) {
-            delete im;
             return HS_INVALID;
         }
         NFA nh;
         memcpy(&nh, bc + ni.nfaOffset, sizeof(nh));
         if ((size_t)ni.nfaOffset + nh.length > h->length) {
-            delete im;
             return HS_INVALID;
         }
         const hs_error_t er = engineParams(bc + ni.nfaOffset, nh.length, &im->nfaParams);
         if (er != HS_SUCCESS) {
-            delete im;
             return er;
         }
         im->nfaOffset = ni.nfaOffset;
         im->nfaLength = nh.length;
-        im->nfaParams.toTag = mixed ? ENGINE_RECORD : 0;
+        im->nfaParams.toTag = shape == SHAPE_LITERALS_OUTFIX ? ENGINE_RECORD : 0;
     }
-    if (soleOutfix) {
-        im->kind = FK_OUTFIX;
-        im->groups = 0;
-        cudaError_t e = cudaMalloc(&im->d_bc, HSB_ROUNDUP(h->length, 16));
-        if (e == cudaSuccess) {
-            e = cudaMemcpy(im->d_bc, bc, h->length, cudaMemcpyHostToDevice);
-        }
-        if (e != cudaSuccess) {
-            freeImage(im);
-            return e == cudaErrorMemoryAllocation ? HS_NOMEM : HS_UNKNOWN_ERROR;
-        }
-        im->deviceBytes = HSB_ROUNDUP(h->length, 16);
-        *out = im;
-        return HS_SUCCESS;
+    /* a literal program that uses a state-carrying opcode of roseRunProgram_l that the device
+     * interpreter does not implement (delayed literals, SOM, chained reports) is refused here
+     * rather than mid-scan */
+    std::vector<LitTail> tails;
+    const hs_error_t er = loadReportRules((const hs_database_t *)(im->dbCopy.data() + im->dbCopyShift), &im->rules,
+                                          &tails);
+    if (er != HS_SUCCESS) {
+        return er;
     }
     const HWLM *hw = (const HWLM *)(bc + r->fmatcherOffset);
     const u32 engOff = r->fmatcherOffset + HWLM_ENGINE_OFFSET;
-    std::vector<u8> table, pairBitmap, pairBitmap2;
-    std::vector<LitTail> tails;
-    bool programsOk = true;
+    std::vector<u8> table, bitmap, bitmap2;
     /* FK_PAIR32 / FK_GRAM4 tables from the literals' tails (FDR sets, and fat Teddy with its 16
      * buckets folded onto 8 first-stage bits) */
     auto pairStage = [&](bool allowGram) {
@@ -581,7 +540,7 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
              * instead (FK_GRAM4), exact raw 4-byte keys in L2 behind it */
             im->kind = FK_GRAM4;
             im->keyBytes = 4;
-            pairBitmap.swap(gramBitmap);
+            bitmap.swap(gramBitmap);
             /* second level in L2: one BYTE per slot = the buckets of the literals whose
              * raw 4-byte key hashes there (~64 slots per key, <= 64 MB), so that a
              * survivor reaches confirm with its real buckets, not all eight */
@@ -589,13 +548,13 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
             while (lg2 < 26 && (1ull << lg2) < (u64)keys.size() * 64) {
                 lg2++;
             }
-            pairBitmap2.assign((size_t)1 << lg2, 0);
+            bitmap2.assign((size_t)1 << lg2, 0);
             for (const LitTail &t : tails) {
                 const u32 v = (u32)(t.v >> 32), care = (u32)(t.msk >> 32), dc = ~care;
                 u32 sub = 0;
                 do {
                     const u32 k = (v & care) | sub;
-                    pairBitmap2[(k * 0x85EBCA6Bu) >> (32 - lg2)] |= (u8)(1u << (t.bucket & 7));
+                    bitmap2[(k * 0x85EBCA6Bu) >> (32 - lg2)] |= (u8)(1u << (t.bucket & 7));
                     sub = (sub - dc) & dc;
                 } while (sub);
             }
@@ -616,10 +575,13 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
         if (keyed) {
             im->keyBytes = kb;
             im->bitmapBits = 262144;
-            buildPairBitmaps(keys, im->bitmapBits, &pairBitmap, &pairBitmap2, &im->bitmap2Shift);
+            buildPairBitmaps(keys, im->bitmapBits, &bitmap, &bitmap2, &im->bitmap2Shift);
         }
     };
-    if (hw->type == HWLM_ENGINE_NOOD) {
+    if (shape == SHAPE_SOLE_OUTFIX) {
+        im->kind = FK_OUTFIX;
+        im->groups = 0;
+    } else if (hw->type == HWLM_ENGINE_NOOD) {
         /* single literal: one bucket, slots = the last <= 4 bytes of msk/cmp
          * (first char in the low byte: src/hwlm/noodle_build.cpp:100-118) */
         NoodTable n;
@@ -643,93 +605,61 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
             }
             memcpy(&table[b * 4], &e, 4);
         }
-        programsOk = collectProgramReports(bc, h->length, n.id, &im->exhaustible, nullptr, &im->comb.lkeyReport, mixed);
-    } else if (hw->type == HWLM_ENGINE_FDR) {
+    } else {
+        /* FDR or Teddy: loadReportRules refused any other matcher */
         FDR f;
         memcpy(&f, bc + engOff, sizeof(f));
         im->confirmKind = CK_FDR;
         im->confOff = engOff + f.confOffset;
         if (f.engineID == 0) {
-            programsOk = walkConfirm(bc, h->length, im->confOff, 8, &im->exhaustible, &tails, &im->comb.lkeyReport, mixed);
             pairStage(true);
-        } else if (teddyIdValid(f.engineID)) {
-            const u32 oct = teddyNumBuckets(f.engineID) / 8;
-            programsOk = walkConfirm(bc, h->length, im->confOff, 8 * oct, &im->exhaustible, &tails,
-                                     &im->comb.lkeyReport, mixed);
-            if (oct == 2) {
-                /* fat Teddy (49..96 literals): the class-pair kernel with 8 bucket bits that
-                 * carry buckets i and i + 8 (confirmKernel unfolds them) */
-                pairStage(false);
-                im->bucketFold = 1;
-            } else {
-                /* per-byte entry: slot m = lo_m[b & 15] | hi_m[b >> 4]
-                 * (src/fdr/teddy.c:918-969, teddy_compile.cpp:440-509) */
-                const u32 nm = teddyNumMasks(f.engineID);
-                const u8 *mb = bc + engOff + TEDDY_MASK_OFFSET;
-                im->kind = FK_BYTE32;
-                table.assign(256 * 4, 0);
-                for (u32 b = 0; b < 256; b++) {
-                    u32 e = 0;
-                    for (u32 m = 0; m < nm; m++) {
-                        e |= (u32)(u8)(mb[2 * m * 16 + (b & 15)] | mb[(2 * m + 1) * 16 + (b >> 4)]) << (8 * m);
-                    }
-                    memcpy(&table[b * 4], &e, 4);
-                }
-            }
+        } else if (teddyNumBuckets(f.engineID) == 16) {
+            /* fat Teddy (49..96 literals): the class-pair kernel with 8 bucket bits that
+             * carry buckets i and i + 8 (confirmKernel unfolds them) */
+            pairStage(false);
+            im->bucketFold = 1;
         } else {
-            delete im;
-            return HS_INVALID;
+            /* per-byte entry: slot m = lo_m[b & 15] | hi_m[b >> 4]
+             * (src/fdr/teddy.c:918-969, teddy_compile.cpp:440-509) */
+            const u32 nm = teddyNumMasks(f.engineID);
+            const u8 *mb = bc + engOff + TEDDY_MASK_OFFSET;
+            im->kind = FK_BYTE32;
+            table.assign(256 * 4, 0);
+            for (u32 b = 0; b < 256; b++) {
+                u32 e = 0;
+                for (u32 m = 0; m < nm; m++) {
+                    e |= (u32)(u8)(mb[2 * m * 16 + (b & 15)] | mb[(2 * m + 1) * 16 + (b >> 4)]) << (8 * m);
+                }
+                memcpy(&table[b * 4], &e, 4);
+            }
         }
-    } else {
-        delete im;
-        return HS_INVALID;
     }
-    if (!programsOk) {
-        /* a literal program uses a state-carrying opcode of roseRunProgram_l that
-         * the device interpreter does not implement (delayed literals, SOM,
-         * chained / logical reports): refuse here rather than mid-scan */
-        delete im;
-        return HS_ARCH_ERROR;
-    }
-    im->tableBytes = (u32)table.size();
-    std::vector<u8> bitmap, bitmap2;
-    if (im->kind == FK_PAIR32 || im->kind == FK_GRAM4) {
-        bitmap.swap(pairBitmap);
-        bitmap2.swap(pairBitmap2);
-    } else {
+    if (im->kind == FK_BYTE32) {
         bitmap = buildBitmap(tails, &im->keyBytes, &im->bitmapShift, &bitmap2, &im->bitmap2Shift);
     }
-    im->bitmapBytes = (u32)bitmap.size();
-    cudaError_t e = cudaMalloc(&im->d_bc, HSB_ROUNDUP(h->length, 16));
-    if (e == cudaSuccess && !bitmap.empty()) {
-        e = cudaMalloc(&im->d_bitmap, bitmap.size());
-        if (e == cudaSuccess) {
-            e = cudaMemcpy(im->d_bitmap, bitmap.data(), bitmap.size(), cudaMemcpyHostToDevice);
-        }
-    }
-    if (e == cudaSuccess && !bitmap2.empty()) {
-        e = cudaMalloc(&im->d_bitmap2, bitmap2.size());
-        if (e == cudaSuccess) {
-            e = cudaMemcpy(im->d_bitmap2, bitmap2.data(), bitmap2.size(), cudaMemcpyHostToDevice);
-        }
-    } else {
+    if (bitmap2.empty()) {
         im->bitmap2Shift = 0;
     }
-    if (e == cudaSuccess) {
-        e = cudaMalloc(&im->d_table, HSB_ROUNDUP(table.size(), 16));
-    }
-    if (e == cudaSuccess) {
-        e = cudaMemcpy(im->d_bc, bc, h->length, cudaMemcpyHostToDevice);
-    }
-    if (e == cudaSuccess) {
-        e = cudaMemcpy(im->d_table, table.data(), table.size(), cudaMemcpyHostToDevice);
-    }
+    im->tableBytes = (u32)table.size();
+    im->bitmapBytes = (u32)bitmap.size();
+    cudaError_t e = cudaSuccess;
+    auto upload = [&](u8 **d, const void *src, size_t bytes, size_t allocBytes) {
+        if (e == cudaSuccess && bytes) {
+            e = cudaMalloc(d, allocBytes);
+            if (e == cudaSuccess) {
+                e = cudaMemcpy(*d, src, bytes, cudaMemcpyHostToDevice);
+            }
+        }
+    };
+    upload(&im->d_bc, bc, h->length, HSB_ROUNDUP(h->length, 16));
+    upload(&im->d_table, table.data(), table.size(), HSB_ROUNDUP(table.size(), 16));
+    upload(&im->d_bitmap, bitmap.data(), bitmap.size(), bitmap.size());
+    upload(&im->d_bitmap2, bitmap2.data(), bitmap2.size(), bitmap2.size());
     if (e != cudaSuccess) {
-        freeImage(im);
         return e == cudaErrorMemoryAllocation ? HS_NOMEM : HS_UNKNOWN_ERROR;
     }
     im->deviceBytes = HSB_ROUNDUP(h->length, 16) + HSB_ROUNDUP(table.size(), 16) + bitmap.size() + bitmap2.size();
-    *out = im;
+    *out = im.release();
     return HS_SUCCESS;
 }
 
@@ -844,7 +774,7 @@ bool markInUse(hs_scratch *s) { /* src/scratch.h:249-271 */
 }
 void unmarkInUse(hs_scratch *s) { s->in_use = 0; }
 
-hs_error_t findImage(hs_scratch *s, const hs_database_t *db, const DevImage **out) {
+hs_error_t findImage(hs_scratch *s, const hs_database_t *db, DevImage **out) {
     const DbHeader *h = (const DbHeader *)db;
     for (DevImage *im : *s->images) {
         if (im->db == db && im->crc == h->crc32 && im->length == h->length) {
@@ -1082,84 +1012,6 @@ hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
     return HS_SUCCESS;
 }
 
-size_t postprocess(const DevImage *im, DevMatch *m, size_t n) {
-    return postprocessRecords(im->exhaustible, (MatchRec *)m, n);
-}
-
-/* Records of a database with logical combinations, in delivery order with the combination
- * reports added (postprocessCombinations); lengths[i] is the length of block i. */
-void postprocessComb(const DevImage *im, std::vector<DevMatch> *v, const u32 *lengths, size_t nblocks) {
-    static_assert(sizeof(MatchRec) == sizeof(DevMatch), "record layout");
-    std::vector<MatchRec> recs(v->size());
-    memcpy(recs.data(), v->data(), v->size() * sizeof(DevMatch));
-    postprocessCombinations(im->comb, im->exhaustible, &recs, lengths, nblocks);
-    v->resize(recs.size());
-    memcpy(v->data(), recs.data(), recs.size() * sizeof(DevMatch));
-}
-
-/* Records of a scan, ordered and with the order-dependent report rules applied (see
- * postprocessRecords).  Databases with an outfix: the engine kernel's records carry report PROGRAM
- * offsets (and the padding of the lanes' reserved slots) -- all of a single-outfix database's
- * records, and those tagged ENGINE_RECORD beside a literal matcher; each is replaced by the reports
- * its program raises -- roseReportAdaptor -> roseRunProgram (src/rose/match.c:611-633) -- first,
- * and the literals' records join them as they are.  Databases with logical combinations need the
- * block lengths (lengths[0, nblocks)). */
-hs_error_t postprocessVec(const DevImage *im, std::vector<DevMatch> *v, const u32 *lengths = nullptr,
-                          size_t nblocks = 0) {
-    if (im->comb.any() && !lengths && nblocks) {
-        return HS_INVALID;
-    }
-    if (!im->nfaLength) {
-        if (im->comb.any()) {
-            postprocessComb(im, v, lengths, nblocks);
-        } else {
-            v->resize(postprocess(im, v->data(), v->size()));
-        }
-        return HS_SUCCESS;
-    }
-    const u8 *bc = (const u8 *)dbRose((const hs_database_t *)(im->dbCopy.data() + im->dbCopyShift));
-    std::vector<DevMatch> outv;
-    outv.reserve(v->size());
-    const bool tagged = im->kind != FK_OUTFIX;
-    for (DevMatch m : *v) {
-        if (tagged) {
-            if (!(m.to & ENGINE_RECORD)) {
-                outv.push_back(m); /* a literal's record */
-                continue;
-            }
-            m.to &= ~ENGINE_RECORD;
-        }
-        if (m.id == 0xffffffffu) {
-            continue; /* a slot some lane reserved and did not fill */
-        }
-        auto it = im->progReports.find(m.id);
-        if (it == im->progReports.end()) {
-            std::vector<ProgReport> reps;
-            if (m.id % INSTR_ALIGN || m.id < sizeof(RoseEngine) || m.id >= im->length ||
-                !collectProgramReports(bc, im->length, m.id, &im->exhaustible, &reps, &im->comb.lkeyReport)) {
-                return HS_UNKNOWN_ERROR; /* a program with a state-carrying opcode (or a corrupt record) */
-            }
-            it = im->progReports.emplace(m.id, std::move(reps)).first;
-        }
-        for (const ProgReport &rp : it->second) {
-            if (m.to < rp.min_bound || m.to > rp.max_bound) {
-                continue; /* CHECK_BOUNDS (hs_expr_ext min_offset / max_offset) */
-            }
-            DevMatch o = m;
-            o.id = rp.onmatch;
-            o.to = (u64)((long long)m.to + rp.offset_adjust) | (rp.logical ? LKEY_RECORD : 0);
-            outv.push_back(o);
-        }
-    }
-    if (im->comb.any()) {
-        postprocessComb(im, &outv, lengths, nblocks);
-    } else {
-        outv.resize(postprocess(im, outv.data(), outv.size()));
-    }
-    v->swap(outv);
-    return HS_SUCCESS;
-}
-
 hs_error_t finishScan(hs_scratch *s, u32 *count) {
     /* wait for THIS scan only: a later scan may already be queued behind it
      * on the same stream (double-buffered callers) */
@@ -1246,7 +1098,7 @@ struct ScanTimes {
 };
 
 /* Scan a corpus on the scratch's stream (uploading it through `up`, if given) and
- * read its records back: ordered, with the report rules applied (postprocessVec), or
+ * read its records back: ordered, with the report rules applied (ReportRules::deliver), or
  * raw when !ordered.  When the record ring overflows, it grows and the corpus, resident
  * by then, is scanned again as one range.  A second pass finds the real record count;
  * a third may be needed, because the candidate list can overflow before the ring does.
@@ -1255,7 +1107,7 @@ struct ScanTimes {
  * candidate count only, which is too small to size the ring for one range over the whole
  * corpus.  So that pass does not count: the rescans then run exactly as for a corpus
  * that was resident from the start. */
-hs_error_t scanRecords(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c, const Upload *up,
+hs_error_t scanRecords(hs_scratch *s, DevImage *im, const hs_b200_corpus *c, const Upload *up,
                        bool ordered, std::vector<DevMatch> *matches, ScanTimes *times = nullptr,
                        const u32 *lengths = nullptr) {
     ScanTimes unused;
@@ -1287,7 +1139,7 @@ hs_error_t scanRecords(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
             CUDA_TRY(cudaStreamSynchronize(s->stream));
         }
         t.read = nowMs();
-        return ordered ? postprocessVec(im, matches, lengths, c->nblocks) : HS_SUCCESS;
+        return ordered ? im->rules.deliver(matches, lengths, c->nblocks) : HS_SUCCESS;
     }
     return HS_UNKNOWN_ERROR;
 }
@@ -1515,7 +1367,7 @@ hs_error_t hs_alloc_scratch(const hs_database_t *db, hs_scratch_t **scratch) {
         s->in_use = 1;
     }
     DeviceGuard guard(s->device);
-    const DevImage *im = nullptr;
+    DevImage *im = nullptr;
     r = findImage(s, db, &im);
     unmarkInUse(s);
     if (r != HS_SUCCESS) {
@@ -1805,7 +1657,7 @@ hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corp
         return HS_SCRATCH_IN_USE;
     }
     DeviceGuard guard(scratch->device);
-    const DevImage *im = nullptr;
+    DevImage *im = nullptr;
     r = findImage(scratch, db, &im);
     if (r == HS_SUCCESS) {
         cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
@@ -1964,7 +1816,7 @@ hs_error_t hs_b200_fetch_matches(const hs_database_t *db, hs_scratch_t *scratch,
         return HS_INVALID;
     }
     DeviceGuard guard(scratch->device);
-    const DevImage *im = nullptr;
+    DevImage *im = nullptr;
     hs_error_t r = findImage(scratch, db, &im);
     if (r != HS_SUCCESS) {
         return r;
@@ -1976,12 +1828,12 @@ hs_error_t hs_b200_fetch_matches(const hs_database_t *db, hs_scratch_t *scratch,
                                  cudaMemcpyDeviceToHost, scratch->copyStream));
         CUDA_TRY(cudaStreamSynchronize(scratch->copyStream));
     }
-    if (im->comb.any()) {
+    if (im->rules.comb.any()) {
         /* the combinations are evaluated per block, over the blocks of the corpus last scanned */
         const hs_b200_corpus *c = scratch->lastCorpus;
-        r = c ? postprocessVec(im, &tmp, c->h_len.data(), c->h_len.size()) : HS_INVALID;
+        r = c ? im->rules.deliver(&tmp, c->h_len.data(), c->h_len.size()) : HS_INVALID;
     } else {
-        r = postprocessVec(im, &tmp);
+        r = im->rules.deliver(&tmp, nullptr, 0);
     }
     if (r != HS_SUCCESS) {
         return r;
@@ -2064,11 +1916,7 @@ hs_error_t hs_b200_nfa_scan_corpus(const void *nfa, size_t nfa_len, const hs_b20
     if (e != cudaSuccess) {
         rv = e == cudaErrorMemoryAllocation ? HS_NOMEM : HS_UNKNOWN_ERROR;
     } else {
-        std::sort(host.begin(), host.end(), [](const DevMatch &a, const DevMatch &b) {
-            if (a.block != b.block) return a.block < b.block;
-            if (a.to != b.to) return a.to < b.to;
-            return a.id < b.id;
-        });
+        std::sort(host.begin(), host.end(), RecordOrder());
         *nmatches = host.size();
         memcpy(out, host.data(), std::min(cap, host.size()) * sizeof(DevMatch));
         if (host.size() > cap) {
@@ -2087,7 +1935,7 @@ hs_error_t hs_b200_nfa_scan_corpus(const void *nfa, size_t nfa_len, const hs_b20
 
 /* Copy host blocks into the scratch's inline corpus and scan them, with the
  * host->device copy pipelined against the kernel in chunk_mb pieces. */
-static hs_error_t scanHostBlocks(const DevImage *im, hs_scratch *s, const char *data,
+static hs_error_t scanHostBlocks(DevImage *im, hs_scratch *s, const char *data,
                                  const unsigned long long *offsets, const unsigned *lengths,
                                  size_t nblocks, std::vector<DevMatch> *matches,
                                  bool countOnly = false) {
@@ -2167,9 +2015,8 @@ static hs_error_t scanHostBlocks(const DevImage *im, hs_scratch *s, const char *
         CUDA_TRY(cudaStreamWaitEvent(s->stream, (*s->chunkEvents)[ci], 0));
         return HS_SUCCESS;
     };
-    /* nobody will look at the order, and neither dedupe keys nor
-     * exhaustion keys exist: the raw count IS the delivered count */
-    const bool plain = countOnly && im->exhaustible.empty() && !im->hasDedupe && !im->nfaLength && !im->comb.any();
+    /* nobody will look at the order: when no report rule applies, the raw count IS the delivered count */
+    const bool plain = countOnly && im->rules.rawCountDelivered();
     ScanTimes tm;
     r = scanRecords(s, im, c, &up, !plain, matches, &tm, lengths);
     if (r == HS_SUCCESS && trace) {
@@ -2197,7 +2044,7 @@ static hs_error_t blockScan(const hs_database_t *db, hs_scratch *s, const char *
         return HS_SCRATCH_IN_USE;
     }
     if (!(skipShort && dbRose(db)->minWidth > lengths[0])) {
-        const DevImage *im = nullptr;
+        DevImage *im = nullptr;
         std::vector<DevMatch> matches;
         r = findImage(s, db, &im);
         if (r == HS_SUCCESS) {
@@ -2255,7 +2102,6 @@ hs_error_t hs_b200_scan_blocks_collect(const hs_database_t *db, const char *data
                          if (nmatches) {
                              *nmatches = matches.size();
                          }
-                         static_assert(sizeof(DevMatch) == sizeof(hs_b200_match_t), "record layout");
                          memcpy(out, matches.data(), std::min(cap, matches.size()) * sizeof(DevMatch));
                          return matches.size() > cap ? HS_INSUFFICIENT_SPACE : HS_SUCCESS;
                      });
@@ -2353,7 +2199,7 @@ static hs_error_t streamWrite(hs_stream *st, const char *data, unsigned int leng
     if (st->status & 1) {
         r = HS_SCAN_TERMINATED; /* the stream is broken: src/runtime.c:883-893 */
     } else if (!(st->status & 2) && length != 0) {
-        const DevImage *im = nullptr;
+        DevImage *im = nullptr;
         r = findImage(scratch, st->db, &im);
         std::vector<DevMatch> matches;
         std::vector<char> buf;
@@ -2371,7 +2217,7 @@ static hs_error_t streamWrite(hs_stream *st, const char *data, unsigned int leng
                 if (m.to <= st->hlen) {
                     continue; /* ended in the look-behind: raised by an earlier write */
                 }
-                if (im->exhaustible.count(m.id) && !st->seen->insert(m.id).second) {
+                if (im->rules.exhaustible.count(m.id) && !st->seen->insert(m.id).second) {
                     continue; /* HS_FLAG_SINGLEMATCH: already raised on this stream */
                 }
                 if (onEvent && onEvent(m.id, 0, st->offset - st->hlen + m.to, 0, context)) {
@@ -2381,7 +2227,7 @@ static hs_error_t streamWrite(hs_stream *st, const char *data, unsigned int leng
                 }
             }
             if (r == HS_SUCCESS) {
-                if (rose->canExhaust && rose->ekeyCount && st->seen->size() >= im->exhaustible.size()) {
+                if (rose->canExhaust && rose->ekeyCount && st->seen->size() >= im->rules.exhaustible.size()) {
                     st->status |= 2;
                 }
                 /* maintainHistoryBuffer (src/runtime.c:478-508) */
@@ -2724,7 +2570,7 @@ static hs_error_t streamsScanImpl(hs_b200_stream_set_t *set, const char *data,
         return HS_INVALID; /* the set's state and the scratch's ring must share a device */
     }
     DeviceGuard guard(set->device);
-    const DevImage *im = nullptr;
+    DevImage *im = nullptr;
     hs_error_t r = findImage(s, set->db, &im);
     if (r != HS_SUCCESS) {
         return r;

@@ -31,14 +31,6 @@
 
 namespace hsb {
 
-/* One match record as the device writes it: identical to hs_b200_match_t
- * (include/hs_b200.h). */
-struct DevMatch {
-    u32 id;
-    u32 block;
-    u64 to;
-};
-
 /* First-stage ("shift-OR") filter variants.  An entry read at sampled position
  * x holds SLOTS bytes; byte p has bit b SET iff no literal of bucket b can end
  * at position x+p given the bytes at x (FDR: src/fdr/fdr.c:157-327; Teddy:

@@ -8,17 +8,22 @@
 
 namespace hsb {
 
-/* Linear walk over one literal program.  A program is a sequence of blocks, each
+namespace {
+
+/* Linear walk over one program of rr's bytecode.  A program is a sequence of blocks, each
  * ending in END or FINAL_REPORT; later blocks are reached through the fail_jump
  * of a check in an earlier one (src/rose/rose_build_program.cpp:525-829), so
  * the walk continues past a terminator while a jump target lies beyond it.
  * Returns false on an opcode the device interpreter (scan_kernels.cu
  * runProgram) does not implement -- the state-carrying ones of
- * roseRunProgram_l: PUSH_DELAYED, CATCH_UP* (CATCH_UP is accepted on request), SOM_*, TRIGGER_SUFFIX, REPORT_CHAIN,
+ * roseRunProgram_l: PUSH_DELAYED, CATCH_UP* (CATCH_UP is accepted beside an outfix), SOM_*, TRIGGER_SUFFIX, REPORT_CHAIN,
  * REPORT_SOM*, SET_EXHAUST.  SET_LOGICAL is a report of its own here (a logical-key record
- * on the device); FLUSH_COMBINATION and SET_COMBINATION follow from it on the host. */
-bool collectProgramReports(const u8 *bc, u32 bcLen, u32 prog, std::unordered_set<u32> *ex,
-                           std::vector<ProgReport> *reports, LkeyReports *lkeys, bool catchUp) {
+ * on the device); FLUSH_COMBINATION and SET_COMBINATION follow from it on the host.
+ * Collects the exhaustible reports and the lkeys' reports into rr; reports, if given, receives
+ * every report instruction, in program order. */
+bool collectProgramReports(ReportRules *rr, u32 prog, std::vector<ProgReport> *reports) {
+    const u8 *bc = rr->bc;
+    const u32 bcLen = rr->bcLen;
     u32 pc = prog, furthest = prog;
     u32 lastReport = INVALID_EKEY; /* the report of the current report block, for SET_LOGICAL */
     /* CHECK_BOUNDS guards the instructions up to its fail_jump target */
@@ -98,7 +103,7 @@ bool collectProgramReports(const u8 *bc, u32 bcLen, u32 prog, std::unordered_set
         case OP_REPORT_EXHAUST: {
             InstrReportExhaust in;
             memcpy(&in, bc + pc, sizeof(in));
-            ex->insert(in.onmatch);
+            rr->exhaustible.insert(in.onmatch);
             lastReport = in.onmatch;
             if (reports) {
                 report(in.onmatch, in.offset_adjust);
@@ -124,8 +129,8 @@ bool collectProgramReports(const u8 *bc, u32 bcLen, u32 prog, std::unordered_set
         case OP_SET_LOGICAL: {
             InstrSetLogical in;
             memcpy(&in, bc + pc, sizeof(in));
-            if (lkeys && lastReport != INVALID_EKEY) {
-                (*lkeys)[in.lkey] = lastReport;
+            if (lastReport != INVALID_EKEY) {
+                rr->comb.lkeyReport[in.lkey] = lastReport;
             }
             if (reports) {
                 report(in.lkey, in.offset_adjust);
@@ -138,7 +143,9 @@ bool collectProgramReports(const u8 *bc, u32 bcLen, u32 prog, std::unordered_set
         case OP_CLEAR_WORK_DONE: pc += INSTR_ALIGN; break;
         case OP_INCLUDED_JUMP: STEP(InstrIncludedJump); break;
         case OP_CATCH_UP:
-            if (!catchUp) {
+            /* beside an outfix, CATCH_UP only orders the outfix's reports before the literal's -- which the
+             * host's ordering does */
+            if (rr->shape != SHAPE_LITERALS_OUTFIX) {
                 return false;
             }
             STEP(InstrCatchUp);
@@ -154,10 +161,9 @@ bool collectProgramReports(const u8 *bc, u32 bcLen, u32 prog, std::unordered_set
 
 /* Walk the hash-confirm structures to enumerate literal programs
  * (src/fdr/fdr_confirm.h:36-94). */
-bool walkConfirm(const u8 *bc, u32 bcLen, u32 confOff, u32 nBuckets,
-                 std::unordered_set<u32> *ex, std::vector<LitTail> *tails, LkeyReports *lkeys, bool catchUp) {
+bool walkConfirm(ReportRules *rr, u32 confOff, u32 nBuckets, std::vector<LitTail> *tails) {
     bool ok = true;
-    const u8 *confBase = bc + confOff;
+    const u8 *confBase = rr->bc + confOff;
     for (u32 b = 0; b < nBuckets; b++) {
         u32 cf;
         memcpy(&cf, confBase + 4 * b, 4);
@@ -178,8 +184,10 @@ bool walkConfirm(const u8 *bc, u32 bcLen, u32 confOff, u32 nBuckets,
             for (;;) {
                 LitInfo x;
                 memcpy(&x, li, sizeof(x));
-                ok &= collectProgramReports(bc, bcLen, x.id, ex, nullptr, lkeys, catchUp);
-                tails->push_back({x.v, x.msk, x.size, b});
+                ok &= collectProgramReports(rr, x.id, nullptr);
+                if (tails) {
+                    tails->push_back({x.v, x.msk, x.size, b});
+                }
                 if (!x.next) {
                     break;
                 }
@@ -190,36 +198,10 @@ bool walkConfirm(const u8 *bc, u32 bcLen, u32 confOff, u32 nBuckets,
     return ok;
 }
 
-hs_error_t collectExhaustible(const hs_database_t *db, std::unordered_set<u32> *ex, LkeyReports *lkeys) {
-    const DbHeader *h = (const DbHeader *)db;
-    if (!h || h->magic != DB_MAGIC) {
-        return HS_INVALID;
-    }
-    const RoseEngine *r = dbRose(db);
-    const u8 *bc = (const u8 *)r;
-    if (r->runtimeImpl != RUNTIME_PURE_LITERAL || !r->fmatcherOffset) {
-        return HS_ARCH_ERROR;
-    }
-    const HWLM *hw = (const HWLM *)(bc + r->fmatcherOffset);
-    const u32 engOff = r->fmatcherOffset + HWLM_ENGINE_OFFSET;
-    if (hw->type == HWLM_ENGINE_NOOD) {
-        NoodTable n;
-        memcpy(&n, bc + engOff, sizeof(n));
-        return collectProgramReports(bc, h->length, n.id, ex, nullptr, lkeys) ? HS_SUCCESS : HS_ARCH_ERROR;
-    }
-    FDR f;
-    memcpy(&f, bc + engOff, sizeof(f));
-    const u32 nb = f.engineID == 0 ? 8 : teddyNumBuckets(f.engineID);
-    std::vector<LitTail> tails;
-    return walkConfirm(bc, h->length, engOff + f.confOffset, nb, ex, &tails, lkeys) ? HS_SUCCESS : HS_ARCH_ERROR;
-}
-
-size_t postprocessRecords(const std::unordered_set<u32> &exhaustible, MatchRec *m, size_t n) {
-    std::sort(m, m + n, [](const MatchRec &a, const MatchRec &b) {
-        if (a.block != b.block) return a.block < b.block;
-        if (a.to != b.to) return a.to < b.to;
-        return a.id < b.id;
-    });
+/* Order records for delivery and apply dedupe and exhaustion (ReportRules::deliver).  Returns the number
+ * of records kept (in place, sorted by (block, to, id)). */
+size_t postprocessRecords(const std::unordered_set<u32> &exhaustible, DevMatch *m, size_t n) {
+    std::sort(m, m + n, RecordOrder());
     size_t w = 0;
     std::unordered_set<u32> seen;
     u32 curBlock = 0xffffffffu;
@@ -269,8 +251,6 @@ void loadCombinations(const RoseEngine *r, Combinations *cb) {
     }
 }
 
-namespace {
-
 /* the per-block state of src/rose/program_runtime.c:2026-2120: logical values of lkeys and operations,
  * the combinations touched since the last flush */
 struct CombState {
@@ -306,19 +286,21 @@ struct CombState {
     }
 };
 
-} // namespace
-
+/* The rules for a database with logical combinations, whose records include logical-key records: the
+ * records of blocks [0, nblocks) (block i is lengths[i] bytes long) in delivery order -- by (block, to),
+ * at one offset the reports by id and then the combinations it completes, by ckey -- with the
+ * combination reports added and the logical-key records gone. */
 void postprocessCombinations(const Combinations &cb, const std::unordered_set<u32> &exhaustible,
-                             std::vector<MatchRec> *v, const u32 *lengths, size_t nblocks) {
-    std::vector<MatchRec> &m = *v;
-    std::sort(m.begin(), m.end(), [](const MatchRec &a, const MatchRec &b) {
+                             std::vector<DevMatch> *v, const u32 *lengths, size_t nblocks) {
+    std::vector<DevMatch> &m = *v;
+    std::sort(m.begin(), m.end(), [](const DevMatch &a, const DevMatch &b) {
         if (a.block != b.block) return a.block < b.block;
         const u64 ta = a.to & ~LKEY_RECORD, tb = b.to & ~LKEY_RECORD;
         if (ta != tb) return ta < tb;
         if ((a.to & LKEY_RECORD) != (b.to & LKEY_RECORD)) return (a.to & LKEY_RECORD) < (b.to & LKEY_RECORD);
         return a.id < b.id;
     });
-    std::vector<MatchRec> out;
+    std::vector<DevMatch> out;
     out.reserve(m.size());
     CombState st(cb);
     std::unordered_map<u32, u64> firstAt; /* exhaustible id -> offset of its one delivered report */
@@ -357,7 +339,7 @@ void postprocessCombinations(const Combinations &cb, const std::unordered_set<u3
             st.anyActive = false;
         };
         for (size_t k = b0; k < i; k++) {
-            const MatchRec &r = m[k];
+            const DevMatch &r = m[k];
             const u64 to = r.to & ~LKEY_RECORD;
             if (to > last) {
                 flush(last); /* FLUSH_COMBINATION at the first report past the last one that set an lkey */
@@ -413,6 +395,123 @@ void postprocessCombinations(const Combinations &cb, const std::unordered_set<u3
     v->swap(out);
 }
 
+} // namespace
+
+DbShape dbShape(const hs_database_t *db) {
+    const DbHeader *h = (const DbHeader *)db;
+    const RoseEngine *r = dbRose(db);
+    const u8 *bc = (const u8 *)r;
+    if (r->runtimeImpl == RUNTIME_PURE_LITERAL && r->fmatcherOffset) {
+        return SHAPE_PURE_LITERAL;
+    }
+    if (r->runtimeImpl == RUNTIME_SINGLE_OUTFIX && r->mode == MODE_BLOCK && r->queueCount == 1 &&
+        r->outfixBeginQueue == 0 && r->outfixEndQueue == 1 && r->nfaInfoOffset && !r->amatcherOffset &&
+        !r->ematcherOffset && !r->fmatcherOffset && !r->hasSom) {
+        return SHAPE_SOLE_OUTFIX;
+    }
+    /* the one FULL_ROSE shape run here: the floating literal matcher, whose role-less programs report
+     * directly, and one outfix on queue 0 (DESIGN.md section 10d) -- no anchored, EOD or small-block
+     * matcher, no roles, leftfixes, suffixes, delayed literals, MPV, SOM or long-literal table, and an
+     * EOD program that at most checks the engines' EOD accepts */
+    if (r->runtimeImpl == RUNTIME_FULL_ROSE && r->mode == MODE_BLOCK && r->fmatcherOffset && !r->amatcherOffset &&
+        !r->ematcherOffset && !r->sbmatcherOffset && !r->drmatcherOffset && r->queueCount == 1 &&
+        r->activeArrayCount == 1 && r->outfixBeginQueue == 0 && r->outfixEndQueue == 1 &&
+        r->leftfixBeginQueue == 1 && r->nfaInfoOffset && !r->activeLeftCount && !r->rosePrefixCount &&
+        !r->rolesWithStateCount && !r->delay_count && !r->anchored_count && r->initMpvNfa == MO_INVALID_IDX &&
+        !r->hasSom && !r->longLitTableOffset && !r->ckeyCount && !r->eagerIterOffset && !r->delayProgramOffset &&
+        !r->anchoredProgramOffset && !r->boundary.reportEodOffset && !r->boundary.reportZeroOffset &&
+        !r->boundary.reportZeroEodOffset && !r->lastByteHistoryIterOffset &&
+        (!r->eodProgramOffset ||
+         ((size_t)r->eodProgramOffset + 16 <= h->length && r->eodProgramOffset % INSTR_ALIGN == 0 &&
+          bc[r->eodProgramOffset] == OP_ENGINES_EOD &&
+          bc[r->eodProgramOffset + HSB_ROUNDUP(sizeof(InstrEnginesEod), INSTR_ALIGN)] == OP_END))) {
+        return SHAPE_LITERALS_OUTFIX;
+    }
+    return SHAPE_UNSUPPORTED;
+}
+
+hs_error_t loadReportRules(const hs_database_t *db, ReportRules *rules, std::vector<LitTail> *tails) {
+    const RoseEngine *r = dbRose(db);
+    rules->shape = dbShape(db);
+    if (rules->shape == SHAPE_UNSUPPORTED) {
+        return HS_ARCH_ERROR;
+    }
+    rules->bc = (const u8 *)r;
+    rules->bcLen = ((const DbHeader *)db)->length;
+    rules->hasDedupe = r->dkeyCount != 0;
+    if (r->ckeyCount) {
+        loadCombinations(r, &rules->comb);
+    }
+    if (rules->shape == SHAPE_SOLE_OUTFIX) {
+        return HS_SUCCESS; /* no literal programs: the engine's are walked as its records are delivered */
+    }
+    const HWLM *hw = (const HWLM *)(rules->bc + r->fmatcherOffset);
+    const u32 engOff = r->fmatcherOffset + HWLM_ENGINE_OFFSET;
+    bool ok;
+    if (hw->type == HWLM_ENGINE_NOOD) {
+        NoodTable n;
+        memcpy(&n, rules->bc + engOff, sizeof(n));
+        ok = collectProgramReports(rules, n.id, nullptr);
+    } else if (hw->type == HWLM_ENGINE_FDR) {
+        FDR f;
+        memcpy(&f, rules->bc + engOff, sizeof(f));
+        if (f.engineID != 0 && !teddyIdValid(f.engineID)) {
+            return HS_INVALID;
+        }
+        ok = walkConfirm(rules, engOff + f.confOffset, f.engineID == 0 ? 8 : teddyNumBuckets(f.engineID), tails);
+    } else {
+        return HS_INVALID;
+    }
+    return ok ? HS_SUCCESS : HS_ARCH_ERROR;
+}
+
+hs_error_t ReportRules::deliver(std::vector<DevMatch> *v, const u32 *lengths, size_t nblocks) {
+    if (comb.any() && !lengths && nblocks) {
+        return HS_INVALID;
+    }
+    if (shape != SHAPE_PURE_LITERAL) {
+        std::vector<DevMatch> out;
+        out.reserve(v->size());
+        for (DevMatch m : *v) {
+            if (shape == SHAPE_LITERALS_OUTFIX) {
+                if (!(m.to & ENGINE_RECORD)) {
+                    out.push_back(m); /* a literal's record */
+                    continue;
+                }
+                m.to &= ~ENGINE_RECORD;
+            }
+            if (m.id == 0xffffffffu) {
+                continue; /* a slot some lane reserved and did not fill */
+            }
+            auto it = progReports.find(m.id);
+            if (it == progReports.end()) {
+                std::vector<ProgReport> reps;
+                if (m.id % INSTR_ALIGN || m.id < sizeof(RoseEngine) || m.id >= bcLen ||
+                    !collectProgramReports(this, m.id, &reps)) {
+                    return HS_UNKNOWN_ERROR; /* a program with a state-carrying opcode (or a corrupt record) */
+                }
+                it = progReports.emplace(m.id, std::move(reps)).first;
+            }
+            for (const ProgReport &rp : it->second) {
+                if (m.to < rp.min_bound || m.to > rp.max_bound) {
+                    continue; /* CHECK_BOUNDS (hs_expr_ext min_offset / max_offset) */
+                }
+                DevMatch o = m;
+                o.id = rp.onmatch;
+                o.to = (u64)((long long)m.to + rp.offset_adjust) | (rp.logical ? LKEY_RECORD : 0);
+                out.push_back(o);
+            }
+        }
+        v->swap(out);
+    }
+    if (comb.any()) {
+        postprocessCombinations(comb, exhaustible, v, lengths, nblocks);
+    } else {
+        v->resize(postprocessRecords(exhaustible, v->data(), v->size()));
+    }
+    return HS_SUCCESS;
+}
+
 } // namespace hsb
 
 extern "C" hs_error_t hs_b200_postprocess_matches(const hs_database_t *db, hs_b200_match_t *recs,
@@ -423,14 +522,8 @@ extern "C" hs_error_t hs_b200_postprocess_matches(const hs_database_t *db, hs_b2
     if (hsb::dbRose(db)->ckeyCount) {
         return HS_INVALID; /* combination reports need the block lengths: hs_b200_postprocess_blocks */
     }
-    std::unordered_set<hsb::u32> ex;
-    hs_error_t r = hsb::collectExhaustible(db, &ex);
-    if (r != HS_SUCCESS) {
-        return r;
-    }
-    static_assert(sizeof(hsb::MatchRec) == sizeof(hs_b200_match_t), "record layout");
-    *nout = hsb::postprocessRecords(ex, (hsb::MatchRec *)recs, n);
-    return HS_SUCCESS;
+    /* without combinations no record is added: the result fits where the records were */
+    return hs_b200_postprocess_blocks(db, recs, n, nullptr, 0, recs, n, nout);
 }
 
 extern "C" hs_error_t hs_b200_postprocess_blocks(const hs_database_t *db, const hs_b200_match_t *recs, size_t n,
@@ -443,25 +536,25 @@ extern "C" hs_error_t hs_b200_postprocess_blocks(const hs_database_t *db, const 
     if (h->magic != hsb::DB_MAGIC) {
         return HS_INVALID;
     }
-    std::unordered_set<hsb::u32> ex;
-    hsb::Combinations cb;
-    hs_error_t r = hsb::collectExhaustible(db, &ex, &cb.lkeyReport);
+    hsb::ReportRules rules;
+    hs_error_t r = hsb::loadReportRules(db, &rules);
     if (r != HS_SUCCESS) {
         return r;
     }
-    std::vector<hsb::MatchRec> v((const hsb::MatchRec *)recs, (const hsb::MatchRec *)recs + n);
-    if (hsb::dbRose(db)->ckeyCount) {
-        hsb::loadCombinations(hsb::dbRose(db), &cb);
-        hsb::postprocessCombinations(cb, ex, &v, lengths, nblocks);
-    } else {
-        v.resize(hsb::postprocessRecords(ex, v.data(), v.size()));
+    if (rules.shape != hsb::SHAPE_PURE_LITERAL) {
+        return HS_ARCH_ERROR; /* engine records are resolved by the scan entry points only */
+    }
+    std::vector<hsb::DevMatch> v((const hsb::DevMatch *)recs, (const hsb::DevMatch *)recs + n);
+    r = rules.deliver(&v, lengths, nblocks);
+    if (r != HS_SUCCESS) {
+        return r;
     }
     *nout = v.size();
     if (v.size() > cap) {
         return HS_INSUFFICIENT_SPACE;
     }
     if (!v.empty()) {
-        memcpy(out, v.data(), v.size() * sizeof(hsb::MatchRec));
+        memcpy(out, v.data(), v.size() * sizeof(hsb::DevMatch));
     }
     return HS_SUCCESS;
 }

@@ -1,10 +1,10 @@
 /*
- * db_walk.h -- host-side walks over a literal database's bytecode: enumerate
- * the literal tails held in the hash-confirm structures
- * (src/fdr/fdr_confirm.h:36-94), find the reports that carry an exhaustion key
- * (HS_FLAG_SINGLEMATCH; REPORT_EXHAUST, src/rose/rose_program.h:485), and apply
- * the order-dependent report rules -- logical combinations included -- to a list of
- * raw match records.
+ * db_walk.h -- how a database's raw match records become delivered matches: the
+ * database's shape, the walk over its report programs (the literal programs held in
+ * the hash-confirm structures, src/fdr/fdr_confirm.h:36-94, and the engine's report
+ * programs), the reports that carry an exhaustion key (HS_FLAG_SINGLEMATCH;
+ * REPORT_EXHAUST, src/rose/rose_program.h:485), and the order-dependent report
+ * rules -- logical combinations included -- applied to a list of raw records.
  */
 #ifndef HSB200_DB_WALK_H
 #define HSB200_DB_WALK_H
@@ -19,20 +19,26 @@
 
 namespace hsb {
 
+static_assert(sizeof(DevMatch) == sizeof(hs_b200_match_t) && offsetof(DevMatch, id) == offsetof(hs_b200_match_t, id) &&
+                  offsetof(DevMatch, block) == offsetof(hs_b200_match_t, block) &&
+                  offsetof(DevMatch, to) == offsetof(hs_b200_match_t, to),
+              "record layout");
+
+/* Delivery order of records: by block, then end offset, then id. */
+struct RecordOrder {
+    bool operator()(const DevMatch &a, const DevMatch &b) const {
+        if (a.block != b.block) return a.block < b.block;
+        if (a.to != b.to) return a.to < b.to;
+        return a.id < b.id;
+    }
+};
+
 struct LitTail {
     u64 v, msk;
     u32 size;
     u32 bucket;
 };
 
-struct MatchRec { /* == hs_b200_match_t */
-    u32 id;
-    u32 block;
-    u64 to;
-};
-
-/* Both return false if a program holds an opcode the device does not implement
- * (callers refuse the database with HS_ARCH_ERROR instead of failing mid-scan). */
 /* a report instruction of a program: what it raises, and the bounds on the match end (CHECK_BOUNDS,
  * src/rose/program_runtime.c:2319-2326) under which the program reaches it */
 struct ProgReport {
@@ -44,15 +50,6 @@ struct ProgReport {
 /* lkey -> the report id whose report block sets it (a SET_LOGICAL after a report instruction; a quiet
  * sub-expression has none) */
 typedef std::unordered_map<u32, u32> LkeyReports;
-/* catchUp: the program belongs to a database with an outfix, where CATCH_UP only orders the outfix's
- * reports before the literal's -- which the host's ordering does -- and is accepted */
-bool collectProgramReports(const u8 *bc, u32 bcLen, u32 prog, std::unordered_set<u32> *ex,
-                           std::vector<ProgReport> *reports = nullptr, /* every report instruction, in program order */
-                           LkeyReports *lkeys = nullptr, bool catchUp = false);
-
-bool walkConfirm(const u8 *bc, u32 bcLen, u32 confOff, u32 nBuckets,
-                 std::unordered_set<u32> *ex, std::vector<LitTail> *tails, LkeyReports *lkeys = nullptr,
-                 bool catchUp = false);
 
 /* Logical combinations of a database (RoseEngine.ckeyCount != 0): the tables the reference evaluates
  * per block (src/rose/program_runtime.c:2026-2120, src/report.h:190-245), copied from the bytecode. */
@@ -65,31 +62,58 @@ struct Combinations {
     LkeyReports lkeyReport;
     bool any() const { return !combs.empty(); }
 };
-void loadCombinations(const RoseEngine *r, Combinations *cb);
 
-/* The bit of MatchRec.to that marks a logical-key record (id = lkey): written by SET_LOGICAL, consumed by
- * postprocessCombinations.  No match offset reaches 2^63. */
+/* The bit of DevMatch.to that marks a logical-key record (id = lkey): written by SET_LOGICAL, consumed by
+ * the combination rules.  No match offset reaches 2^63. */
 static const u64 LKEY_RECORD = 1ull << 63;
-/* The bit of MatchRec.to that marks an engine's record in a database with a literal matcher and an
+/* The bit of DevMatch.to that marks an engine's record in a database with a literal matcher and an
  * outfix: its id is a report PROGRAM offset, resolved on the host; the literal records carry report ids. */
 static const u64 ENGINE_RECORD = 1ull << 62;
 
-/** Reports compiled with HS_FLAG_SINGLEMATCH in a pure-literal database. */
-hs_error_t collectExhaustible(const hs_database_t *db, std::unordered_set<u32> *ex, LkeyReports *lkeys = nullptr);
+/* The database shapes the device runs (DESIGN.md sections 10a, 10d). */
+enum DbShape {
+    SHAPE_UNSUPPORTED = 0, /* needs the full rose interpreter (SURVEY.md section 8f rank 1): not in this build */
+    SHAPE_PURE_LITERAL,    /* the floating literal matcher alone */
+    SHAPE_SOLE_OUTFIX,     /* one engine over the whole block, no literal matcher */
+    SHAPE_LITERALS_OUTFIX, /* the floating literal matcher beside one outfix (FULL_ROSE, block mode) */
+};
+DbShape dbShape(const hs_database_t *db);
 
-/** Order records for delivery and apply the order-dependent report rules the
- * device skipped: one report per (block, id, to) (dedupe, src/report.h:55-119)
- * and, for HS_FLAG_SINGLEMATCH reports, only the first match per block
- * (exhaustion keys, src/report.h:121-147, program_runtime.c:464-481).
- * Returns the number of records kept (in place, sorted by (block, to, id)). */
-size_t postprocessRecords(const std::unordered_set<u32> &exhaustible, MatchRec *m, size_t n);
+/* The report rules of one database.  Borrows the database's bytecode, which must outlive it. */
+struct ReportRules {
+    DbShape shape = SHAPE_UNSUPPORTED;
+    bool hasDedupe = false;                /* RoseEngine.dkeyCount != 0 */
+    std::unordered_set<u32> exhaustible;   /* report ids under HS_FLAG_SINGLEMATCH (an engine's: found with its
+                                            * programs as they are first met) */
+    Combinations comb;
+    const u8 *bc = nullptr;
+    u32 bcLen = 0;
+    /* an engine's report program offset -> the report instructions it reaches, filled as programs are met */
+    std::unordered_map<u32, std::vector<ProgReport>> progReports;
 
-/* The same for a database with logical combinations, whose records include logical-key records:
- * the records of blocks [0, nblocks) (block i is lengths[i] bytes long) in delivery order -- by
- * (block, to), at one offset the reports by id and then the combinations it completes, by ckey --
- * with the combination reports added and the logical-key records gone. */
-void postprocessCombinations(const Combinations &cb, const std::unordered_set<u32> &exhaustible,
-                             std::vector<MatchRec> *v, const u32 *lengths, size_t nblocks);
+    /* Without dedupe keys, exhaustion keys, combinations or engine records, the raw record count is the
+     * delivered count. */
+    bool rawCountDelivered() const {
+        return shape == SHAPE_PURE_LITERAL && exhaustible.empty() && !hasDedupe && !comb.any();
+    }
+
+    /* Records of a scan in delivery order, (block, to, id), with the report rules the device skipped
+     * applied.  An engine's records carry report PROGRAM offsets (and the padding of the lanes' reserved
+     * slots) -- all of a single-outfix database's records, and those tagged ENGINE_RECORD beside a literal
+     * matcher; each is replaced by the reports its program raises -- roseReportAdaptor -> roseRunProgram
+     * (src/rose/match.c:611-633) -- with CHECK_BOUNDS and offset_adjust applied, and the literals' records
+     * join them as they are.  Then one report per (block, id, to) (dedupe, src/report.h:55-119) and, for
+     * HS_FLAG_SINGLEMATCH reports, only the first match per block (exhaustion keys, src/report.h:121-147,
+     * program_runtime.c:464-481); with logical combinations, the combination reports are added and the
+     * logical-key records removed, which needs the block lengths (lengths[0, nblocks)). */
+    hs_error_t deliver(std::vector<DevMatch> *v, const u32 *lengths, size_t nblocks);
+};
+
+/* Classify the database and walk the floating matcher's literal programs once: HS_ARCH_ERROR for a shape
+ * the device does not run, or for a program that holds an opcode the device does not implement (callers
+ * refuse the database instead of failing mid-scan).  tails, if given, receives the LitInfo v/msk/size and
+ * bucket of every literal of an FDR or Teddy matcher. */
+hs_error_t loadReportRules(const hs_database_t *db, ReportRules *rules, std::vector<LitTail> *tails = nullptr);
 
 } // namespace hsb
 #endif

@@ -29,7 +29,7 @@ struct PairTables {
     double modelRate;   /* modelled candidates per byte on uniformly random printable ASCII */
 };
 
-/* tails: LitInfo v/msk/size + bucket of every literal (walkConfirm); slotBase:
+/* tails: LitInfo v/msk/size + bucket of every literal (loadReportRules); slotBase:
  * 0 = suffix slots 0..3 (sets with one-byte literals), 1 = slots 1..4. */
 void buildPairTables(const std::vector<LitTail> &tails, u32 slotBase, PairTables *out,
                      u32 maxClass0 = 32, u32 maxClass1 = 32);

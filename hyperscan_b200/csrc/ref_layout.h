@@ -593,6 +593,14 @@ static inline u32 fatbitSize(u32 total_bits) {
     return m < 32 ? 32 : m;
 }
 
+/* ---- not a reference structure: one match record as the device writes it and the host
+ * orders it, identical to hs_b200_match_t (include/hs_b200.h; pinned in db_walk.h) */
+struct DevMatch {
+    u32 id;
+    u32 block;
+    u64 to;
+};
+
 } // namespace hsb
 
 #endif
