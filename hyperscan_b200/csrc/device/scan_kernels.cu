@@ -539,15 +539,12 @@ __device__ __forceinline__ void sts32(u32 addr, u32 x) {
 #endif
 
 /* OR the 128-bit stream E[0..3] (one entry per word of the lane, all at the
- * same in-word position) into a[] at byte offset O (0..4): one funnel shift
+ * same in-word position) into a[] at byte offset O (0..3): one funnel shift
  * per output word instead of two shifts per entry. */
 template <int O> __device__ __forceinline__ void orStream(u32 (&a)[6], const u32 (&E)[4]) {
     if constexpr (O == 0) {
 #pragma unroll
         for (int k = 0; k < 4; k++) a[k] |= E[k];
-    } else if constexpr (O == 4) {
-#pragma unroll
-        for (int k = 0; k < 4; k++) a[k + 1] |= E[k];
     } else {
         a[0] |= E[0] << (8 * O);
 #pragma unroll
@@ -925,9 +922,12 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelWide(const HSB_GRID_CONSTAN
  *   pair row (c1 << 5 | c0) (128 B): [u32 entry: 4 slots x 8 buckets] x 32 lanes
  *
  * so the pair address is ONE logic op of the two class words and every lookup is
- * PRMT/LOP3 + LDS.  Sample at x = bytes (x, x+1) keyed (c0(byte x), c1(byte x+1));
- * entry byte i says which buckets cannot END at x + i + SB (SB = slot base: 1 when every
- * literal has at least two bytes, so that all four samples see both bytes of a pair).
+ * PRMT/LOP3 + LDS.  A sample is keyed (c0(first byte), c1(second byte)); entry byte i
+ * says which buckets cannot END i + SB bytes after the FIRST byte (SB = slot base: 1 when
+ * every literal has at least two bytes, so that all four slots see both bytes of a pair).
+ * The sample is placed so that its entry applies to the end positions x .. x + 3: SB = 1
+ * keys x by the bytes (x - 1, x) -- one class lookup per byte of the lane, the class word
+ * of the byte before it comes from the left neighbour --, SB = 0 by (x, x + 1).
  * Candidates: per-warp queue -> prefilter bitmaps -> candidate list in HBM ->
  * confirmKernel (the hot kernel carries no confirm code). */
 
@@ -952,20 +952,28 @@ __device__ __forceinline__ u32 pairIndex(u32 a, u32 b) {
 #endif
 }
 
-/* Shift-OR contributions of one lane's 16 positions: w[0..3] the lane's bytes,
- * w[4] the word after them.  a[0..3]: own end positions, a[4]: overflow into the
- * next lane (bit set = bucket impossible). */
-template <int SB>
-__device__ __forceinline__ void pairFilter(const u32 (&w)[5], u32 clsAddr, u32 laneOff, u32 (&a)[6]) {
-    u32 E[17];
+/* Class words of the 16 bytes of v into E[O .. O + 15] (the lane's own copies: row
+ * offset byte << 8 | laneOff, conflict free). */
+template <int O>
+__device__ __forceinline__ void laneClasses(const uint4 v, u32 clsAddr, u32 laneOff, u32 (&E)[17]) {
+    const u32 w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
     for (int k = 0; k < 4; k++) {
 #pragma unroll
         for (int r = 0; r < 4; r++) {
-            E[4 * k + r] = lds32(clsAddr + __byte_perm(w[k], laneOff, 0x5504 + (r << 4)));
+            E[O + 4 * k + r] = lds32(clsAddr + __byte_perm(w[k], laneOff, 0x5504 + (r << 4)));
         }
     }
-    E[16] = lds32(clsAddr + __byte_perm(w[4], laneOff, 0x5504));
+}
+
+/* Shift-OR contributions of one lane's 16 positions from the class words E[0..16] of 17
+ * consecutive bytes: sample j keyed (E[j], E[j + 1]) applies to the lane's end positions
+ * j .. j + 3 (SB = 1: E[0] is the byte before the lane; SB = 0: E[16] the byte after it).
+ * a[0..3]: own end positions, a[4]: overflow into the next lane (bit set = bucket
+ * impossible).  The pair lookups are conflict free as long as the lanes' first operands
+ * carry lane fields that are a permutation of 0..31: E[0] of SB = 1 is the left
+ * neighbour's word, a rotation by one. */
+__device__ __forceinline__ void pairFilter(const u32 (&E)[17], u32 clsAddr, u32 (&a)[6]) {
 #pragma unroll
     for (int i = 0; i < 6; i++) {
         a[i] = 0;
@@ -976,14 +984,13 @@ __device__ __forceinline__ void pairFilter(const u32 (&w)[5], u32 clsAddr, u32 l
         u32 P[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) {
-            /* l << 2 | c0(x) << 7 from the first byte's word, c1(x + 1) << 12 from the second's */
+            /* lane << 2 | c0 << 7 from the first byte's word, c1 << 12 from the second's */
             P[k] = lds32(pairAddr + pairIndex(E[4 * k + r], E[4 * k + r + 1]));
         }
-        if (r + SB == 0) orStream<0>(a, P);
-        if (r + SB == 1) orStream<1>(a, P);
-        if (r + SB == 2) orStream<2>(a, P);
-        if (r + SB == 3) orStream<3>(a, P);
-        if (r + SB == 4) orStream<4>(a, P);
+        if (r == 0) orStream<0>(a, P);
+        if (r == 1) orStream<1>(a, P);
+        if (r == 2) orStream<2>(a, P);
+        if (r == 3) orStream<3>(a, P);
     }
 }
 
@@ -1136,57 +1143,15 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelPair(const HSB_GRID_CONSTAN
     const u32 warp = threadIdx.x >> 5;
     const u32 nwarps = blockDim.x >> 5;
 
-    /* expand the tables: p.table = 256 class words, then 1024 pair entries; the
-     * (32 KiB) prefilter bitmap, if any, fills the class rows' upper halves */
-    {
-        const u32 *g = reinterpret_cast<const u32 *>(p.table);
-        const u32 *bm = reinterpret_cast<const u32 *>(p.bitmap);
-        u32 *s = reinterpret_cast<u32 *>(smem);
-        const bool keyed = p.bitmapBytes != 0;
-        for (u32 i = threadIdx.x; i < 256 * 64; i += blockDim.x) {
-            const u32 row = i >> 6, l = i & 31;
-            if ((i >> 5) & 1) {
-                s[i] = keyed ? __ldg(bm + row * 32 + l) : 0u;
-            } else {
-                s[i] = __ldg(g + row) | (l << 2);
-            }
-        }
-        u32 *sp = s + 256 * 64;
-        for (u32 i = threadIdx.x; i < p.pairBytes / 4; i += blockDim.x) {
-            sp[i] = __ldg(g + 256 + (i >> 5));
-        }
-    }
-    __syncthreads();
-
-    const u32 clsAddr = smemAddr(smem);
-    const u32 bitmapAddr = clsAddr + 128;
-    const u32 laneOff = lane * 4;
-    const u32 qAddr = clsAddr + PAIR_CLASS_BYTES + p.pairBytes + warp * PairQueue::WARP_BYTES;
-
     /* this warp's contiguous run of tiles */
     const u32 gwarp = blockIdx.x * nwarps + warp;
     const u32 totalWarps = gridDim.x * nwarps;
     const u32 q = p.ntiles / totalWarps, rem = p.ntiles % totalWarps;
     const u32 myCount = q + (gwarp < rem ? 1u : 0u);
     const u32 myFirst = p.tileFirst + gwarp * q + min(gwarp, rem);
-    if (myCount == 0) {
-        return;
-    }
     const u64 runStart = (u64)myFirst * p.tileBytes;
-    u64 runEnd = runStart + (u64)myCount * p.tileBytes;
-    if (runEnd > p.corpusBytes) {
-        runEnd = p.corpusBytes;
-    }
-    const u32 nsteps = (u32)((runEnd - runStart + 511) >> 9);
     const u8 *ptr = p.corpus + runStart + lane * 16; /* this lane's 16 bytes of the current step */
     const u8 *const endPtr = p.corpus + p.readableEnd;
-    if (lane == 0) {
-        sts64(qAddr + PairQueue::RUN_START, (u32)runStart, (u32)(runStart >> 32));
-    }
-
-    u32 carry = 0; /* lane 31's overflow of the previous step */
-    u32 stats[3] = {0, 0, 0};
-    u32 qn = 0;
 
     auto load = [&](const u8 *src, bool guard) -> uint4 {
         uint4 r = make_uint4(0, 0, 0, 0);
@@ -1195,27 +1160,115 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelPair(const HSB_GRID_CONSTAN
         }
         return r;
     };
-    const size_t pfBytes = (size_t)p.pfDist * 512 + lane * 48; /* even lanes: 16 x 128 B, 2 KiB */
-    uint4 nxt = load(ptr, true);
+    /* L2 prefetch of the 2 KiB (four steps) that lie pfDist steps after the lane's
+     * position `at`: even lanes, 16 x 128 B */
+    const size_t pfBytes = (size_t)p.pfDist * 512 + lane * 48;
+    auto prefetchAhead = [&](const u8 *at) {
+        if ((lane & 1) == 0) {
+            const u8 *pf = at + pfBytes;
+            if (pf < endPtr) {
+                prefetchL2(pf);
+            }
+        }
+    };
+
+    /* the stream starts before the tables are expanded: steps 0 and 1, the 16 bytes
+     * before the run and the first prefetch are in flight during the expansion */
+    uint4 cur = make_uint4(0, 0, 0, 0), nxt = cur, hv = cur;
+    if (myCount != 0) {
+        cur = load(ptr, true);
+        nxt = load(ptr + 512, true);
+        if (runStart != 0) {
+            hv = __ldg(reinterpret_cast<const uint4 *>(p.corpus + runStart - 16));
+        }
+        prefetchAhead(ptr);
+    }
+
+    /* expand the tables: p.table = 256 class words, then 1024 pair entries; the
+     * (32 KiB) prefilter bitmap, if any, fills the class rows' upper halves.  In 16-byte
+     * units: a class row is 8 units of {c | l << 2} for four lanes l and 8 units of the
+     * bitmap, a pair row 8 units of its entry four times */
+    {
+        const u32 *g = reinterpret_cast<const u32 *>(p.table);
+        const uint4 *bm = reinterpret_cast<const uint4 *>(p.bitmap);
+        const u32 sBase = smemAddr(smem);
+        const bool keyed = p.bitmapBytes != 0;
+        for (u32 u = threadIdx.x; u < PAIR_CLASS_BYTES / 32; u += blockDim.x) {
+            const u32 c = __ldg(g + (u >> 3));
+            const uint4 b = keyed ? __ldg(bm + u) : make_uint4(0, 0, 0, 0);
+            const u32 a = sBase + (u >> 3) * 256 + (u & 7) * 16, l = (u & 7) * 16;
+            sts128(a, c | l, c | (l + 4), c | (l + 8), c | (l + 12));
+            sts128(a + 128, b.x, b.y, b.z, b.w);
+        }
+        for (u32 u = threadIdx.x; u < p.pairBytes / 16; u += blockDim.x) {
+            const u32 e = __ldg(g + 256 + (u >> 3));
+            sts128(sBase + PAIR_CLASS_BYTES + u * 16, e, e, e, e);
+        }
+    }
+    __syncthreads();
+
+    const u32 clsAddr = smemAddr(smem);
+    const u32 bitmapAddr = clsAddr + 128;
+    const u32 laneOff = lane * 4;
+    const u32 qAddr = clsAddr + PAIR_CLASS_BYTES + p.pairBytes + warp * PairQueue::WARP_BYTES;
+    if (myCount == 0) {
+        return;
+    }
+    u64 runEnd = runStart + (u64)myCount * p.tileBytes;
+    if (runEnd > p.corpusBytes) {
+        runEnd = p.corpusBytes;
+    }
+    const u32 nsteps = (u32)((runEnd - runStart + 511) >> 9);
+    if (lane == 0) {
+        sts64(qAddr + PairQueue::RUN_START, (u32)runStart, (u32)(runStart >> 32));
+    }
+
+    u32 carry = 0; /* lane 31's overflow of the previous step */
+    u32 stats[3] = {0, 0, 0};
+    u32 qn = 0;
+
+    /* SB = 1: lane 31's last class word of the previous step (lane field 31: the pair
+     * lookups stay a rotation of the banks).  Entering the run at the start of the corpus
+     * byte 0x00 stands in for the byte before it, as it does in confirm (confValAt); a slot
+     * that reaches before a literal's first byte never constrains its bucket anyway. */
+    u32 prevCls = SB == 1 ? lds32(clsAddr + 31 * 4) : 0u;
     u32 prevW = 0; /* heavy: the last word of the previous step (own lane's; lane 31's is the one used) */
     if (runStart != 0) {
         /* state entering the run: the 16 bytes before it, as "lane -1" */
-        const uint4 hv = __ldg(reinterpret_cast<const uint4 *>(p.corpus + runStart - 16));
-        const u32 hw[5] = {hv.x, hv.y, hv.z, hv.w, __shfl_sync(0xffffffffu, nxt.x, 0)};
+        u32 hE[17];
+        if constexpr (SB == 1) {
+            laneClasses<1>(hv, clsAddr, laneOff, hE);
+            hE[0] = hE[1]; /* sample 0 does not overflow */
+            prevCls = __shfl_sync(0xffffffffu, hE[16], 31);
+        } else {
+            laneClasses<0>(hv, clsAddr, laneOff, hE);
+            hE[16] = lds32(clsAddr + __byte_perm(__shfl_sync(0xffffffffu, cur.x, 0), laneOff, 0x5504));
+        }
         u32 ha[6];
-        pairFilter<SB>(hw, clsAddr, laneOff, ha);
+        pairFilter(hE, clsAddr, ha);
         carry = ha[4];
         prevW = hv.w;
     }
     u32 step = 0;
     u32 prevRecv = carry;
-    /* one 512-byte step: cur = the lane's 16 bytes, nextFirst = first word of the NEXT
-     * step (lane 0 hands it to lane 31 in the rotate shuffle) */
-    auto compute = [&](const uint4 cur, const u32 nextFirst, const u32 chunk) {
-        const u32 w4 = __shfl_sync(0xffffffffu, lane == 0 ? nextFirst : cur.x, (lane + 1) & 31);
-        const u32 w[5] = {cur.x, cur.y, cur.z, cur.w, w4};
+    /* one 512-byte step: v = the lane's 16 bytes, nextFirst = first word of the NEXT
+     * step (SB = 0: lane 0 hands it to lane 31 in the rotate shuffle) */
+    auto compute = [&](const uint4 v, const u32 nextFirst, const u32 chunk) {
+        u32 E[17];
+        if constexpr (SB == 1) {
+            laneClasses<1>(v, clsAddr, laneOff, E);
+            /* the class word of the byte before the lane: the left neighbour's last (ONE
+             * rotate shuffle); lane 0 takes lane 31's of the previous step */
+            const u32 left = __shfl_sync(0xffffffffu, E[16], (lane + 31) & 31);
+            E[0] = lane == 0 ? prevCls : left;
+            prevCls = left;
+        } else {
+            const u32 w4 = __shfl_sync(0xffffffffu, lane == 0 ? nextFirst : v.x, (lane + 1) & 31);
+            laneClasses<0>(v, clsAddr, laneOff, E);
+            E[16] = lds32(clsAddr + __byte_perm(w4, laneOff, 0x5504));
+        }
         u32 a[6];
-        pairFilter<SB>(w, clsAddr, laneOff, a);
+        pairFilter(E, clsAddr, a);
         /* ONE rotate-by-one shuffle: lanes 1..31 receive their left neighbour's
          * overflow, lane 0 receives lane 31's = the carry into the NEXT step */
         const u32 recv = __shfl_sync(0xffffffffu, a[4], (lane + 31) & 31);
@@ -1230,8 +1283,8 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelPair(const HSB_GRID_CONSTAN
                  * entries are drained at once */
                 /* the word before the lane's: the left neighbour's last, lane 0: lane 31's
                  * of the previous step (kept in a register, no corpus read) */
-                const u32 pw = __shfl_sync(0xffffffffu, lane == 31 ? prevW : cur.w, (lane + 31) & 31);
-                const u32 wv[5] = {pw, cur.x, cur.y, cur.z, cur.w};
+                const u32 pw = __shfl_sync(0xffffffffu, lane == 31 ? prevW : v.w, (lane + 31) & 31);
+                const u32 wv[5] = {pw, v.x, v.y, v.z, v.w};
 #pragma unroll
                 for (int k = 0; k < 4; k++) {
                     const u32 m = ~a[k];
@@ -1251,7 +1304,7 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelPair(const HSB_GRID_CONSTAN
                     }
                 }
             }
-            prevW = cur.w;
+            prevW = v.w;
             return;
         }
         const u32 bal = __ballot_sync(0xffffffffu, all != 0xffffffffu);
@@ -1270,26 +1323,19 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelPair(const HSB_GRID_CONSTAN
             }
         }
     };
-    /* Register pipeline two steps deep: the first thing a step does is hand lane 31
-     * the next step's first word, so a load issued only one step ahead would be waited
-     * for at once (long-scoreboard stalls of a full L2 round trip per step).  The load
-     * issued in step s fetches step s + 2; it needs no bounds check while that whole
-     * step is readable for every lane -- everywhere but at the very end of the corpus. */
+    /* Register pipeline two steps deep (cur = step 0 and nxt = step 1 are in flight since
+     * before the barrier): with SB = 0 the first thing a step does is hand lane 31 the
+     * next step's first word, so a load issued only one step ahead would be waited for at
+     * once (long-scoreboard stalls of a full L2 round trip per step).  The load issued in
+     * step s fetches step s + 2; it needs no bounds check while that whole step is
+     * readable for every lane -- everywhere but at the very end of the corpus. */
     const u64 readableSteps = (p.readableEnd - runStart) >> 9;
     const u32 nFast = readableSteps >= (u64)nsteps + 2 ? nsteps : (readableSteps > 2 ? (u32)readableSteps - 2 : 0);
-    uint4 cur = nxt;                    /* step 0 */
-    nxt = load(ptr + 512, true);        /* step 1 */
     /* main loop: four steps per iteration (loads at immediate offsets, no register
-     * moves between steps) and ONE L2 prefetch of the 2 KiB that lie pfDist steps ahead
-     * (even lanes, 16 x 128 B) */
+     * moves between steps) and ONE L2 prefetch, at its end, of the next iteration's
+     * 2 KiB pfDist steps ahead (the first iteration's went out before the barrier) */
 #pragma unroll 1
     for (; step + 4 <= nFast; step += 4, ptr += 2048) {
-        if ((lane & 1) == 0) {
-            const u8 *pf = ptr + pfBytes;
-            if (pf < endPtr) {
-                prefetchL2(pf);
-            }
-        }
         const uint4 n2 = ldCs128(ptr + 1024);
         compute(cur, nxt.x, step * 32 + lane);
         const uint4 n3 = ldCs128(ptr + 1536);
@@ -1298,6 +1344,7 @@ __global__ void __launch_bounds__(MAXT, 1) scanKernelPair(const HSB_GRID_CONSTAN
         compute(n2, n3.x, step * 32 + 64 + lane);
         nxt = ldCs128(ptr + 2560);
         compute(n3, cur.x, step * 32 + 96 + lane);
+        prefetchAhead(ptr + 2048);
     }
 #pragma unroll 1
     for (; step < nsteps; step++, ptr += 512) {
