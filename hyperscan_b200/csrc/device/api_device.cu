@@ -50,15 +50,16 @@ std::atomic<unsigned long long> g_launches{0};
 struct RuntimeOpts {
     int warps = 0;           /* per CTA; 0 = 28 (896 threads x 72 registers) */
     int tileBytes = 1024;
-    int pfDist = 4;          /* L2 prefetch distance (kernels.h ScanParams.pfDist).  On an H100 SXM (700 W)
-                              * 4 against 8 took 17 % off the Teddy-48 and noodle kernels and 3 % off FDR with
-                              * 1 000 literals, and left 5 000 / 50 000 literals unchanged (1 GiB, tools/sweep.py);
-                              * on a card limited to 400 W, whose clock is power-bound, 4 and 8 are level */
+    int pfDist = -1;         /* L2 prefetch distance (kernels.h ScanParams.pfDist); -1 = per kernel: 2 steps
+                              * (1 KiB) for the pair kernel, 4 for the others.  On an H100 SXM (700 W) 4 against 8
+                              * took 17 % off the Teddy-48 and noodle kernels and left 5 000 / 50 000 literals
+                              * unchanged (1 GiB, tools/sweep.py); the pair kernel at 2 steps against 4 took 2-6 %
+                              * off 96 (fat Teddy), 200 and 1 000 literals (DESIGN.md section 3.3); on a card
+                              * limited to 400 W, whose clock is power-bound, 4 and 8 are level */
     int gram = 1;            /* FDR sets: 1 = class 4-gram first stage (FK_GRAM4) for sets that would fill the
                               * pair kernel's 32 KiB bitmap beyond 10 % (all literals >= 4 bytes), 2 = whenever
                               * possible, 0 = never */
-    int heavy = 1;           /* FK_PAIR32 candidate path: 0 = per-lane entries, 2 = per-word entries (sets that
-                              * pass many candidates), 1 = by the modelled first-stage rate */
+    int heavy = 1;           /* FK_PAIR32 candidate path: 1 (and 2) = per-word entries, 0 = per-lane entries */
     int dfaIlp = 1;          /* DFA kernels: blocks walked by one lane at a time; 2 = two interleaved state chains
                               * per lane (half the warps for the same block count) */
     int chunkMB = 128;       /* host->device pipeline granularity */
@@ -104,7 +105,6 @@ struct DevImage {
     u32 nfaOffset = 0, nfaLength = 0;   /* the outfix engine (bytecode offset, NFA.length), alone (FK_OUTFIX) or
                                          * beside the literal matcher; nfaLength == 0: none */
     DfaParams nfaParams;                /* ... and what launchDfa needs to know about it */
-    double pairRate = 0;     /* FK_PAIR32: modelled first-stage candidates per byte (printable ASCII) */
     u8 *d_bitmap2 = nullptr; /* second level (HBM / L2) for large literal sets */
     u32 bitmap2Shift = 0;
     int kind = FK_BYTE32;
@@ -564,7 +564,6 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
         PairTables pt;
         buildPairTables(tails, (u32)im->slotBase, &pt, 32, 32);
         im->pairBytes = pt.nClass1 * 4096;
-        im->pairRate = pt.modelRate;
         if (getenv("HSB200_TRACE")) {
             fprintf(stderr, "[hs_b200] class-pair tables: %u x %u classes, modelled %.4f candidates/byte, "
                             "%zu prefilter keys\n", pt.nClass0, pt.nClass1, pt.modelRate, keys.size());
@@ -896,18 +895,19 @@ hs_error_t planScan(const hs_scratch *s, const DevImage *im, ScanPlan *pl) {
     }
     pl->cfg.kind = im->kind;
     pl->cfg.slotBase = im->slotBase;
-    /* pair-kernel candidate path: per-lane queue entries while candidates are rare; one entry
-     * per word with candidates for sets that saturate the first stage (heavy=2 forces it).
-     * The modelled rate assumes independent slots and is ~30x below the observed one:
-     * 0.0015 modelled is ~40 candidates per KiB, where the per-word path starts to win */
-    pl->cfg.heavy = im->kind == FK_PAIR32 && (g_opts.heavy == 2 || (g_opts.heavy == 1 && im->pairRate > 0.0015));
+    /* pair-kernel candidate path: one queue entry per word with candidates.  Its drain needs
+     * no corpus read and reserves list slots once per warp, and it was level or faster on
+     * every set measured, from 0.015 to 7 candidates per KiB (DESIGN.md section 3.3);
+     * heavy=0 selects the per-lane entries */
+    pl->cfg.heavy = im->kind == FK_PAIR32 && g_opts.heavy != 0;
     pl->cfg.grid = s->smCount;
     pl->cfg.warps = warps;
     pl->tileBytes = (u32)std::max(512, g_opts.tileBytes) & ~511u;
     if (wide) {
         pl->tileBytes = std::max(1024u, pl->tileBytes & ~1023u); /* a warp-iteration covers 1 KiB */
     }
-    pl->pfDist = (u32)std::max(0, std::min(64, g_opts.pfDist));
+    const int pfDist = g_opts.pfDist >= 0 ? g_opts.pfDist : im->kind == FK_PAIR32 ? 2 : 4;
+    pl->pfDist = (u32)std::min(64, pfDist);
     return HS_SUCCESS;
 }
 

@@ -573,11 +573,11 @@ hs_error_t hs_b200_test_compile_programs(const char *const *lits, const size_t *
 
 /* Runtime tunables (process-wide; also HSB200_* environment variables): the scan
  * geometry -- "warps" per CTA (0 = 28), "tile_bytes", "pf_dist" (L2 prefetch
- * distance), "chunk_mb" (host->device pipeline granularity), "initial_ring" (match
- * records) -- and switches that force either side of a choice the library makes
- * from the database: "gram" (class 4-gram first stage for FDR sets: 0 never, 1 from
- * 10 000 prefilter keys, 2 whenever all literals have 4 bytes), "heavy" (class-pair
- * candidate path: per-word queue entries 0 never / 1 by the modelled rate / 2
+ * distance, -1 = the kernel's own), "chunk_mb" (host->device pipeline granularity),
+ * "initial_ring" (match records) -- and switches that force either side of a choice
+ * the library makes from the database: "gram" (class 4-gram first stage for FDR sets:
+ * 0 never, 1 from 10 000 prefilter keys, 2 whenever all literals have 4 bytes),
+ * "heavy" (class-pair candidate path: per-word queue entries 0 never / 1 and 2
  * always) and "dfa_ilp" (DFA kernels: blocks per lane, 1).  "gram" applies to
  * scratches allocated afterwards.  The defaults are the measured best (DESIGN.md
  * section 3); the others exist for A/B runs (tools/sweep.py) and tests.  Any other

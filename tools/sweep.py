@@ -17,7 +17,7 @@ from hyperscan_b200 import capi, synth  # noqa: E402
 
 DEFAULT = ("pf_dist=4;pf_dist=2;pf_dist=8;pf_dist=16;warps=24;warps=32;tile_bytes=4096;heavy=0;heavy=2;"
            "gram=0;gram=2")
-BASE = {"warps": 0, "tile_bytes": 1024, "pf_dist": 4, "heavy": 1, "gram": 1}
+BASE = {"warps": 0, "tile_bytes": 1024, "pf_dist": -1, "heavy": 1, "gram": 1}  # the library defaults
 
 
 def main():
