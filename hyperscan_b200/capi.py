@@ -144,6 +144,8 @@ def lib():
         L.hs_b200_postprocess_matches.argtypes = [vp, vp, C.c_size_t, u64p]
         L.hs_b200_postprocess_blocks.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t, u64p]
         L.hs_b200_fetch_matches.argtypes = [vp, vp, vp, C.c_size_t, u64p]
+        L.hs_b200_order_matches_async.argtypes = [vp, vp, vp, C.c_size_t, vp, vp]
+        L.hs_b200_order_records_async.argtypes = [vp, vp, vp, C.c_size_t, vp, C.c_size_t, vp, vp]
         L.hs_b200_db_info.argtypes = [vp, C.POINTER(DbInfo)]
         L.hs_b200_set_build_option.argtypes = [cp, C.c_int]
         L.hs_b200_set_runtime_option.argtypes = [cp, C.c_int]
@@ -446,6 +448,52 @@ def fetch_matches(db, scratch):
         _check(lib().hs_b200_fetch_matches(db.ptr, scratch.ptr, out.ctypes.data, out.size, C.byref(n)),
                "fetch")
     return out
+
+
+ORDER_RING_OVERFLOW = (1 << 64) - 1   # *d_count after a ring overflow (HS_B200_ORDER_RING_OVERFLOW)
+
+
+def _dev_ptr(x):
+    """Device address of a torch CUDA tensor (or of a numpy array: the SIMT emulator's "device" memory is the
+    host's), or an address given as an int; None stays NULL."""
+    if x is None:
+        return None
+    if hasattr(x, "data_ptr"):
+        if not x.is_cuda:
+            raise ValueError("expected a CUDA tensor")
+        if not x.is_contiguous():
+            raise ValueError("expected a contiguous tensor")
+        return x.data_ptr()
+    if isinstance(x, np.ndarray):
+        return x.ctypes.data
+    return int(x)
+
+
+def _capacity(out):
+    if out is None:
+        return 0
+    if hasattr(out, "data_ptr"):
+        return out.numel() * out.element_size() // MATCH_DTYPE.itemsize
+    if isinstance(out, np.ndarray):
+        return out.nbytes // MATCH_DTYPE.itemsize
+    raise ValueError("give the capacity of a raw device address explicitly")
+
+
+def order_matches_async(db, scratch, out, count, stream=None, cap=None):
+    """hs_b200_order_matches_async: the delivered matches of the last hs_b200_scan_corpus_async, ordered on the
+    device into `out` (a CUDA tensor of 16-byte records, e.g. torch.empty(n * 16, dtype=torch.uint8) or
+    int64 [n, 2]) and their count into `count` (one int64 / uint64 element), on `stream` (a cudaStream_t
+    address, e.g. torch.cuda.current_stream().cuda_stream; None = the scratch's stream).  Returns at once."""
+    cap = _capacity(out) if cap is None else int(cap)
+    _check(lib().hs_b200_order_matches_async(db.ptr, scratch.ptr, _dev_ptr(out), cap, _dev_ptr(count),
+                                             C.c_void_p(stream or 0)), "order_matches_async")
+
+
+def order_records_async(db, scratch, recs, n, out, count, stream=None, cap=None):
+    """hs_b200_order_records_async: the same for n raw records already in device memory (`recs`)."""
+    cap = _capacity(out) if cap is None else int(cap)
+    _check(lib().hs_b200_order_records_async(db.ptr, scratch.ptr, _dev_ptr(recs), int(n), _dev_ptr(out), cap,
+                                             _dev_ptr(count), C.c_void_p(stream or 0)), "order_records_async")
 
 
 def scan_corpus(db, corpus, scratch, fetch=True):

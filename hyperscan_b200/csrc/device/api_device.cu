@@ -34,6 +34,7 @@
 #include "../host/db_walk.h"
 #include "../host/pair_table.h"
 #include "kernels.h"
+#include "order_kernels.h"
 
 using namespace hsb;
 
@@ -114,6 +115,13 @@ struct DevImage {
     u64 groups = 0;
     u32 minWidth = 0;
     ReportRules rules;                   /* how its records are delivered (borrows dbCopy) */
+    /* the same rules as device tables, for hs_b200_order_*_async (order_kernels.h): OrderParams'
+     * table fields; orderStatus != HS_SUCCESS when an engine program cannot be laid out */
+    hs_error_t orderStatus = HS_SUCCESS;
+    u8 *d_rules = nullptr;
+    OrderParams orderTables;
+    u32 maxFanout = 1;
+    s32 maxAdjust = 0;
     size_t deviceBytes = 0;
 };
 
@@ -445,7 +453,57 @@ void freeImage(DevImage *im) {
     cudaFree(im->d_table);
     cudaFree(im->d_bitmap);
     cudaFree(im->d_bitmap2);
+    cudaFree(im->d_rules);
     delete im;
+}
+
+/* The report rules of an image as device tables (DeviceRules, one allocation): program reports, program
+ * offsets and starts, report ids and their exhaustible marks.  An engine program the tables cannot hold
+ * leaves orderStatus set; only the device ordering refuses the database then. */
+hs_error_t uploadOrderTables(DevImage *im) {
+    DeviceRules dr;
+    im->orderStatus = buildDeviceRules(&im->rules, im->nfaLength ? im->rules.bc + im->nfaOffset : nullptr,
+                                       im->nfaLength, &dr);
+    if (im->orderStatus != HS_SUCCESS) {
+        return HS_SUCCESS;
+    }
+    std::vector<OrderRep> reps(dr.reps.size());
+    for (size_t i = 0; i < reps.size(); i++) {
+        const ProgReport &r = dr.reps[i];
+        reps[i] = {r.onmatch, r.offset_adjust, r.min_bound, r.max_bound, r.logical ? 1u : 0u, 0};
+    }
+    const size_t repBytes = reps.size() * sizeof(OrderRep), offBytes = dr.progOff.size() * 4,
+                 startBytes = dr.progStart.size() * 4, idBytes = dr.ids.size() * 4, exBytes = dr.ids.size();
+    const size_t total = repBytes + offBytes + startBytes + idBytes + exBytes;
+    std::vector<u8> img(total + 1);
+    size_t at = 0;
+    auto put = [&](const void *src, size_t n) {
+        if (n) {
+            memcpy(img.data() + at, src, n);
+        }
+        at += n;
+        return at - n;
+    };
+    const size_t oRep = put(reps.data(), repBytes), oOff = put(dr.progOff.data(), offBytes),
+                 oStart = put(dr.progStart.data(), startBytes), oIds = put(dr.ids.data(), idBytes),
+                 oEx = put(dr.idExhaustible.data(), exBytes);
+    CUDA_TRY(cudaMalloc(&im->d_rules, img.size()));
+    CUDA_TRY(cudaMemcpy(im->d_rules, img.data(), img.size(), cudaMemcpyHostToDevice));
+    im->deviceBytes += img.size();
+    OrderParams &t = im->orderTables;
+    memset(&t, 0, sizeof(t));
+    t.shape = (u32)im->rules.shape;
+    t.reps = (const OrderRep *)(im->d_rules + oRep);
+    t.progOff = (const u32 *)(im->d_rules + oOff);
+    t.progStart = (const u32 *)(im->d_rules + oStart);
+    t.nProg = (u32)dr.progOff.size();
+    t.ids = (const u32 *)(im->d_rules + oIds);
+    t.idEx = im->d_rules + oEx;
+    t.nIds = (u32)dr.ids.size();
+    t.anyEx = std::find(dr.idExhaustible.begin(), dr.idExhaustible.end(), 1) != dr.idExhaustible.end();
+    im->maxFanout = std::max<u32>(1, dr.maxFanout);
+    im->maxAdjust = dr.maxAdjust;
+    return HS_SUCCESS;
 }
 
 /* Derive the device image: a copy of the bytecode plus the first-stage table
@@ -658,6 +716,10 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
         return e == cudaErrorMemoryAllocation ? HS_NOMEM : HS_UNKNOWN_ERROR;
     }
     im->deviceBytes = HSB_ROUNDUP(h->length, 16) + HSB_ROUNDUP(table.size(), 16) + bitmap.size() + bitmap2.size();
+    const hs_error_t ordered = uploadOrderTables(im.get());
+    if (ordered != HS_SUCCESS) {
+        return ordered;
+    }
     *out = im.release();
     return HS_SUCCESS;
 }
@@ -684,6 +746,7 @@ struct hs_b200_corpus {
     const u8 *streamHist = nullptr;
     const u64 *streamOffset = nullptr;
     std::vector<u32> h_len;  /* block lengths, for the end-of-block evaluation of logical combinations */
+    u32 maxLen = 0;          /* the longest block (resident corpora): bounds a match's end offset */
 };
 
 /* ---- scratch ------------------------------------------------------------------ */
@@ -713,6 +776,12 @@ struct hs_scratch {
     DevMatch *peers[MAX_PEERS];
     bool pending;
     u32 lastCount;
+    /* of the last hs_b200_scan_corpus_async: bounds of its records' block and end offset, for the sort key
+     * of hs_b200_order_matches_async */
+    u64 lastBlocks, lastMaxLen;
+    /* temporaries of hs_b200_order_*_async (order_kernels.h), grown on demand */
+    u8 *d_order;
+    size_t orderBytes;
     float lastMs;
     int smCount, maxSmem;
 };
@@ -1456,6 +1525,7 @@ hs_error_t hs_free_scratch(hs_scratch_t *s) {
     delete s->tmpOff;
     freeCorpus(s->inlineCorpus);
     cudaFree(s->d_out);
+    cudaFree(s->d_order);
     cudaFree(s->d_counters);
     if (s->h_counters) cudaFreeHost(s->h_counters);
     if (s->h_stage) cudaFreeHost(s->h_stage);
@@ -1561,6 +1631,7 @@ hs_error_t hs_b200_corpus_upload(const char *data, const unsigned long long *off
     c->readableEnd = HSB_ROUNDUP(total, 16) + 16;
     if (e == cudaSuccess) {
         r = setBlocks(c, packed.data(), lengths, nblocks, total, payload, 0, uniPitch, uniLen);
+        c->maxLen = nblocks ? *std::max_element(lengths, lengths + nblocks) : 0;
         if (r == HS_SUCCESS && cudaDeviceSynchronize() != cudaSuccess) {
             r = HS_UNKNOWN_ERROR;
         }
@@ -1614,6 +1685,7 @@ hs_error_t hs_b200_corpus_wrap(const void *d_data, size_t data_bytes,
     c->readableEnd = HSB_ROUNDUP((u64)data_bytes, 16);
     std::vector<u64> off(offsets, offsets + nblocks);
     r = setBlocks(c, off.data(), lengths, nblocks, prevEnd, payload, 0);
+    c->maxLen = nblocks ? *std::max_element(lengths, lengths + nblocks) : 0;
     if (r == HS_SUCCESS && cudaDeviceSynchronize() != cudaSuccess) {
         r = HS_UNKNOWN_ERROR;
     }
@@ -1666,10 +1738,16 @@ hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corp
             scratch->h_counters[CTR_ERROR] = 0;
             scratch->pending = false;
             scratch->lastCount = 0;
+            /* the device count too: the stream-ordered readers of the ring see no records */
+            if (cudaMemsetAsync(scratch->d_counters, 0, CTR_COUNT * sizeof(u32), st) != cudaSuccess) {
+                r = HS_UNKNOWN_ERROR;
+            }
         } else {
             r = enqueueScan(scratch, im, corpus, st);
         }
         scratch->lastCorpus = corpus;
+        scratch->lastBlocks = corpus->nblocks;
+        scratch->lastMaxLen = corpus->maxLen;
     }
     unmarkInUse(scratch);
     return r;
@@ -1849,6 +1927,158 @@ hs_error_t hs_b200_fetch_matches(const hs_database_t *db, hs_scratch_t *scratch,
         memcpy(out, tmp.data(), m * sizeof(DevMatch));
     }
     return HS_SUCCESS;
+}
+
+/* ---- the report rules on the device ---------------------------------------------------------
+ *
+ * ReportRules::deliver as kernels (order_kernels.h), enqueued behind the scan on its stream: the
+ * delivered matches stay in device memory and the host never waits. */
+
+static u32 bitWidth(u64 v) {
+    u32 b = 0;
+    for (; v; v >>= 1) {
+        b++;
+    }
+    return b;
+}
+
+/* the image of `db` the scratch already holds (an order entry builds none: the scan built it) */
+static DevImage *heldImage(hs_scratch *s, const hs_database_t *db) {
+    const DbHeader *h = (const DbHeader *)db;
+    for (DevImage *im : *s->images) {
+        if (im->db == db && im->crc == h->crc32 && im->length == h->length) {
+            return im;
+        }
+    }
+    return nullptr;
+}
+
+static hs_error_t checkOrderArgs(const hs_database_t *db, hs_scratch_t *scratch, void *d_out, size_t cap,
+                                 void *d_count, DevImage **im) {
+    if (!db || !scratch || !d_count || (cap && !d_out)) {
+        return HS_INVALID;
+    }
+    hs_error_t r = checkScanArgs(db, scratch);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    if (dbRose(db)->ckeyCount) {
+        return HS_INVALID; /* combination reports are evaluated per block on the host */
+    }
+    *im = heldImage(scratch, db);
+    if (!*im) {
+        return HS_INVALID;
+    }
+    return (*im)->orderStatus;
+}
+
+/* Enqueue the ordering of the records at `in` -- the record ring (ringCount = its count on the device,
+ * inCap = its capacity) or n records -- into d_out[0, cap) and *d_count on `st`, with the temporaries
+ * in the scratch: tile sums and digit histograms, two record buffers for the resolved records (each
+ * input record becomes at most maxFanout), and for exhaustible ids a hash table of twice as many slots. */
+static hs_error_t enqueueOrder(hs_scratch *s, const DevImage *im, const DevMatch *in, const u32 *ringCount, u32 inCap,
+                               u32 inN, void *d_out, size_t cap, void *d_count, u32 maxPasses, cudaStream_t st) {
+    const u64 n = ringCount ? inCap : inN;
+    const u64 m = n * im->maxFanout;
+    if (m >= 0xfffff000ull) {
+        return HS_NOMEM; /* positions are 32-bit */
+    }
+    OrderParams p = im->orderTables;
+    const u64 tiles = (std::max(n, m) + ORDER_TILE - 1) / ORDER_TILE;
+    u64 slots = 0;
+    if (p.anyEx && m) {
+        for (slots = 2; slots < 2 * m; slots <<= 1) {
+        }
+        if (slots > 0x80000000ull) {
+            return HS_NOMEM;
+        }
+    }
+    size_t at = 0;
+    auto carve = [&](size_t bytes) {
+        const size_t o = at;
+        at = HSB_ROUNDUP(at + bytes, 256);
+        return o;
+    };
+    const size_t oSt = carve(sizeof(OrderState)), oTile = carve((tiles + 1) * 4), oHist = carve(256 * (tiles + 1) * 4),
+                 oBin = carve(ORDER_MAX_PASSES * 256 * 4), oBuf0 = carve(m * sizeof(DevMatch)),
+                 oBuf1 = carve(m * sizeof(DevMatch)), oKey = carve(slots * 8), oFirst = carve(slots * 4);
+    if (at > s->orderBytes) {
+        cudaFree(s->d_order); /* (synchronises with any ordering still using it) */
+        s->d_order = nullptr;
+        s->orderBytes = 0;
+        CUDA_TRY(cudaMalloc(&s->d_order, at));
+        s->orderBytes = at;
+    }
+    u8 *b = s->d_order;
+    p.in = in;
+    p.inCount = ringCount;
+    p.inCap = inCap;
+    p.inN = inN;
+    p.st = (OrderState *)(b + oSt);
+    p.buf[0] = (DevMatch *)(b + oBuf0);
+    p.buf[1] = (DevMatch *)(b + oBuf1);
+    p.bufCap = (u32)m;
+    p.tileSum = (u32 *)(b + oTile);
+    p.hist = (u32 *)(b + oHist);
+    p.tileCap = (u32)tiles + 1;
+    p.binTotal = (u32 *)(b + oBin);
+    p.exKey = (u64 *)(b + oKey);
+    p.exFirst = (u32 *)(b + oFirst);
+    p.exSlots = (u32)slots;
+    p.anyEx = slots != 0;
+    p.out = (DevMatch *)d_out;
+    p.outCap = cap;
+    p.count = (unsigned long long *)d_count;
+    if (slots) {
+        CUDA_TRY(cudaMemsetAsync(b + oKey, 0xff, oFirst + slots * 4 - oKey, st));
+    }
+    unsigned launched = 0;
+    const cudaError_t e = launchOrder(p, maxPasses, st, &launched);
+    g_launches += launched;
+    return e == cudaSuccess ? HS_SUCCESS : HS_UNKNOWN_ERROR;
+}
+
+hs_error_t hs_b200_order_matches_async(const hs_database_t *db, hs_scratch_t *scratch, void *d_out, size_t cap,
+                                       void *d_count, void *cuda_stream) {
+    DevImage *im = nullptr;
+    hs_error_t r = checkOrderArgs(db, scratch, d_out, cap, d_count, &im);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    if (markInUse(scratch)) {
+        return HS_SCRATCH_IN_USE;
+    }
+    DeviceGuard guard(scratch->device);
+    /* the key needs no more bits than the last scan's block count, its longest block and the id table */
+    const u32 keyBits = bitWidth(im->orderTables.nIds ? im->orderTables.nIds - 1 : 0) +
+                        bitWidth(scratch->lastMaxLen + (u64)std::max(0, im->maxAdjust)) +
+                        bitWidth(scratch->lastBlocks ? scratch->lastBlocks - 1 : 0);
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
+    r = enqueueOrder(scratch, im, scratch->d_out, scratch->d_counters + CTR_MATCHES, scratch->outCap, 0, d_out, cap,
+                     d_count, (keyBits + 7) / 8, st);
+    unmarkInUse(scratch);
+    return r;
+}
+
+hs_error_t hs_b200_order_records_async(const hs_database_t *db, hs_scratch_t *scratch, const void *d_recs, size_t n,
+                                       void *d_out, size_t cap, void *d_count, void *cuda_stream) {
+    DevImage *im = nullptr;
+    hs_error_t r = checkOrderArgs(db, scratch, d_out, cap, d_count, &im);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    if ((n && !d_recs) || n > 0xfffffff0u) {
+        return HS_INVALID;
+    }
+    if (markInUse(scratch)) {
+        return HS_SCRATCH_IN_USE;
+    }
+    DeviceGuard guard(scratch->device);
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
+    r = enqueueOrder(scratch, im, (const DevMatch *)d_recs, nullptr, 0, (u32)n, d_out, cap, d_count,
+                     ORDER_MAX_PASSES, st);
+    unmarkInUse(scratch);
+    return r;
 }
 
 /* ---- DFA engines in block mode ------------------------------------------------------

@@ -184,6 +184,69 @@ struct DfaParams {
 };
 cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t stream);
 
+/* ---- the report rules on the device (order_kernels.h): raw records -> delivered matches ---- */
+
+/* a report instruction an engine's program reaches (db_walk.h ProgReport) */
+struct OrderRep {
+    u32 onmatch;
+    s32 adjust;
+    u64 lo, hi;    /* CHECK_BOUNDS on the record's end offset */
+    u32 logical;   /* SET_LOGICAL: the record becomes a logical-key record */
+    u32 pad;
+};
+
+enum { ORDER_THREADS = 256, ORDER_ITEMS = 8, ORDER_TILE = ORDER_THREADS * ORDER_ITEMS,
+       ORDER_MAX_PASSES = 16 /* 8-bit digits of a key of 32 (block) + 64 (to) + 32 (id) bits */ };
+
+/* device-side progress of one ordering */
+struct OrderState {
+    u64 maxTo;
+    u32 n;           /* input records (0 after a ring overflow) */
+    u32 m;           /* records after resolution */
+    u32 kept;        /* records after dedupe and exhaustion */
+    u32 maxBlock, maxId;
+    u32 unknownIds;  /* some record carries an id outside the id table: the key holds ids, not ranks */
+    u32 overflow;
+    u32 passes;      /* radix passes the key needs */
+    u32 idBits, toBits, blockBits;
+};
+
+struct OrderParams {
+    /* the database's tables (DeviceRules) */
+    u32 shape;                /* DbShape */
+    const u32 *progOff, *progStart;
+    const OrderRep *reps;
+    u32 nProg;
+    const u32 *ids;
+    const u8 *idEx;
+    u32 nIds;
+    u32 anyEx;
+    /* input: n records at `in`; with inCount, n = *inCount (the scan's record count), and a count above
+     * inCap is a ring overflow */
+    const DevMatch *in;
+    const u32 *inCount;
+    u32 inCap;
+    u32 inN;
+    /* temporaries, sized by the caller: resolved records up to bufCap; tiles of max(inCap, bufCap) */
+    OrderState *st;
+    DevMatch *buf[2];
+    u32 bufCap;
+    u32 *tileSum;
+    u32 *hist;       /* [256][tileCap] per pass */
+    u32 tileCap;
+    u32 *binTotal;   /* [ORDER_MAX_PASSES][256] */
+    u64 *exKey;      /* anyEx: hash table of (block, id rank) -> first record, exSlots (a power of two) */
+    u32 *exFirst;
+    u32 exSlots;
+    /* output */
+    DevMatch *out;
+    u64 outCap;
+    unsigned long long *count;
+};
+/* Enqueue the whole ordering on `stream`, with at most maxPasses radix passes (the key needs no more for
+ * the input at hand); *launches receives the number of kernels launched. */
+cudaError_t launchOrder(const OrderParams &p, u32 maxPasses, cudaStream_t stream, unsigned *launches);
+
 /* accel primitives (src/nfa/shufti.c, truffle.c, vermicelli.h): first
  * position in [0,len) whose byte is in the class, or len. */
 cudaError_t launchAccelFind(int type, const u8 *params, const u8 *d_buf, u64 len,

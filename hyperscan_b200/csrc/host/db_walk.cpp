@@ -29,7 +29,13 @@ bool collectProgramReports(ReportRules *rr, u32 prog, std::vector<ProgReport> *r
     /* CHECK_BOUNDS guards the instructions up to its fail_jump target */
     struct Guard { u32 until; u64 lo, hi; };
     std::vector<Guard> guards;
-    auto report = [&](u32 onmatch, s32 adjust) {
+    auto report = [&](u32 onmatch, s32 adjust, bool logical = false) {
+        if (!logical) {
+            rr->reportIds.insert(onmatch);
+        }
+        if (!reports) {
+            return;
+        }
         u64 lo = 0, hi = ~0ull;
         for (const Guard &g : guards) {
             if (pc < g.until) {
@@ -37,7 +43,7 @@ bool collectProgramReports(ReportRules *rr, u32 prog, std::vector<ProgReport> *r
                 hi = std::min(hi, g.hi);
             }
         }
-        reports->push_back({onmatch, adjust, lo, hi, false});
+        reports->push_back({onmatch, adjust, lo, hi, logical});
     };
     auto jump = [&](u32 from, u32 rel) { furthest = std::max(furthest, from + rel); };
 #define STEP(T) pc += (u32)HSB_ROUNDUP(sizeof(T), INSTR_ALIGN)
@@ -61,11 +67,9 @@ bool collectProgramReports(ReportRules *rr, u32 prog, std::vector<ProgReport> *r
             STEP(InstrEnd);
             break;
         case OP_FINAL_REPORT: {
-            if (reports) {
-                InstrFinalReport in;
-                memcpy(&in, bc + pc, sizeof(in));
-                report(in.onmatch, in.offset_adjust);
-            }
+            InstrFinalReport in;
+            memcpy(&in, bc + pc, sizeof(in));
+            report(in.onmatch, in.offset_adjust);
             if (furthest <= pc) {
                 return true;
             }
@@ -94,9 +98,7 @@ bool collectProgramReports(ReportRules *rr, u32 prog, std::vector<ProgReport> *r
             InstrReport in;
             memcpy(&in, bc + pc, sizeof(in));
             lastReport = in.onmatch;
-            if (reports) {
-                report(in.onmatch, in.offset_adjust);
-            }
+            report(in.onmatch, in.offset_adjust);
             STEP(InstrReport);
             break;
         }
@@ -105,9 +107,7 @@ bool collectProgramReports(ReportRules *rr, u32 prog, std::vector<ProgReport> *r
             memcpy(&in, bc + pc, sizeof(in));
             rr->exhaustible.insert(in.onmatch);
             lastReport = in.onmatch;
-            if (reports) {
-                report(in.onmatch, in.offset_adjust);
-            }
+            report(in.onmatch, in.offset_adjust);
             STEP(InstrReportExhaust);
             break;
         }
@@ -115,9 +115,7 @@ bool collectProgramReports(ReportRules *rr, u32 prog, std::vector<ProgReport> *r
             InstrDedupeAndReport in;
             memcpy(&in, bc + pc, sizeof(in));
             lastReport = in.onmatch;
-            if (reports) {
-                report(in.onmatch, in.offset_adjust);
-            }
+            report(in.onmatch, in.offset_adjust);
             STEP_JUMP(InstrDedupeAndReport);
             break;
         }
@@ -132,10 +130,7 @@ bool collectProgramReports(ReportRules *rr, u32 prog, std::vector<ProgReport> *r
             if (lastReport != INVALID_EKEY) {
                 rr->comb.lkeyReport[in.lkey] = lastReport;
             }
-            if (reports) {
-                report(in.lkey, in.offset_adjust);
-                reports->back().logical = true;
-            }
+            report(in.lkey, in.offset_adjust, true);
             STEP(InstrSetLogical);
             break;
         }
@@ -463,6 +458,174 @@ hs_error_t loadReportRules(const hs_database_t *db, ReportRules *rules, std::vec
         return HS_INVALID;
     }
     return ok ? HS_SUCCESS : HS_ARCH_ERROR;
+}
+
+namespace {
+
+/* The report program offsets an engine can raise (its reports were remapped to programs at build time):
+ * McClellan / Sheng -- the single report, or the accept and EOD-accept report lists of every state's aux
+ * record (struct report_list {count; reports[]}); LimEx -- the accept and EOD-accept tables (NFAAccept) and
+ * the exceptions' report lists (MO_INVALID_IDX-terminated).  Offsets are relative to struct NFA (DFAs) or
+ * to the LimEx structure that follows it.  False on a table that runs past the engine. */
+struct EngineWalk {
+    const u8 *nfa;
+    u32 len;
+    std::vector<u32> *out;
+    bool ok = true;
+    u32 at(u64 off) {
+        u32 v = 0;
+        if (off + 4 > len) {
+            ok = false;
+        } else {
+            memcpy(&v, nfa + off, 4);
+        }
+        return v;
+    }
+    void countedList(u32 off) { /* struct report_list */
+        const u32 n = at(off);
+        for (u32 i = 0; i < n && ok; i++) {
+            out->push_back(at((u64)off + 4 + 4 * (u64)i));
+        }
+    }
+    void terminatedList(u64 off) {
+        for (u32 i = 0; ok; i++) {
+            const u32 id = at(off + 4 * (u64)i);
+            if (id == MO_INVALID_IDX) {
+                break;
+            }
+            out->push_back(id);
+        }
+    }
+    void dfaAux(u32 auxOff, u32 auxSize, u32 states) {
+        for (u32 s = 0; s < states && ok; s++) {
+            const u64 a = (u64)auxOff + (u64)s * auxSize;
+            for (u32 list : {at(a), at(a + 4)}) { /* accept, accept_eod */
+                if (list) {
+                    countedList(list);
+                }
+            }
+        }
+    }
+    template <class Nfa, class Exc> void limex() {
+        const u64 base = sizeof(NFA);
+        if (base + sizeof(Nfa) > len) {
+            ok = false;
+            return;
+        }
+        Nfa lx;
+        memcpy(&lx, nfa + base, sizeof(lx));
+        for (auto t : {std::make_pair(lx.acceptOffset, lx.acceptCount), std::make_pair(lx.acceptEodOffset, lx.acceptEodCount)}) {
+            for (u32 i = 0; i < t.second && ok; i++) {
+                const u64 a = base + t.first + (u64)i * sizeof(NFAAccept);
+                if (a + sizeof(NFAAccept) > len) {
+                    ok = false;
+                    break;
+                }
+                NFAAccept acc;
+                memcpy(&acc, nfa + a, sizeof(acc));
+                if (acc.single_report) {
+                    out->push_back(acc.reports);
+                } else {
+                    terminatedList(base + acc.reports);
+                }
+            }
+        }
+        for (u32 i = 0; i < lx.exceptionCount && ok; i++) {
+            const u64 x = base + lx.exceptionOffset + (u64)i * sizeof(Exc);
+            if (x + sizeof(Exc) > len) {
+                ok = false;
+                break;
+            }
+            Exc e;
+            memcpy(&e, nfa + x, sizeof(e));
+            if (e.reports != MO_INVALID_IDX) {
+                terminatedList(base + e.reports);
+            }
+        }
+    }
+};
+
+bool enginePrograms(const u8 *nfa, u32 len, std::vector<u32> *out) {
+    EngineWalk w{nfa, len, out};
+    if (len < sizeof(NFA)) {
+        return false;
+    }
+    NFA h;
+    memcpy(&h, nfa, sizeof(h));
+    switch (h.type) {
+    case NFA_MCCLELLAN_8:
+    case NFA_MCCLELLAN_16: {
+        if (sizeof(NFA) + sizeof(McClellan) > len) {
+            return false;
+        }
+        McClellan m;
+        memcpy(&m, nfa + sizeof(NFA), sizeof(m));
+        if (m.flags & MCCLELLAN_FLAG_SINGLE) {
+            out->push_back(m.arb_report);
+        } else {
+            w.dfaAux(m.aux_offset, sizeof(MStateAux), m.state_count);
+        }
+        break;
+    }
+    case NFA_SHENG: {
+        if (sizeof(NFA) + sizeof(Sheng) > len) {
+            return false;
+        }
+        Sheng s;
+        memcpy(&s, nfa + sizeof(NFA), sizeof(s));
+        if (s.flags & SHENG_FLAG_SINGLE_REPORT) {
+            out->push_back(s.report);
+        } else {
+            w.dfaAux(s.aux_offset, sizeof(SstateAux), s.n_states);
+        }
+        break;
+    }
+    case NFA_LIMEX_32: w.limex<LimExNFA32, NFAException32>(); break;
+    case NFA_LIMEX_64: w.limex<LimExNFA64, NFAException64>(); break;
+    case NFA_LIMEX_128: w.limex<LimExNFA128, NFAException128>(); break;
+    case NFA_LIMEX_256: w.limex<LimExNFA256, NFAException256>(); break;
+    case NFA_LIMEX_512: w.limex<LimExNFA512, NFAException512>(); break;
+    default: return false;
+    }
+    return w.ok;
+}
+
+} // namespace
+
+hs_error_t buildDeviceRules(ReportRules *rules, const u8 *nfa, u32 nfaLen, DeviceRules *out) {
+    *out = DeviceRules();
+    if (nfa) {
+        std::vector<u32> progs;
+        if (!enginePrograms(nfa, nfaLen, &progs)) {
+            return HS_INVALID;
+        }
+        std::sort(progs.begin(), progs.end());
+        progs.erase(std::unique(progs.begin(), progs.end()), progs.end());
+        out->progStart.push_back(0);
+        for (u32 prog : progs) {
+            auto it = rules->progReports.find(prog);
+            if (it == rules->progReports.end()) {
+                std::vector<ProgReport> reps;
+                if (prog % INSTR_ALIGN || prog < sizeof(RoseEngine) || prog >= rules->bcLen ||
+                    !collectProgramReports(rules, prog, &reps)) {
+                    return HS_UNKNOWN_ERROR; /* as ReportRules::deliver would answer a record of it */
+                }
+                it = rules->progReports.emplace(prog, std::move(reps)).first;
+            }
+            out->progOff.push_back(prog);
+            out->reps.insert(out->reps.end(), it->second.begin(), it->second.end());
+            out->progStart.push_back((u32)out->reps.size());
+            out->maxFanout = std::max<u32>(out->maxFanout, (u32)it->second.size());
+            for (const ProgReport &rp : it->second) {
+                out->maxAdjust = std::max<s32>(out->maxAdjust, rp.offset_adjust);
+            }
+        }
+    }
+    out->ids.assign(rules->reportIds.begin(), rules->reportIds.end());
+    for (u32 id : out->ids) {
+        out->idExhaustible.push_back(rules->exhaustible.count(id) ? 1 : 0);
+    }
+    return HS_SUCCESS;
 }
 
 hs_error_t ReportRules::deliver(std::vector<DevMatch> *v, const u32 *lengths, size_t nblocks) {

@@ -9,6 +9,7 @@
 #ifndef HSB200_DB_WALK_H
 #define HSB200_DB_WALK_H
 
+#include <set>
 #include <unordered_map>
 #include <unordered_set>
 #include <utility>
@@ -90,6 +91,8 @@ struct ReportRules {
     u32 bcLen = 0;
     /* an engine's report program offset -> the report instructions it reaches, filled as programs are met */
     std::unordered_map<u32, std::vector<ProgReport>> progReports;
+    /* the report ids the programs walked so far can raise (logical keys excluded) */
+    std::set<u32> reportIds;
 
     /* Without dedupe keys, exhaustion keys, combinations or engine records, the raw record count is the
      * delivered count. */
@@ -114,6 +117,25 @@ struct ReportRules {
  * refuse the database instead of failing mid-scan).  tails, if given, receives the LitInfo v/msk/size and
  * bucket of every literal of an FDR or Teddy matcher. */
 hs_error_t loadReportRules(const hs_database_t *db, ReportRules *rules, std::vector<LitTail> *tails = nullptr);
+
+/* The report rules as tables, for the device's form of ReportRules::deliver (order_kernels.h). */
+struct DeviceRules {
+    /* every report program the engine can raise, ascending; program k's report instructions are
+     * reps[progStart[k], progStart[k + 1]) */
+    std::vector<u32> progOff, progStart;
+    std::vector<ProgReport> reps;
+    u32 maxFanout = 1;  /* the most records one input record becomes (at least 1: a literal's record) */
+    s32 maxAdjust = 0;  /* the largest offset_adjust (at least 0) */
+    /* every report id a record can carry, ascending (the dense rank of an id is its index), and whether
+     * it is exhaustible (HS_FLAG_SINGLEMATCH) */
+    std::vector<u32> ids;
+    std::vector<u8> idExhaustible;
+};
+/* Walk every report program of the engine (its bytes nfa[0, nfaLen), struct NFA first; none if nfa is
+ * null) as ReportRules::deliver would on meeting it, which completes rules->progReports and
+ * rules->exhaustible, and lay the rules out as tables.  HS_INVALID: the engine's report lists run past
+ * its end; HS_UNKNOWN_ERROR: a program holds an opcode the device does not implement. */
+hs_error_t buildDeviceRules(ReportRules *rules, const u8 *nfa, u32 nfaLen, DeviceRules *out);
 
 } // namespace hsb
 #endif

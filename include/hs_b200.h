@@ -407,6 +407,33 @@ hs_error_t hs_b200_fetch_matches(const hs_database_t *db, hs_scratch_t *scratch,
                                  hs_b200_match_t *out, size_t cap,
                                  unsigned long long *nmatches);
 
+/* The report rules on the device: the same delivered matches as hs_b200_fetch_matches /
+ * hs_b200_postprocess_matches -- same records, same (block, to, id) order, same count -- computed by
+ * kernels and written to device memory, enqueued on a CUDA stream with no host synchronisation.
+ * Every database shape the device scans is taken (pure literal, single outfix, literals beside an
+ * outfix); a database with logical combinations is refused (HS_INVALID), as are NULL arguments
+ * (d_out may be NULL only with cap = 0) and a scratch that holds no image of `db` (one that was not
+ * allocated for it).  Temporaries live in the scratch, which must not be used by another call
+ * until the ordering has been enqueued. */
+#define HS_B200_ORDER_RING_OVERFLOW (~0ULL)
+/* Enqueue, on cuda_stream (the one the scan was enqueued on; NULL = the scratch's stream), the
+ * delivery of the last scan enqueued with hs_b200_scan_corpus_async: the matches
+ * hs_b200_fetch_matches would return, written to d_out[0, cap) (hs_b200_match_t[]) and their count
+ * to *d_count (an unsigned long long in device memory; it may exceed cap, and then only the first
+ * cap are written).  If the scan's record ring overflowed, *d_count = HS_B200_ORDER_RING_OVERFLOW:
+ * hs_b200_scan_corpus_finish then returns HS_INSUFFICIENT_SPACE and grows the ring as it does
+ * for every overflow, and the caller scans again. */
+hs_error_t hs_b200_order_matches_async(const hs_database_t *db, hs_scratch_t *scratch,
+                                       void *d_out, size_t cap, void *d_count, void *cuda_stream);
+/* The same for n raw records already in device memory (e.g. the all-gathered records of several
+ * ranks, block indices already global): what the host report rules make of them
+ * (hs_b200_postprocess_matches for a pure-literal database; for a database with an engine, whose
+ * records carry report programs, the delivery hs_b200_fetch_matches applies).  Records whose id
+ * names no report program of the engine are dropped. */
+hs_error_t hs_b200_order_records_async(const hs_database_t *db, hs_scratch_t *scratch,
+                                       const void *d_recs, size_t n, void *d_out, size_t cap,
+                                       void *d_count, void *cuda_stream);
+
 /* Stream sets: `nstreams` streams of one HS_MODE_STREAM literal database whose
  * state (7 look-behind bytes + count, 64-bit offset: 16 bytes per stream) stays
  * in HBM between calls.  hs_b200_streams_scan() gives every stream one write
