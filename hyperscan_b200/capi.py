@@ -58,7 +58,7 @@ class PlatformInfo(C.Structure):
 class DbInfo(C.Structure):
     _fields_ = [("runtime_impl", C.c_uint), ("hwlm_type", C.c_uint), ("engine_id", C.c_uint),
                 ("fdr_domain", C.c_uint), ("fdr_stride", C.c_uint), ("num_literals", C.c_uint),
-                ("bytecode_len", C.c_uint), ("min_width", C.c_uint)]
+                ("bytecode_len", C.c_uint), ("min_width", C.c_uint), ("engine_count", C.c_uint)]
 
 
 MATCH_CB = C.CFUNCTYPE(C.c_int, C.c_uint, C.c_ulonglong, C.c_ulonglong, C.c_uint, C.c_void_p)

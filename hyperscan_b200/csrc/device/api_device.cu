@@ -103,9 +103,13 @@ struct DevImage {
     u32 bitmapBytes = 0, bitmapShift = 0, keyBytes = 0;
     u32 pairBytes = 0, bitmapBits = 0; /* FK_PAIR32 layout (kernels.h) */
     u32 bucketFold = 0;
-    u32 nfaOffset = 0, nfaLength = 0;   /* the outfix engine (bytecode offset, NFA.length), alone (FK_OUTFIX) or
-                                         * beside the literal matcher; nfaLength == 0: none */
-    DfaParams nfaParams;                /* ... and what launchDfa needs to know about it */
+    /* the outfix engines (bytecode offset, NFA.length) in queue order: one alone (FK_OUTFIX) or beside the
+     * literal matcher, or several alone (FK_OUTFIX); empty: none */
+    std::vector<std::pair<u32, u32>> engines;
+    /* what launchDfa needs to run them over a corpus: the one engine's parameters, or for several engines
+     * one fused launch per engine kind over the descriptors at d_engines */
+    std::vector<DfaParams> engineRuns;
+    DfaEngine *d_engines = nullptr;
     u8 *d_bitmap2 = nullptr; /* second level (HBM / L2) for large literal sets */
     u32 bitmap2Shift = 0;
     int kind = FK_BYTE32;
@@ -454,6 +458,7 @@ void freeImage(DevImage *im) {
     cudaFree(im->d_bitmap);
     cudaFree(im->d_bitmap2);
     cudaFree(im->d_rules);
+    cudaFree(im->d_engines);
     delete im;
 }
 
@@ -462,8 +467,11 @@ void freeImage(DevImage *im) {
  * leaves orderStatus set; only the device ordering refuses the database then. */
 hs_error_t uploadOrderTables(DevImage *im) {
     DeviceRules dr;
-    im->orderStatus = buildDeviceRules(&im->rules, im->nfaLength ? im->rules.bc + im->nfaOffset : nullptr,
-                                       im->nfaLength, &dr);
+    std::vector<EngineBytes> engines;
+    for (const auto &e : im->engines) {
+        engines.push_back({im->rules.bc + e.first, e.second});
+    }
+    im->orderStatus = buildDeviceRules(&im->rules, engines, &dr);
     if (im->orderStatus != HS_SUCCESS) {
         return HS_SUCCESS;
     }
@@ -506,6 +514,47 @@ hs_error_t uploadOrderTables(DevImage *im) {
     return HS_SUCCESS;
 }
 
+/* Several engines: one launch per engine kind present instead of one per engine (DfaParams.engines), so
+ * that a corpus too small to fill the GPU for one engine runs all of them side by side.  Replaces
+ * im->engineRuns (one per engine, nfa set) with one run per kind, in the order the kinds first appear in
+ * the queues, over descriptors uploaded to im->d_engines. */
+hs_error_t fuseEngineRuns(DevImage *im) {
+    std::vector<DfaEngine> descs;
+    std::vector<DfaParams> runs;
+    std::vector<size_t> firstDesc;
+    std::vector<bool> done(im->engineRuns.size(), false);
+    for (size_t q = 0; q < im->engineRuns.size(); q++) {
+        if (done[q]) {
+            continue;
+        }
+        DfaParams run = im->engineRuns[q];
+        run.nfa = nullptr;
+        run.tableBytes = run.states = run.squashes = 0;
+        run.nengines = 0;
+        firstDesc.push_back(descs.size());
+        for (size_t j = q; j < im->engineRuns.size(); j++) {
+            const DfaParams &e = im->engineRuns[j];
+            if (e.kind != run.kind) {
+                continue;
+            }
+            done[j] = true;
+            descs.push_back({e.nfa, e.tableBytes, e.states, e.squashes, 0});
+            run.tableBytes = std::max(run.tableBytes, e.tableBytes);
+            run.states = std::max(run.states, e.states);
+            run.nengines++;
+        }
+        runs.push_back(run);
+    }
+    CUDA_TRY(cudaMalloc(&im->d_engines, descs.size() * sizeof(DfaEngine)));
+    CUDA_TRY(cudaMemcpy(im->d_engines, descs.data(), descs.size() * sizeof(DfaEngine), cudaMemcpyHostToDevice));
+    im->deviceBytes += descs.size() * sizeof(DfaEngine);
+    for (size_t i = 0; i < runs.size(); i++) {
+        runs[i].engines = im->d_engines + firstDesc[i];
+    }
+    im->engineRuns.swap(runs);
+    return HS_SUCCESS;
+}
+
 /* Derive the device image: a copy of the bytecode plus the first-stage table
  * in the form the shift-OR kernel consumes (DESIGN.md section 3). */
 hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
@@ -540,27 +589,32 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
          * engine runs on the DFA / NFA kernels (dfa_kernels.cu) straight from the bytecode copy;
          * the programs are resolved on the host when the records are delivered (ReportRules).  With
          * a literal matcher beside it (roseBlockExec's outfix), the engine's records are tagged so
-         * that the host can tell them from the literals' */
-        if ((size_t)r->nfaInfoOffset + sizeof(NfaInfo) > h->length) {
+         * that the host can tell them from the literals'.  Several outfixes without a literal matcher
+         * (roseBlockExec over several outfix queues) all run over every block, into one record ring */
+        const u32 k = r->queueCount;
+        if ((size_t)r->nfaInfoOffset + (size_t)k * sizeof(NfaInfo) > h->length) {
             return HS_INVALID;
         }
-        NfaInfo ni;
-        memcpy(&ni, bc + r->nfaInfoOffset, sizeof(ni));
-        if (ni.nfaOffset % 64 || (size_t)ni.nfaOffset + sizeof(NFA) > h->length) {
-            return HS_INVALID;
+        for (u32 q = 0; q < k; q++) {
+            NfaInfo ni;
+            memcpy(&ni, bc + r->nfaInfoOffset + q * sizeof(NfaInfo), sizeof(ni));
+            if (ni.nfaOffset % 64 || (size_t)ni.nfaOffset + sizeof(NFA) > h->length) {
+                return HS_INVALID;
+            }
+            NFA nh;
+            memcpy(&nh, bc + ni.nfaOffset, sizeof(nh));
+            if ((size_t)ni.nfaOffset + nh.length > h->length) {
+                return HS_INVALID;
+            }
+            DfaParams dp;
+            const hs_error_t er = engineParams(bc + ni.nfaOffset, nh.length, &dp);
+            if (er != HS_SUCCESS) {
+                return er;
+            }
+            dp.toTag = shape == SHAPE_LITERALS_OUTFIX ? ENGINE_RECORD : 0;
+            im->engines.push_back({ni.nfaOffset, nh.length});
+            im->engineRuns.push_back(dp);
         }
-        NFA nh;
-        memcpy(&nh, bc + ni.nfaOffset, sizeof(nh));
-        if ((size_t)ni.nfaOffset + nh.length > h->length) {
-            return HS_INVALID;
-        }
-        const hs_error_t er = engineParams(bc + ni.nfaOffset, nh.length, &im->nfaParams);
-        if (er != HS_SUCCESS) {
-            return er;
-        }
-        im->nfaOffset = ni.nfaOffset;
-        im->nfaLength = nh.length;
-        im->nfaParams.toTag = shape == SHAPE_LITERALS_OUTFIX ? ENGINE_RECORD : 0;
     }
     /* a literal program that uses a state-carrying opcode of roseRunProgram_l that the device
      * interpreter does not implement (delayed literals, SOM, chained reports) is refused here
@@ -635,7 +689,7 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
             buildPairBitmaps(keys, im->bitmapBits, &bitmap, &bitmap2, &im->bitmap2Shift);
         }
     };
-    if (shape == SHAPE_SOLE_OUTFIX) {
+    if (shape == SHAPE_SOLE_OUTFIX || shape == SHAPE_OUTFIXES) {
         im->kind = FK_OUTFIX;
         im->groups = 0;
     } else if (hw->type == HWLM_ENGINE_NOOD) {
@@ -716,6 +770,15 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
         return e == cudaErrorMemoryAllocation ? HS_NOMEM : HS_UNKNOWN_ERROR;
     }
     im->deviceBytes = HSB_ROUNDUP(h->length, 16) + HSB_ROUNDUP(table.size(), 16) + bitmap.size() + bitmap2.size();
+    for (size_t q = 0; q < im->engines.size(); q++) {
+        im->engineRuns[q].nfa = im->d_bc + im->engines[q].first;
+    }
+    if (shape == SHAPE_OUTFIXES) {
+        const hs_error_t fused = fuseEngineRuns(im.get());
+        if (fused != HS_SUCCESS) {
+            return fused;
+        }
+    }
     const hs_error_t ordered = uploadOrderTables(im.get());
     if (ordered != HS_SUCCESS) {
         return ordered;
@@ -1024,9 +1087,9 @@ void fillParams(const hs_scratch *s, const DevImage *im, const hs_b200_corpus *c
     }
 }
 
-/* Run an engine (dp from engineParams; its bytes at `nfa` in device memory) over every
- * block of corpus c, into the record ring out[0, outCap) and its counters. */
-cudaError_t launchEngine(DfaParams dp, const u8 *nfa, const hs_b200_corpus *c, DevMatch *out, u32 outCap,
+/* Run an engine (dp from engineParams, dp.nfa its bytes in device memory), or a fused launch of several
+ * (dp.engines), over every block of corpus c, into the record ring out[0, outCap) and its counters. */
+cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u32 outCap,
                          u32 *counters, int smCount, int maxSmem, cudaStream_t stream) {
     dp.corpus = c->d_data;
     dp.readableEnd = c->readableEnd;
@@ -1035,7 +1098,6 @@ cudaError_t launchEngine(DfaParams dp, const u8 *nfa, const hs_b200_corpus *c, D
     dp.nblocks = (u32)c->nblocks;
     dp.uniformPitch = c->uniformPitch;
     dp.uniformLen = c->uniformLen;
-    dp.nfa = nfa;
     dp.out = out;
     dp.outCap = outCap;
     dp.counters = counters;
@@ -1069,13 +1131,16 @@ hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
         CUDA_TRY(launchConfirm(cfg, p, stream));
         g_launches++;
     }
-    if (im->nfaLength) {
+    if (!im->engineRuns.empty()) {
         /* a block is one thread's walk from its first byte: after the last range of the corpus,
-         * the engine runs over every block, into the same record ring */
+         * the engines run over every block, into the same record ring (whose count only ever grows by
+         * whole groups of eight slots while no literal record is in it: the fused launches need no
+         * alignSharedRing between them) */
         const u32 ntiles = (u32)((c->bytes + pl.tileBytes - 1) / pl.tileBytes);
         if (t1 >= ntiles) {
-            CUDA_TRY(launchEngine(im->nfaParams, im->d_bc + im->nfaOffset, c, s->d_out, s->outCap, s->d_counters,
-                                  s->smCount, s->maxSmem, stream));
+            for (const DfaParams &dp : im->engineRuns) {
+                CUDA_TRY(launchEngine(dp, c, s->d_out, s->outCap, s->d_counters, s->smCount, s->maxSmem, stream));
+            }
         }
     }
     return HS_SUCCESS;
@@ -1112,9 +1177,10 @@ struct Upload {
  * ranges, read the counters back.  The only place a scan's stream sequence is issued. */
 hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
                        cudaStream_t stream, const Upload *up = nullptr) {
-    if (s->nPeers && im->nfaLength && im->kind != FK_OUTFIX) {
+    if (s->nPeers && (im->rules.shape == SHAPE_LITERALS_OUTFIX || im->rules.shape == SHAPE_OUTFIXES)) {
         /* the engine kernel stores no records into the peers' exchange buffers, and the count it
-         * publishes would cover them: an exchange of both halves' records is not built */
+         * publishes would cover them: an exchange of both halves' records, or of several engines',
+         * is not built */
         return HS_ARCH_ERROR;
     }
     ScanPlan pl;
@@ -2113,6 +2179,7 @@ hs_error_t hs_b200_nfa_scan_corpus(const void *nfa, size_t nfa_len, const hs_b20
     std::vector<DevMatch> host;
     cudaError_t e = cudaMalloc(&d_nfa, HSB_ROUNDUP(nfa_len, 16));
     if (e == cudaSuccess) e = cudaMemcpy(d_nfa, nfa, nfa_len, cudaMemcpyHostToDevice);
+    p.nfa = d_nfa;
     if (e == cudaSuccess) e = cudaMalloc(&d_ctr, CTR_COUNT * sizeof(u32));
     if (e == cudaSuccess) e = cudaEventCreate(&ev0);
     if (e == cudaSuccess) e = cudaEventCreate(&ev1);
@@ -2121,7 +2188,7 @@ hs_error_t hs_b200_nfa_scan_corpus(const void *nfa, size_t nfa_len, const hs_b20
         if (e != cudaSuccess) break;
         e = cudaMemset(d_ctr, 0, CTR_COUNT * sizeof(u32));
         if (e == cudaSuccess) e = cudaEventRecord(ev0, 0);
-        if (e == cudaSuccess) e = launchEngine(p, d_nfa, corpus, d_out, capDev, d_ctr, smCount, maxSmem, 0);
+        if (e == cudaSuccess) e = launchEngine(p, corpus, d_out, capDev, d_ctr, smCount, maxSmem, 0);
         if (e == cudaSuccess) e = cudaEventRecord(ev1, 0);
         u32 ctr[CTR_COUNT] = {0};
         if (e == cudaSuccess) e = cudaMemcpy(ctr, d_ctr, sizeof(ctr), cudaMemcpyDeviceToHost);

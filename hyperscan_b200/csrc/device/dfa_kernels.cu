@@ -56,11 +56,11 @@ __device__ __forceinline__ u32 emitDfaMatch(const DfaParams &p, u32 cursor, u32 
     return cursor + 1;
 }
 
-/* struct report_list {u32 count; ReportID report[]} at NFA offset `off` */
-__device__ u32 emitReportList(const DfaParams &p, u32 cursor, u32 off, u32 block, u64 to) {
-    const u32 n = g32(p.nfa + off);
+/* struct report_list {u32 count; ReportID report[]} at offset `off` of the engine at `nfa` */
+__device__ u32 emitReportList(const DfaParams &p, const u8 *nfa, u32 cursor, u32 off, u32 block, u64 to) {
+    const u32 n = g32(nfa + off);
     for (u32 i = 0; i < n; i++) {
-        cursor = emitDfaMatch(p, cursor, g32(p.nfa + off + 4 + 4 * i), block, to);
+        cursor = emitDfaMatch(p, cursor, g32(nfa + off + 4 + 4 * i), block, to);
     }
     return cursor;
 }
@@ -223,8 +223,9 @@ template <int W> struct StOps<WideSt<W>> {
 };
 
 /* LimEx report list: ReportID[] terminated by MO_INVALID_IDX (limexRunReports, limex_runtime.h:90-103) */
-__device__ HSB_NOINLINE u32 emitLimexReports(const DfaParams &p, u32 cursor, u32 listOff, u32 block, u64 to) {
-    const u8 *lx = p.nfa + sizeof(NFA);
+__device__ HSB_NOINLINE u32 emitLimexReports(const DfaParams &p, const u8 *nfa, u32 cursor, u32 listOff, u32 block,
+                                             u64 to) {
+    const u8 *lx = nfa + sizeof(NFA);
     for (u32 i = 0;; i++) {
         const u32 id = g32(lx + listOff + 4 * i);
         if (id == MO_INVALID_IDX) {
@@ -238,9 +239,9 @@ __device__ HSB_NOINLINE u32 emitLimexReports(const DfaParams &p, u32 cursor, u32
 /* accepts of the states in `found` through an NFAAccept table (PROCESS_ACCEPTS_IMPL_FN,
  * limex_common_impl.h:116-163; the squash of PROCESS_ACCEPTS_FN is dead code there) */
 template <class ST>
-__device__ HSB_NOINLINE u32 emitLimexAccepts(const DfaParams &p, u32 cursor, ST found, ST mask, u32 tableOff,
-                                             u32 block, u64 to) {
-    const u8 *lx = p.nfa + sizeof(NFA);
+__device__ HSB_NOINLINE u32 emitLimexAccepts(const DfaParams &p, const u8 *nfa, u32 cursor, ST found, ST mask,
+                                             u32 tableOff, u32 block, u64 to) {
+    const u8 *lx = nfa + sizeof(NFA);
     StOps<ST>::forEach(found, [&](const u32 bit) {
         const u32 idx = StOps<ST>::rank(mask, bit);
         const u8 *a = lx + tableOff + idx * (u32)sizeof(NFAAccept);
@@ -248,7 +249,7 @@ __device__ HSB_NOINLINE u32 emitLimexAccepts(const DfaParams &p, u32 cursor, ST 
         if (__ldg(a + offsetof(NFAAccept, single_report))) {
             cursor = emitDfaMatch(p, cursor, reports, block, to);
         } else {
-            cursor = emitLimexReports(p, cursor, reports, block, to);
+            cursor = emitLimexReports(p, nfa, cursor, reports, block, to);
         }
     });
     return cursor;
@@ -389,19 +390,34 @@ struct DfaConsts {
 /* reports of a state that was just entered at offset `to` (doComplexReport, mcclellan.c:43-91;
  * fireReports, sheng_impl.h:116-155).  what = the one report of a single-report engine, else
  * the offset of the state's aux record.  Returns the lane's record cursor. */
-__device__ HSB_NOINLINE u32 emitAccept(const DfaParams &p, u32 cursor, u32 single, u32 what, u32 block, u64 to) {
+__device__ HSB_NOINLINE u32 emitAccept(const DfaParams &p, const u8 *nfa, u32 cursor, u32 single, u32 what, u32 block,
+                                       u64 to) {
     if (single) {
         return emitDfaMatch(p, cursor, what, block, to);
     }
-    return emitReportList(p, cursor, g32(p.nfa + what), block, to);
+    return emitReportList(p, nfa, cursor, g32(nfa + what), block, to);
 }
 
-template <int ENGINE, int SMEM_TABLE, int CH, int ILP>
+template <int ENGINE, int SMEM_TABLE, int CH, int ILP, bool FUSED>
 __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(const HSB_GRID_CONSTANT DfaParams p) {
     HSB_DYNAMIC_SMEM(smem);
     typedef DfaTile<CH> Tile;
     const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-    const u8 *eng = p.nfa + sizeof(NFA); /* struct mcclellan / struct sheng */
+    /* the engine: p's own, or in a fused launch engine blockIdx.x / ctas of p.engines (the grid is engine-major:
+     * `ctas` CTAs per engine), read once per CTA */
+    const u8 *nfa = p.nfa;
+    u32 tableBytes = p.tableBytes, squashes = p.squashes;
+    u32 cta = blockIdx.x, ctas = gridDim.x;
+    if constexpr (FUSED) {
+        ctas = gridDim.x / p.nengines;
+        const u32 which = blockIdx.x / ctas;
+        cta = blockIdx.x - which * ctas;
+        const DfaEngine *e = p.engines + which;
+        nfa = e->nfa;
+        tableBytes = e->tableBytes;
+        squashes = e->squashes;
+    }
+    const u8 *eng = nfa + sizeof(NFA); /* struct mcclellan / struct sheng */
     const u8 *succG = eng + sizeof(McClellan);
     DfaConsts k;
     k.as = 0;
@@ -533,10 +549,10 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
         if (SMEM_TABLE) {
             u32 *d = reinterpret_cast<u32 *>(smem + 256);
             const u32 *g = reinterpret_cast<const u32 *>(succG);
-            for (u32 i = threadIdx.x; i < (p.tableBytes + 3) / 4; i += blockDim.x) {
+            for (u32 i = threadIdx.x; i < (tableBytes + 3) / 4; i += blockDim.x) {
                 d[i] = __ldg(g + i);
             }
-            tabArea += HSB_ROUNDUP(p.tableBytes, 16);
+            tabArea += HSB_ROUNDUP(tableBytes, 16);
         }
     }
     __syncthreads();
@@ -585,10 +601,10 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
             Ops::forEach(Ops::band(s, tShift[8]), [&](const u32 bit) {
                 const u32 rep = reinterpret_cast<const u32 *>(smem + T::REP)[bit];
                 if (rep != MO_INVALID_IDX && pos != 0) {
-                    cursor = emitLimexReports(p, cursor, rep, blk, pos);
+                    cursor = emitLimexReports(p, nfa, cursor, rep, blk, pos);
                 }
                 local = Ops::bor(local, Ops::loadChunks(reinterpret_cast<const uint4 *>(smem + T::LOCAL), T::STATES, bit));
-                if (p.squashes) {
+                if (squashes) {
                     keep = Ops::band(keep, Ops::loadChunks(reinterpret_cast<const uint4 *>(smem + T::KEEP), T::STATES, bit));
                 }
             });
@@ -612,7 +628,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                 const ST *e = lxRows + 4 * bit;
                 const u32 rep = Ops::low32(e[3]);
                 if (rep != MO_INVALID_IDX && pos != 0) {
-                    cursor = emitLimexReports(p, cursor, rep, blk, pos);
+                    cursor = emitLimexReports(p, nfa, cursor, rep, blk, pos);
                 }
                 lim = Ops::bor(lim, e[0]);
                 local = Ops::bor(local, e[1]);
@@ -633,7 +649,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
             if (s < k.shermanLimit) {
                 e = SMEM_TABLE ? succ16[(s << k.as) + cp] : __ldg(succ16 + (s << k.as) + cp);
             } else {
-                e = shermanNext(p.nfa, k.shermanOffset, k.shermanLimit, s, cp, reinterpret_cast<const u16 *>(succG),
+                e = shermanNext(nfa, k.shermanOffset, k.shermanLimit, s, cp, reinterpret_cast<const u16 *>(succG),
                                 k.as);
             }
             s = e & MCC_STATE_MASK;
@@ -651,7 +667,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
      * of the group: ILP independent state chains in one instruction stream */
     const u32 perGroup = 32 * ILP;
     const u32 ngroups = (p.nblocks + perGroup - 1) / perGroup;
-    for (u32 g = blockIdx.x * nwarps + warp; g < ngroups; g += gridDim.x * nwarps) {
+    for (u32 g = cta * nwarps + warp; g < ngroups; g += ctas * nwarps) {
         u32 b[ILP], len[ILP];
         ST s[ILP];
         u64 off[ILP];
@@ -734,7 +750,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll
                         for (int u = 0; u < ILP; u++) {
                             if (step(w[u][j >> 2], j & 3, s[u], done + c * 16 + j, b[u])) {
-                                cursor = emitAccept(p, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + c * 16 + j + 1);
+                                cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + c * 16 + j + 1);
                             }
                         }
                     }
@@ -768,7 +784,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll
                         for (u32 j = 0; j < 16; j++) {
                             if (step(w[j >> 2], j & 3, s[u], done + cc * 16 + j, b[u])) {
-                                cursor = emitAccept(p, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
+                                cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
                             }
                         }
                         live[u] = !dead(s[u]);
@@ -780,7 +796,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll 1
                         for (u32 j = 0; j < m; j++) {
                             if (step(w[j >> 2] >> (8 * (j & 3)), 0, s[u], done + cc * 16 + j, b[u])) {
-                                cursor = emitAccept(p, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
+                                cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
                             }
                         }
                         live[u] = !dead(s[u]);
@@ -797,20 +813,20 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                     /* STREAM_FN's closing accept check (only if the block had bytes to stream),
                      * then nfaExecLimEx*_testEOD (limex_common_impl.h:192-218) */
                     if (len[u] && Ops::any(Ops::band(s[u], lxAccept))) {
-                        cursor = emitLimexAccepts<ST>(p, cursor, Ops::band(s[u], lxAccept), lxAccept,
+                        cursor = emitLimexAccepts<ST>(p, nfa, cursor, Ops::band(s[u], lxAccept), lxAccept,
                                                       g32(eng + offsetof(LxNfa, acceptOffset)), b[u], len[u]);
                     }
                     if (Ops::any(Ops::band(s[u], lxAcceptEod))) {
-                        cursor = emitLimexAccepts<ST>(p, cursor, Ops::band(s[u], lxAcceptEod), lxAcceptEod,
+                        cursor = emitLimexAccepts<ST>(p, nfa, cursor, Ops::band(s[u], lxAcceptEod), lxAcceptEod,
                                                       g32(eng + offsetof(LxNfa, acceptEodOffset)), b[u], len[u]);
                     }
                 }
             } else if (b[u] < p.nblocks) {
                 const u32 eodOff = ENGINE == ENG_SHENG ? (u32)offsetof(SstateAux, accept_eod)
                                                        : (u32)offsetof(MStateAux, accept_eod);
-                const u32 eod = g32(p.nfa + k.auxOffset + k.auxSize * (Ops::low32(s[u]) & k.stateMask) + eodOff);
+                const u32 eod = g32(nfa + k.auxOffset + k.auxSize * (Ops::low32(s[u]) & k.stateMask) + eodOff);
                 if (eod) {
-                    cursor = emitReportList(p, cursor, eod, b[u], len[u]);
+                    cursor = emitReportList(p, nfa, cursor, eod, b[u], len[u]);
                 }
             }
         }
@@ -824,18 +840,23 @@ cudaError_t launchStaged(const DfaParams &p, int smCount, size_t tableBytes, cud
      * ilp 2: two blocks per lane, 64 bytes of each per refill (160 KiB of tiles);
      * ilp 1: one block per lane, 128 bytes per refill (144 KiB) */
     const int threads = StagedThreads<ENGINE>::N;
-    const bool two = p.ilp == 2 && ENGINE < ENG_LIMEX128; /* (the wide models walk one block per lane) */
+    /* (the wide models, and a fused launch, walk one block per lane) */
+    const bool fused = p.engines != nullptr;
+    const bool two = !fused && p.ilp == 2 && ENGINE < ENG_LIMEX128;
     const size_t tiles = (size_t)(threads / 32) * (two ? 2 * DfaTile<64>::WARP_BYTES : DfaTile<128>::WARP_BYTES);
     const u64 groups = ((u64)p.nblocks + (two ? 63 : 31)) / (two ? 64 : 32);
+    /* per engine: `grid` CTAs over all blocks (a fused launch has that many per engine, and the CTAs of every
+     * engine share the GPU: a corpus too small to fill it for one engine fills it for several) */
     const int grid = (int)std::min<u64>((u64)smCount, (groups + threads / 32 - 1) / (threads / 32));
-    void (*kern)(const DfaParams) =
-        two ? dfaStagedKernel<ENGINE, SMEM_TABLE, 64, 2> : dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1>;
+    void (*kern)(const DfaParams) = fused ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, true>
+                                    : two ? dfaStagedKernel<ENGINE, SMEM_TABLE, 64, 2, false>
+                                          : dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false>;
     const size_t smem = tableBytes + tiles;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) {
         return e;
     }
-    HSB_LAUNCH(kern, grid, threads, smem, stream, p);
+    HSB_LAUNCH(kern, grid * (fused ? (int)p.nengines : 1), threads, smem, stream, p);
     return cudaGetLastError();
 }
 

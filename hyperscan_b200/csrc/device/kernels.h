@@ -48,7 +48,7 @@ enum FilterKind {
                       literals are all >= 4 bytes.  Table image: 256 class words
                       (4 * c); ScanParams.bitmap = the bitmap (bitmapBytes), bit c[e] of word
                       c[e-3] + 33 c[e-2] + 1025 c[e-1] */
-    FK_OUTFIX = 6, /* no literal first stage at all: a single-outfix database, its one engine runs on
+    FK_OUTFIX = 6, /* no literal first stage at all: a database of one outfix or several, its engines run on
                       the DFA / NFA kernels (dfa_kernels.cu) */
 };
 
@@ -161,6 +161,16 @@ cudaError_t launchStreamAssemble(u8 *corpus, const u8 *hist, u32 nstreams, u32 p
 cudaError_t launchStreamAdvance(const u8 *corpus, u8 *hist, u64 *offsets, const u32 *lens, u32 uniformLen,
                                 u32 nstreams, u32 pitch, u32 histReq, cudaStream_t stream);
 
+/* one engine of a fused launch (DfaParams.engines): its bytes in device memory and the DfaParams fields
+ * that differ from engine to engine */
+struct DfaEngine {
+    const u8 *nfa;
+    u32 tableBytes;
+    u32 states;
+    u32 squashes;
+    u32 pad;
+};
+
 /* DFA engines in block mode (dfa_kernels.cu): McClellan 8 / 16, Sheng -- the engine's
  * own bytes (struct NFA first) in device memory, one thread per block. */
 struct DfaParams {
@@ -181,6 +191,11 @@ struct DfaParams {
     u32 *counters;   /* CTR_MATCHES */
     u64 toTag;       /* ORed into every record's offset: ENGINE_RECORD (db_walk.h) when the engine's records
                       * share the ring with a literal matcher's, else 0 */
+    /* != null: ONE launch over nengines engines of this kind (device memory), each over every block; the grid
+     * is engine-major, the CTAs of engines[i] come i-th, and its nfa, tableBytes and squashes stand in for the
+     * fields above.  tableBytes and states then hold the largest engine's, which size the shared memory. */
+    const DfaEngine *engines;
+    u32 nengines;
 };
 cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t stream);
 

@@ -408,6 +408,7 @@ hs_error_t hs_b200_db_info(const hs_database_t *db, hs_b200_db_info_t *out) {
     out->bytecode_len = ((const DbHeader *)db)->length;
     out->min_width = r->minWidth;
     out->num_literals = r->totalNumLiterals;
+    out->engine_count = r->queueCount;
     if (r->fmatcherOffset) {
         const HWLM *h = (const HWLM *)((const u8 *)r + r->fmatcherOffset);
         out->hwlm_type = h->type;
@@ -1070,19 +1071,22 @@ static hs_error_t compileCommon(const char *const *expressions,
                 }
             }
             const bool canSplit = !pats.empty() && !engineHalf.empty() && !anyCombination && !opts.streaming;
+            /* no literals to move out: the expressions themselves can be split over several engines */
+            const bool canSplitEngines = pats.empty() && !anyCombination && !opts.streaming;
             if (canSplit && mixedRoseOption()) {
                 bc = buildMixedRose(pats, engineHalf, opts, nullptr);
             } else {
                 try {
                     bc = buildRegexRose(rpats, opts, ls);
                 } catch (const CompileError &e) {
-                    /* the literals' character positions overflow the one automaton: the literals go to
-                     * a literal matcher and the rest to the engine; if that fails too, the error stays */
-                    if (!canSplit || e.msg.rfind("Pattern set is too large", 0) != 0) {
+                    /* the character positions overflow the one automaton: the literals go to a literal
+                     * matcher and the rest to the engine, or a set without literals goes to several
+                     * engines; if that fails too, the error stays */
+                    if (!(canSplit || canSplitEngines) || e.msg.rfind("Pattern set is too large", 0) != 0) {
                         throw;
                     }
                     try {
-                        bc = buildMixedRose(pats, engineHalf, opts, nullptr);
+                        bc = canSplit ? buildMixedRose(pats, engineHalf, opts, nullptr) : buildMultiOutfixRose(rpats, opts);
                     } catch (const CompileError &) {
                         throw e;
                     }

@@ -404,14 +404,16 @@ DbShape dbShape(const hs_database_t *db) {
         !r->ematcherOffset && !r->fmatcherOffset && !r->hasSom) {
         return SHAPE_SOLE_OUTFIX;
     }
-    /* the one FULL_ROSE shape run here: the floating literal matcher, whose role-less programs report
-     * directly, and one outfix on queue 0 (DESIGN.md section 10d) -- no anchored, EOD or small-block
-     * matcher, no roles, leftfixes, suffixes, delayed literals, MPV, SOM or long-literal table, and an
-     * EOD program that at most checks the engines' EOD accepts */
-    if (r->runtimeImpl == RUNTIME_FULL_ROSE && r->mode == MODE_BLOCK && r->fmatcherOffset && !r->amatcherOffset &&
-        !r->ematcherOffset && !r->sbmatcherOffset && !r->drmatcherOffset && r->queueCount == 1 &&
-        r->activeArrayCount == 1 && r->outfixBeginQueue == 0 && r->outfixEndQueue == 1 &&
-        r->leftfixBeginQueue == 1 && r->nfaInfoOffset && !r->activeLeftCount && !r->rosePrefixCount &&
+    /* the FULL_ROSE shapes run here: outfixes on queues [0, K) only, beside the floating literal matcher,
+     * whose role-less programs report directly (one outfix, DESIGN.md section 10d), or alone (up to
+     * MAX_OUTFIX_QUEUES, section 10e) -- no anchored, EOD or small-block matcher, no roles, leftfixes,
+     * suffixes, delayed literals, MPV, SOM or long-literal table, and an EOD program that at most checks
+     * the engines' EOD accepts */
+    const u32 k = r->queueCount;
+    if (r->runtimeImpl == RUNTIME_FULL_ROSE && r->mode == MODE_BLOCK && (r->fmatcherOffset ? k == 1 : k <= MAX_OUTFIX_QUEUES) &&
+        !r->amatcherOffset && !r->ematcherOffset && !r->sbmatcherOffset && !r->drmatcherOffset && k >= 1 &&
+        r->activeArrayCount == k && r->outfixBeginQueue == 0 && r->outfixEndQueue == k &&
+        r->leftfixBeginQueue == k && r->nfaInfoOffset && !r->activeLeftCount && !r->rosePrefixCount &&
         !r->rolesWithStateCount && !r->delay_count && !r->anchored_count && r->initMpvNfa == MO_INVALID_IDX &&
         !r->hasSom && !r->longLitTableOffset && !r->ckeyCount && !r->eagerIterOffset && !r->delayProgramOffset &&
         !r->anchoredProgramOffset && !r->boundary.reportEodOffset && !r->boundary.reportZeroOffset &&
@@ -420,7 +422,7 @@ DbShape dbShape(const hs_database_t *db) {
          ((size_t)r->eodProgramOffset + 16 <= h->length && r->eodProgramOffset % INSTR_ALIGN == 0 &&
           bc[r->eodProgramOffset] == OP_ENGINES_EOD &&
           bc[r->eodProgramOffset + HSB_ROUNDUP(sizeof(InstrEnginesEod), INSTR_ALIGN)] == OP_END))) {
-        return SHAPE_LITERALS_OUTFIX;
+        return r->fmatcherOffset ? SHAPE_LITERALS_OUTFIX : SHAPE_OUTFIXES;
     }
     return SHAPE_UNSUPPORTED;
 }
@@ -437,8 +439,8 @@ hs_error_t loadReportRules(const hs_database_t *db, ReportRules *rules, std::vec
     if (r->ckeyCount) {
         loadCombinations(r, &rules->comb);
     }
-    if (rules->shape == SHAPE_SOLE_OUTFIX) {
-        return HS_SUCCESS; /* no literal programs: the engine's are walked as its records are delivered */
+    if (rules->shape == SHAPE_SOLE_OUTFIX || rules->shape == SHAPE_OUTFIXES) {
+        return HS_SUCCESS; /* no literal programs: the engines' are walked as their records are delivered */
     }
     const HWLM *hw = (const HWLM *)(rules->bc + r->fmatcherOffset);
     const u32 engOff = r->fmatcherOffset + HWLM_ENGINE_OFFSET;
@@ -592,12 +594,14 @@ bool enginePrograms(const u8 *nfa, u32 len, std::vector<u32> *out) {
 
 } // namespace
 
-hs_error_t buildDeviceRules(ReportRules *rules, const u8 *nfa, u32 nfaLen, DeviceRules *out) {
+hs_error_t buildDeviceRules(ReportRules *rules, const std::vector<EngineBytes> &engines, DeviceRules *out) {
     *out = DeviceRules();
-    if (nfa) {
-        std::vector<u32> progs;
-        if (!enginePrograms(nfa, nfaLen, &progs)) {
-            return HS_INVALID;
+    if (!engines.empty()) {
+        std::vector<u32> progs; /* (the engines' reports are offsets into one bytecode: one table serves all) */
+        for (const EngineBytes &e : engines) {
+            if (!enginePrograms(e.nfa, e.len, &progs)) {
+                return HS_INVALID;
+            }
         }
         std::sort(progs.begin(), progs.end());
         progs.erase(std::unique(progs.begin(), progs.end()), progs.end());

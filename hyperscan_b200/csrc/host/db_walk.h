@@ -71,12 +71,13 @@ static const u64 LKEY_RECORD = 1ull << 63;
  * outfix: its id is a report PROGRAM offset, resolved on the host; the literal records carry report ids. */
 static const u64 ENGINE_RECORD = 1ull << 62;
 
-/* The database shapes the device runs (DESIGN.md sections 10a, 10d). */
+/* The database shapes the device runs (DESIGN.md sections 10a, 10d, 10e). */
 enum DbShape {
     SHAPE_UNSUPPORTED = 0, /* needs the full rose interpreter (SURVEY.md section 8f rank 1): not in this build */
     SHAPE_PURE_LITERAL,    /* the floating literal matcher alone */
     SHAPE_SOLE_OUTFIX,     /* one engine over the whole block, no literal matcher */
     SHAPE_LITERALS_OUTFIX, /* the floating literal matcher beside one outfix (FULL_ROSE, block mode) */
+    SHAPE_OUTFIXES,        /* up to MAX_OUTFIX_QUEUES outfixes and no literal matcher (FULL_ROSE, block mode) */
 };
 DbShape dbShape(const hs_database_t *db);
 
@@ -102,8 +103,8 @@ struct ReportRules {
 
     /* Records of a scan in delivery order, (block, to, id), with the report rules the device skipped
      * applied.  An engine's records carry report PROGRAM offsets (and the padding of the lanes' reserved
-     * slots) -- all of a single-outfix database's records, and those tagged ENGINE_RECORD beside a literal
-     * matcher; each is replaced by the reports its program raises -- roseReportAdaptor -> roseRunProgram
+     * slots) -- all records of a database without a literal matcher, and those tagged ENGINE_RECORD beside
+     * a literal matcher; each is replaced by the reports its program raises -- roseReportAdaptor -> roseRunProgram
      * (src/rose/match.c:611-633) -- with CHECK_BOUNDS and offset_adjust applied, and the literals' records
      * join them as they are.  Then one report per (block, id, to) (dedupe, src/report.h:55-119) and, for
      * HS_FLAG_SINGLEMATCH reports, only the first match per block (exhaustion keys, src/report.h:121-147,
@@ -131,11 +132,16 @@ struct DeviceRules {
     std::vector<u32> ids;
     std::vector<u8> idExhaustible;
 };
-/* Walk every report program of the engine (its bytes nfa[0, nfaLen), struct NFA first; none if nfa is
- * null) as ReportRules::deliver would on meeting it, which completes rules->progReports and
- * rules->exhaustible, and lay the rules out as tables.  HS_INVALID: the engine's report lists run past
- * its end; HS_UNKNOWN_ERROR: a program holds an opcode the device does not implement. */
-hs_error_t buildDeviceRules(ReportRules *rules, const u8 *nfa, u32 nfaLen, DeviceRules *out);
+/* an engine's bytes, struct NFA first */
+struct EngineBytes {
+    const u8 *nfa;
+    u32 len;
+};
+/* Walk every report program of the engines (none for a pure-literal database) as ReportRules::deliver
+ * would on meeting it, which completes rules->progReports and rules->exhaustible, and lay the rules out
+ * as tables.  HS_INVALID: an engine's report lists run past its end; HS_UNKNOWN_ERROR: a program holds an
+ * opcode the device does not implement. */
+hs_error_t buildDeviceRules(ReportRules *rules, const std::vector<EngineBytes> &engines, DeviceRules *out);
 
 } // namespace hsb
 #endif

@@ -311,25 +311,100 @@ void addFloatingMatcher(Blob &blob, RoseEngine *r, const std::vector<HwlmLit> &h
     r->totalNumLiterals = (u32)hl.size();
 }
 
-/* Queue 0 holds the engine at nfaOffset (header hdr) as the database's only outfix: its NfaInfo,
- * the queue counts, its full state in scratch and its stream state at `cur` (nfaStateBegin). */
-void addOutfixQueue(Blob &blob, RoseEngine *r, u32 nfaOffset, const NFA &hdr, u32 cur) {
-    r->activeArrayCount = 1;
-    r->queueCount = 1;
-    r->activeQueueArraySize = fatbitSize(1);
+/* Queues [0, K) hold the K engines added to the blob (`engines`: offset and header of each) as the
+ * database's outfixes: one NfaInfo per queue, the queue counts, each queue's full state in scratch
+ * (64-byte aligned) and its stream state from `cur` (nfaStateBegin) on, in queue order
+ * (allocateStateSpace, src/rose/rose_build_bytecode.cpp:2077-2099). */
+void addOutfixQueues(Blob &blob, RoseEngine *r, const std::vector<std::pair<u32, NFA>> &engines, u32 cur) {
+    const u32 k = (u32)engines.size();
+    r->activeArrayCount = k;
+    r->queueCount = k;
+    r->activeQueueArraySize = fatbitSize(k);
     r->outfixBeginQueue = 0;
-    r->outfixEndQueue = 1;
-    r->leftfixBeginQueue = 1;
-    r->scratchStateSize = (u32)HSB_ROUNDUP(hdr.scratchStateSize, 64); /* the queue's full state, in scratch */
-    NfaInfo ni;
-    memset(&ni, 0, sizeof(ni));
-    ni.nfaOffset = nfaOffset;
-    ni.stateOffset = cur;
-    ni.fullStateOffset = 0;
-    cur += hdr.streamStateSize;
+    r->outfixEndQueue = k;
+    r->leftfixBeginQueue = k;
+    std::vector<NfaInfo> infos(k);
+    memset(infos.data(), 0, k * sizeof(NfaInfo));
+    u32 full = 0;
+    for (u32 q = 0; q < k; q++) {
+        infos[q].nfaOffset = engines[q].first;
+        infos[q].stateOffset = cur;
+        infos[q].fullStateOffset = full;
+        cur += engines[q].second.streamStateSize;
+        full = (u32)HSB_ROUNDUP(full + engines[q].second.scratchStateSize, 64);
+    }
+    r->scratchStateSize = full;
     r->stateOffsets.end = cur;
     r->stateSize = cur;
-    r->nfaInfoOffset = blob.add(&ni, sizeof(ni), 4);
+    r->nfaInfoOffset = blob.add(infos.data(), k * sizeof(NfaInfo), 4);
+}
+
+/* each engine's bytes added to the blob, 64-byte aligned: its offset and header */
+std::vector<std::pair<u32, NFA>> addEngines(Blob &blob, const std::vector<std::vector<u8>> &nfas) {
+    std::vector<std::pair<u32, NFA>> out;
+    for (const std::vector<u8> &nfa : nfas) {
+        NFA hdr;
+        memcpy(&hdr, nfa.data(), sizeof(hdr));
+        out.emplace_back(blob.add(nfa.data(), nfa.size(), 64), hdr);
+    }
+    return out;
+}
+
+/* makeEodProgram (rose_build_bytecode.cpp:3334-3350) with only addEnginesEodProgram: when some engine accepts
+ * at end of data, ENGINES_EOD over a sparse iterator of those queues (buildEodNfaIterator, :2276-2294; with
+ * at most 64 queues the iterator is one record) and END; requiresEodCheck (hasEodAnchors, :2446-2475). */
+void addEnginesEodProgram(Blob &blob, RoseEngine *r, const std::vector<std::pair<u32, NFA>> &engines) {
+    u64 eodQueues = 0;
+    for (u32 q = 0; q < engines.size(); q++) {
+        if (engines[q].second.flags & NFA_ACCEPTS_EOD) {
+            eodQueues |= 1ull << q;
+        }
+    }
+    if (!eodQueues) {
+        return;
+    }
+    const MmbSparseIter it = {eodQueues, 0};
+    const u32 iter = blob.add(&it, sizeof(it), alignof(MmbSparseIter));
+    const u32 prog = blob.reserve(instrSize<InstrEnginesEod>() + instrSize<InstrEnd>(), INSTR_ALIGN);
+    InstrEnginesEod ee;
+    memset(&ee, 0, sizeof(ee));
+    ee.code = OP_ENGINES_EOD;
+    ee.iter_offset = iter;
+    memcpy(blob.at(prog), &ee, sizeof(ee));
+    *blob.at(prog + instrSize<InstrEnginesEod>()) = OP_END;
+    r->eodProgramOffset = prog;
+    r->requiresEodCheck = 1;
+}
+
+/* The state scatter plan of a block-mode database without roles or leftfixes (buildStateScatterPlan,
+ * rose_build_scatter.cpp:66-97): the units that clear the active leaf array of `leaves` <= 64 bits, as the
+ * flat multibit's clear plan splits them (mmbBuildInitRangePlan, src/util/multibit_build.cpp:216-253), in
+ * the order write_out lays them out (u64, u32, u16, u8). */
+void addStateScatterPlan(Blob &blob, RoseEngine *r, u32 leaves) {
+    const u32 at = r->stateOffsets.activeLeafArray;
+    ScatterPlan &sp = r->state_init;
+    auto wide = [&](u32 bits, u32 lo) { return leaves > lo && leaves <= bits; };
+    if (leaves > 56) {
+        const ScatterUnitU64 u = {at, 0};
+        sp.s_u64a_offset = blob.add(&u, sizeof(u), alignof(ScatterUnitU64));
+        sp.s_u64a_count = 1;
+        return;
+    }
+    if (leaves > 24) {
+        const ScatterUnitU32 u = {at, 0};
+        sp.s_u32_offset = blob.add(&u, sizeof(u), alignof(ScatterUnitU32));
+        sp.s_u32_count = 1;
+    }
+    if (wide(16, 8) || wide(24, 16) || wide(48, 40) || wide(56, 48)) {
+        const ScatterUnitU16 u = {leaves > 24 ? at + 4 : at, 0};
+        sp.s_u16_offset = blob.add(&u, sizeof(u), alignof(ScatterUnitU16));
+        sp.s_u16_count = 1;
+    }
+    if (leaves <= 8 || wide(24, 16) || wide(40, 32) || wide(56, 48)) {
+        const ScatterUnitU8 u = {leaves <= 8 ? at : leaves <= 24 ? at + 2 : leaves <= 40 ? at + 4 : at + 6, 0};
+        sp.s_u8_offset = blob.add(&u, sizeof(u), alignof(ScatterUnitU8));
+        sp.s_u8_count = 1;
+    }
 }
 
 /* header + blob, the header's size field set */
@@ -348,16 +423,14 @@ std::vector<u8> emitRose(const Blob &blob, RoseEngine *r) {
  * engine and no literal (rose_build_bytecode.cpp:3672-3690 pickRuntimeImpl); here it is built
  * for literal sets on request, so that the DFA / NFA engines run inside a real database. */
 std::vector<u8> finishOutfixRose(Blob &blob, const std::vector<u8> &nfa, const RoseTail &t) {
-    NFA hdr;
-    memcpy(&hdr, nfa.data(), sizeof(hdr));
-    const u32 nfaOffset = blob.add(nfa.data(), nfa.size(), 64);
+    const std::vector<std::pair<u32, NFA>> engines = addEngines(blob, {nfa});
     RoseEngine r;
     memset(&r, 0, sizeof(r));
     writeLogicalInfo(blob, t.logic, &r);
     commonHeader(&r, t);
     r.runtimeImpl = RUNTIME_SINGLE_OUTFIX;
     r.mode = MODE_BLOCK;
-    addOutfixQueue(blob, &r, nfaOffset, hdr, layoutState(&r, 1, 0, 0));
+    addOutfixQueues(blob, &r, engines, layoutState(&r, 1, 0, 0));
     return emitRose(blob, &r);
 }
 
@@ -382,48 +455,31 @@ std::vector<u8> finishRose(Blob &blob, const std::vector<HwlmLit> &hl, const Ros
     return emitRose(blob, &r);
 }
 
-/* A database with the floating literal matcher over `hl` AND one engine (`nfa`) as the outfix on
- * queue 0 (ROSE_RUNTIME_FULL_ROSE; hs_scan -> roseBlockExec, src/rose/block.c:345-422):
- * init_for_block clears the active leaf array through the state scatter plan, blockInitSufPQ
- * starts the outfix, the literal programs' CATCH_UP and roseCatchUpTo(length) run it, and when it
- * accepts at end of data the EOD program's ENGINES_EOD checks its final state (roseBlockEodExec).
- * litMinLen: the shortest literal; t.minLen: the shortest match of either half. */
-std::vector<u8> finishMixedRose(Blob &blob, const std::vector<HwlmLit> &hl, u32 litMinLen, const std::vector<u8> &nfa,
-                                const RoseTail &t, const CompileOpts &opts, HwlmBuildInfo *info) {
+/* A FULL_ROSE database (hs_scan -> roseBlockExec, src/rose/block.c:345-422) whose engines (`nfas`) run as
+ * the outfixes on queues [0, K), beside the floating literal matcher over `hl` or, with `hl` empty, alone:
+ * init_for_block clears the active leaf array through the state scatter plan, blockInitSufPQ starts every
+ * outfix, the literal programs' CATCH_UP and roseCatchUpTo(length) run them and merge their reports in
+ * offset order, and for the outfixes that accept at end of data the EOD program's ENGINES_EOD checks their
+ * final states (roseBlockEodExec).  litMinLen: the shortest literal; t.minLen: the shortest match of all. */
+std::vector<u8> finishFullRose(Blob &blob, const std::vector<HwlmLit> &hl, u32 litMinLen,
+                               const std::vector<std::vector<u8>> &nfas, const RoseTail &t, const CompileOpts &opts,
+                               HwlmBuildInfo *info) {
     RoseEngine r;
     memset(&r, 0, sizeof(r));
-    addFloatingMatcher(blob, &r, hl, litMinLen, opts, info);
-    NFA hdr;
-    memcpy(&hdr, nfa.data(), sizeof(hdr));
-    const u32 nfaOffset = blob.add(nfa.data(), nfa.size(), 64);
+    if (!hl.empty()) {
+        addFloatingMatcher(blob, &r, hl, litMinLen, opts, info);
+    }
+    const std::vector<std::pair<u32, NFA>> engines = addEngines(blob, nfas);
     commonHeader(&r, t);
     r.runtimeImpl = RUNTIME_FULL_ROSE;
     r.mode = MODE_BLOCK;
     /* no bi-anchored patterns (findMaxBAWidth): roseBlockFloating scans blocks of any length */
     r.amatcherMaxBiAnchoredWidth = ROSE_BOUND_INF;
     r.fmatcherMaxBiAnchoredWidth = ROSE_BOUND_INF;
-    const u32 cur = layoutState(&r, 1, 1, 0);
-    if (hdr.flags & NFA_ACCEPTS_EOD) {
-        /* makeEodProgram (rose_build_bytecode.cpp:3334-3350) with only addEnginesEodProgram: ENGINES_EOD over
-         * a sparse iterator of the queues that accept at EOD (buildEodNfaIterator: queue 0 of 1) */
-        const MmbSparseIter it = {1, 0};
-        const u32 iter = blob.add(&it, sizeof(it), alignof(MmbSparseIter));
-        const u32 prog = blob.reserve(instrSize<InstrEnginesEod>() + instrSize<InstrEnd>(), INSTR_ALIGN);
-        InstrEnginesEod ee;
-        memset(&ee, 0, sizeof(ee));
-        ee.code = OP_ENGINES_EOD;
-        ee.iter_offset = iter;
-        memcpy(blob.at(prog), &ee, sizeof(ee));
-        *blob.at(prog + instrSize<InstrEnginesEod>()) = OP_END;
-        r.eodProgramOffset = prog;
-        r.requiresEodCheck = 1; /* hasEodAnchors (:2446-2475): an outfix accepts at EOD */
-    }
-    /* the state scatter plan of a block-mode database (buildStateScatterPlan, rose_build_scatter.cpp:66-97):
-     * no roles and no leftfixes, so one byte that clears the one-bit active leaf array */
-    const ScatterUnitU8 clearLeaf = {r.stateOffsets.activeLeafArray, 0};
-    r.state_init.s_u8_offset = blob.add(&clearLeaf, sizeof(clearLeaf), alignof(ScatterUnitU8));
-    r.state_init.s_u8_count = 1;
-    addOutfixQueue(blob, &r, nfaOffset, hdr, cur);
+    const u32 cur = layoutState(&r, (u32)engines.size(), hl.empty() ? 0 : 1, 0);
+    addEnginesEodProgram(blob, &r, engines);
+    addStateScatterPlan(blob, &r, (u32)engines.size());
+    addOutfixQueues(blob, &r, engines, cur);
     return emitRose(blob, &r);
 }
 
@@ -827,6 +883,39 @@ std::vector<u8> buildRegexEngine(Blob &blob, const std::vector<RegexPattern> &pa
     }
 }
 
+/* The expressions of a set too large for one engine, in groups whose position automaton fits one: packed
+ * greedily in expression order -- an expression joins the last group while that group's automaton can take
+ * its positions (regexNfaAdd stays within the 512-state model), else it opens the next group.  The same set
+ * therefore always splits the same way.  Throws CompileError when an expression does not fit an engine of
+ * its own. */
+std::vector<std::vector<RegexPattern>> packEngineGroups(const std::vector<RegexPattern> &pats) {
+    std::vector<std::vector<RegexPattern>> groups;
+    RawNfa last; /* the automaton of the last group */
+    for (const RegexPattern &p : pats) {
+        try {
+            const RegexInfo ri = regexInfo(p.re.c_str(), p.flags);
+            /* the reports do not change the positions: placeholders stand in for the report programs */
+            auto add = [&](RawNfa *n) { regexNfaAdd(n, p.re.c_str(), p.flags, 1, ri.needsAdjust ? 2 : 0, p.minLength); };
+            if (!groups.empty()) {
+                RawNfa trial = last;
+                try {
+                    add(&trial);
+                    last = std::move(trial);
+                    groups.back().push_back(p);
+                    continue;
+                } catch (const RegexError &) {
+                }
+            }
+            regexNfaInit(&last);
+            add(&last);
+            groups.push_back({p});
+        } catch (const RegexError &e) {
+            throw CompileError{e.msg, (int)p.index};
+        }
+    }
+    return groups;
+}
+
 } // namespace
 
 std::vector<u8> buildLiteralRose(const std::vector<LitPattern> &patsIn,
@@ -1011,7 +1100,38 @@ std::vector<u8> buildMixedRose(const std::vector<LitPattern> &lits, const std::v
     t.dkeyCount = (u32)dkeys.size();
     t.invDkeyOffset = addInvDkeys(blob, dkeys);
     t.canExhaust = litHighlander && regexHighlander;
-    return finishMixedRose(blob, hl, litMin, eng, t, opts, info);
+    return finishFullRose(blob, hl, litMin, {eng}, t, opts, info);
+}
+
+std::vector<u8> buildMultiOutfixRose(const std::vector<RegexPattern> &pats, const CompileOpts &opts) {
+    if (pats.empty() || opts.streaming) {
+        throw CompileError{"Expression sets of several engines are built for block mode only.", -1};
+    }
+    /* one report id is one exhaustion key and one dedupe key, whichever engine raises it */
+    HighlanderMap highlander;
+    std::map<u32, u32> ekeys, dkeys;
+    const bool allHighlander = assignRegexKeys(pats, &highlander, &ekeys, &dkeys);
+    const std::vector<std::vector<RegexPattern>> groups = packEngineGroups(pats);
+    if (groups.size() > MAX_OUTFIX_QUEUES) {
+        throw CompileError{"Pattern set is too large: it needs more than " + std::to_string(MAX_OUTFIX_QUEUES) +
+                               " engines.", -1};
+    }
+    Blob blob((u32)HSB_ROUNDUP(sizeof(RoseEngine), 64));
+    std::vector<std::vector<u8>> engines;
+    u32 minLen = ~0u;
+    for (const std::vector<RegexPattern> &g : groups) {
+        u32 groupMin = 0;
+        engines.push_back(buildRegexEngine(blob, g, ekeys, dkeys, nullptr, opts, &groupMin));
+        minLen = std::min(minLen, groupMin);
+    }
+    RoseTail t;
+    t.minLen = minLen;
+    t.maxLen = 0;
+    t.ekeyCount = (u32)ekeys.size();
+    t.dkeyCount = (u32)dkeys.size();
+    t.invDkeyOffset = addInvDkeys(blob, dkeys);
+    t.canExhaust = allHighlander;
+    return finishFullRose(blob, std::vector<HwlmLit>(), 0, engines, t, opts, nullptr);
 }
 
 /* Test hook (hs_b200_test_compile_programs): a pure-literal block database whose

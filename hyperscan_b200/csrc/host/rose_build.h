@@ -85,6 +85,13 @@ std::vector<u8> buildRegexRose(const std::vector<RegexPattern> &pats, const Comp
 std::vector<u8> buildMixedRose(const std::vector<LitPattern> &lits, const std::vector<RegexPattern> &regexes,
                                const CompileOpts &opts, HwlmBuildInfo *info);
 
+/** Expressions too many for one engine (ROSE_RUNTIME_FULL_ROSE without a literal matcher): the
+ * expressions packed greedily, in order, into groups whose automaton fits one engine, and each group's
+ * engine (McClellan-8 / 16 or LimEx, as buildRegexRose picks it) as the outfix on its own queue, at most
+ * MAX_OUTFIX_QUEUES.  Report ids share their exhaustion and dedupe keys across all engines.  Block mode
+ * only; no logical combinations.  Throws CompileError, also when one expression alone does not fit. */
+std::vector<u8> buildMultiOutfixRose(const std::vector<RegexPattern> &pats, const CompileOpts &opts);
+
 /** Test hook: pure-literal block database from raw literal programs (`area`
  * is placed at programAreaBase(); lits[i].id = its program's offset in area). */
 u32 programAreaBase();

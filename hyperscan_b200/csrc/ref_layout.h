@@ -369,8 +369,15 @@ struct InstrEnginesEod { u8 code; u32 iter_offset; }; /* iter_offset: an MmbSpar
 
 /* one record of a sparse multibit iterator (struct mmbit_sparse_iter, src/util/multibit_internal.h:59-62) */
 struct MmbSparseIter { u64 mask; u32 val; };
-/* one byte of a state scatter plan (struct scatter_unit_u8, src/util/scatter.h) */
+/* the units of a state scatter plan (struct scatter_unit_u64a / _u32 / _u16 / _u8, src/util/scatter.h:35-40) */
+struct ScatterUnitU64 { u32 offset; u64 val; };
+struct ScatterUnitU32 { u32 offset; u32 val; };
+struct ScatterUnitU16 { u32 offset; u16 val; };
 struct ScatterUnitU8 { u32 offset; u8 val; };
+
+/* Not a reference limit: the most outfix queues a database built and run here has.  Up to 64, the active
+ * leaf array is one flat multibit word and a sparse iterator over it is one record. */
+static const u32 MAX_OUTFIX_QUEUES = 64;
 
 /* ---- logical combinations: src/util/logical.h:42-72 -------------------- */
 

@@ -473,6 +473,8 @@ typedef struct hs_b200_db_info {
     unsigned int num_literals;   /* HWLM literal fragments */
     unsigned int bytecode_len;
     unsigned int min_width;
+    unsigned int engine_count;   /* engines run as outfixes (RoseEngine.queueCount): 0 for a pure-literal database,
+                                  * 1 beside or without a literal matcher, K for a set split over K engines */
 } hs_b200_db_info_t;
 hs_error_t hs_b200_db_info(const hs_database_t *db, hs_b200_db_info_t *info);
 
