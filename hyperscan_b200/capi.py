@@ -150,6 +150,7 @@ def lib():
         L.hs_b200_set_build_option.argtypes = [cp, C.c_int]
         L.hs_b200_set_runtime_option.argtypes = [cp, C.c_int]
         L.hs_b200_last_counters.argtypes = [vp, C.POINTER(C.c_uint * 8)]
+        L.hs_b200_engine_segment_stats.argtypes = [vp, C.POINTER(C.c_ulonglong * 4)]
         L.hs_b200_launch_count.restype = C.c_ulonglong
         L.hs_b200_last_kernel_ms.argtypes = [vp]
         L.hs_b200_last_kernel_ms.restype = C.c_float
@@ -332,6 +333,12 @@ class Scratch:
 
     def last_kernel_ms(self):
         return float(lib().hs_b200_last_kernel_ms(self.ptr))
+
+    def segment_stats(self):
+        """hs_b200_engine_segment_stats: {runs, segments, rewalks, rewalk_bytes} since allocation"""
+        out = (C.c_ulonglong * 4)()
+        _check(lib().hs_b200_engine_segment_stats(self.ptr, C.byref(out)))
+        return dict(zip(("runs", "segments", "rewalks", "rewalk_bytes"), map(int, out)))
 
 
 def scan(db, data, scratch, on_event=None, stop_after=0):

@@ -63,6 +63,9 @@ struct RuntimeOpts {
     int heavy = 1;           /* FK_PAIR32 candidate path: 1 (and 2) = per-word entries, 0 = per-lane entries */
     int dfaIlp = 1;          /* DFA kernels: blocks walked by one lane at a time; 2 = two interleaved state chains
                               * per lane (half the warps for the same block count) */
+    int engineSegment = 0;   /* engine runs: 0 = cut long blocks into segments when the blocks leave most resident
+                              * lanes idle (planSegments), N > 0 = cut every block longer than N into N-byte
+                              * segments, -1 = never cut */
     int chunkMB = 128;       /* host->device pipeline granularity */
     int initialRing = 1 << 20;
 };
@@ -78,7 +81,8 @@ void initOpts() {
         {"HSB200_WARPS", &g_opts.warps},       {"HSB200_TILE", &g_opts.tileBytes},
         {"HSB200_CHUNK_MB", &g_opts.chunkMB},  {"HSB200_RING", &g_opts.initialRing},
         {"HSB200_PF_DIST", &g_opts.pfDist},    {"HSB200_HEAVY", &g_opts.heavy},
-        {"HSB200_GRAM", &g_opts.gram},         {"HSB200_DFA_ILP", &g_opts.dfaIlp}};
+        {"HSB200_GRAM", &g_opts.gram},         {"HSB200_DFA_ILP", &g_opts.dfaIlp},
+        {"HSB200_ENGINE_SEGMENT", &g_opts.engineSegment}};
     for (auto &x : e) {
         const char *s = getenv(x.env);
         if (s && *s) {
@@ -86,6 +90,32 @@ void initOpts() {
         }
     }
 }
+
+/* Memory of the segmented engine runs (launchEngine): in device memory the plan, the first open segment of each
+ * block and the per-segment states, grown on demand; the plan's host image in pinned memory, so that its copy
+ * does not wait for the stream; and what the runs did, for hs_b200_engine_segment_stats. */
+struct SegArea {
+    u8 *d = nullptr;
+    size_t bytes = 0;
+    u8 *h = nullptr;                       /* pinned: the plan being copied */
+    size_t hBytes = 0;
+    cudaEvent_t copied = nullptr;          /* recorded after the last copy out of h */
+    std::vector<u8> plan;                  /* the plan now in d (empty: none) */
+    unsigned long long *d_stats = nullptr; /* SEGSTAT_COUNT counters */
+    unsigned long long runs = 0, segments = 0;
+    SegArea() = default;
+    SegArea(const SegArea &) = delete;
+    SegArea &operator=(const SegArea &) = delete;
+    ~SegArea() {
+        if (copied) {
+            cudaEventSynchronize(copied);
+            cudaEventDestroy(copied);
+        }
+        cudaFreeHost(h);
+        cudaFree(d);
+        cudaFree(d_stats);
+    }
+};
 
 /* ---- device image of one database --------------------------------------- */
 
@@ -845,6 +875,7 @@ struct hs_scratch {
     /* temporaries of hs_b200_order_*_async (order_kernels.h), grown on demand */
     u8 *d_order;
     size_t orderBytes;
+    SegArea *seg;            /* of the engine runs, created on first use */
     float lastMs;
     int smCount, maxSmem;
 };
@@ -1087,10 +1118,57 @@ void fillParams(const hs_scratch *s, const DevImage *im, const hs_b200_corpus *c
     }
 }
 
+/* The segment plan of the default rule (engine_segment = 0; DESIGN.md section 10f): blocks are cut only when
+ * they would leave more than half of the lanes an engine launch keeps resident idle, and only blocks longer
+ * than twice the segment length, which is at least SEG_MIN and otherwise as long as makes the corpus about fill
+ * the resident lanes.  A segment's guess comes from SEG_WARM bytes in front of it; SEG_ROUNDS parallel
+ * SEG_JOIN rounds precede the sequential SEG_SETTLE walk. */
+enum : u32 { SEG_MIN = 4096, SEG_WARM = 256, SEG_ROUNDS = 2 };
+
+/* Cut the blocks of c for an engine of `kind`?  Fills the segment table (every block, in order: a block not cut
+ * is one segment with both flags) and the cut blocks {first segment, segments}; false: one lane per block. */
+bool planSegments(const hs_b200_corpus *c, u32 kind, int smCount, std::vector<DfaSeg> *segs,
+                  std::vector<uint2> *cuts) {
+    const int opt = g_opts.engineSegment;
+    if (opt < 0 || c->nblocks == 0 || c->h_len.size() != c->nblocks) {
+        return false;
+    }
+    u64 segLen = (u64)opt, cutAbove = (u64)opt;
+    if (opt == 0) {
+        const u64 lanes = dfaResidentLanes(kind, smCount);
+        if ((u64)c->nblocks * 2 > lanes) {
+            return false; /* the blocks alone keep half the resident lanes busy or more */
+        }
+        segLen = std::max<u64>(SEG_MIN, HSB_ROUNDUP(c->payload / lanes + 1, 16));
+        cutAbove = 2 * segLen;
+    }
+    if (*std::max_element(c->h_len.begin(), c->h_len.end()) <= cutAbove) {
+        return false;
+    }
+    segs->clear();
+    cuts->clear();
+    for (size_t b = 0; b < c->nblocks; b++) {
+        const u32 len = c->h_len[b];
+        if (len <= cutAbove) {
+            segs->push_back({(u32)b, 0, len, SEG_FIRST | SEG_LAST});
+            continue;
+        }
+        const u32 n = (u32)((len + segLen - 1) / segLen);
+        cuts->push_back(make_uint2((u32)segs->size(), n));
+        for (u32 i = 0; i < n; i++) {
+            const u32 start = (u32)(i * segLen);
+            segs->push_back({(u32)b, start, (u32)std::min<u64>(segLen, len - start),
+                             (i == 0 ? (u32)SEG_FIRST : 0u) | (i == n - 1 ? (u32)SEG_LAST : 0u)});
+        }
+    }
+    return true;
+}
+
 /* Run an engine (dp from engineParams, dp.nfa its bytes in device memory), or a fused launch of several
- * (dp.engines), over every block of corpus c, into the record ring out[0, outCap) and its counters. */
+ * (dp.engines), over every block of corpus c, into the record ring out[0, outCap) and its counters.  Long
+ * blocks are cut into segments walked by lanes of their own (planSegments); `seg` holds their plan and states. */
 cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u32 outCap,
-                         u32 *counters, int smCount, int maxSmem, cudaStream_t stream) {
+                         u32 *counters, int smCount, int maxSmem, SegArea *seg, cudaStream_t stream) {
     dp.corpus = c->d_data;
     dp.readableEnd = c->readableEnd;
     dp.blockOff = c->d_off;
@@ -1101,9 +1179,89 @@ cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u
     dp.out = out;
     dp.outCap = outCap;
     dp.counters = counters;
-    const cudaError_t e = launchDfa(dp, smCount, maxSmem, stream);
+    initOpts();
+    std::vector<DfaSeg> segs;
+    std::vector<uint2> cuts;
+    if (!planSegments(c, dp.kind, smCount, &segs, &cuts)) {
+        const cudaError_t e = launchDfa(dp, smCount, maxSmem, stream);
+        if (e == cudaSuccess) {
+            g_launches++;
+        }
+        return e;
+    }
+    /* [segs][cuts][per engine, per block: first open segment][per engine: guess states, end states] */
+    const size_t engines = dp.engines ? dp.nengines : 1;
+    const size_t segBytes = HSB_ROUNDUP(segs.size() * sizeof(DfaSeg), 256);
+    const size_t planBytes = segBytes + cuts.size() * sizeof(uint2);
+    const size_t openBytes = HSB_ROUNDUP(engines * c->nblocks * sizeof(u32), 256);
+    const size_t statesAt = HSB_ROUNDUP(planBytes, 256) + openBytes;
+    const size_t need = statesAt + engines * 2 * segs.size() * dfaStateBytes(dp.kind);
+    if (!seg->d_stats) {
+        cudaError_t e = cudaMalloc(&seg->d_stats, SEGSTAT_COUNT * sizeof(unsigned long long));
+        if (e == cudaSuccess) e = cudaMemset(seg->d_stats, 0, SEGSTAT_COUNT * sizeof(unsigned long long));
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&seg->copied, cudaEventDisableTiming);
+        if (e != cudaSuccess) {
+            return e;
+        }
+    }
+    if (need > seg->bytes) {
+        cudaFree(seg->d); /* (synchronises with any run still using it) */
+        seg->d = nullptr;
+        seg->bytes = 0;
+        seg->plan.clear();
+        const cudaError_t e = cudaMalloc(&seg->d, need + need / 4);
+        if (e != cudaSuccess) {
+            return e;
+        }
+        seg->bytes = need + need / 4;
+    }
+    /* the plan's image; copied only when it differs from the one in device memory (a scan of the same corpus
+     * again, or the next engine kind of the same scan, reuses it) */
+    std::vector<u8> image(planBytes, 0);
+    memcpy(image.data(), segs.data(), segs.size() * sizeof(DfaSeg));
+    memcpy(image.data() + segBytes, cuts.data(), cuts.size() * sizeof(uint2));
+    cudaError_t e = cudaSuccess;
+    if (image != seg->plan) {
+        e = cudaEventSynchronize(seg->copied); /* the last copy out of the pinned buffer has been made */
+        if (e == cudaSuccess && planBytes > seg->hBytes) {
+            cudaFreeHost(seg->h);
+            seg->h = nullptr;
+            seg->hBytes = 0;
+            e = cudaMallocHost(&seg->h, planBytes + planBytes / 4);
+            if (e == cudaSuccess) {
+                seg->hBytes = planBytes + planBytes / 4;
+            }
+        }
+        if (e == cudaSuccess) {
+            memcpy(seg->h, image.data(), planBytes);
+            e = cudaMemcpyAsync(seg->d, seg->h, planBytes, cudaMemcpyHostToDevice, stream);
+        }
+        if (e == cudaSuccess) e = cudaEventRecord(seg->copied, stream);
+        if (e != cudaSuccess) {
+            seg->plan.clear();
+            return e;
+        }
+        seg->plan.swap(image);
+    }
+    u32 *open = reinterpret_cast<u32 *>(seg->d + HSB_ROUNDUP(planBytes, 256));
+    e = cudaMemsetAsync(open, 0xff, engines * c->nblocks * sizeof(u32), stream);
+    if (e != cudaSuccess) {
+        return e;
+    }
+    dp.segs = reinterpret_cast<const DfaSeg *>(seg->d);
+    dp.nsegs = (u32)segs.size();
+    dp.cuts = reinterpret_cast<const uint2 *>(seg->d + segBytes);
+    dp.ncuts = (u32)cuts.size();
+    dp.warm = SEG_WARM;
+    dp.segOpen = open;
+    dp.segStates = seg->d + statesAt;
+    dp.segStats = seg->d_stats;
+    unsigned launches = 0;
+    e = launchDfaSegments(dp, smCount, maxSmem, SEG_ROUNDS, stream, &launches);
+    g_launches += launches;
     if (e == cudaSuccess) {
-        g_launches++;
+        seg->runs++;
+        seg->segments += segs.size();
     }
     return e;
 }
@@ -1139,7 +1297,14 @@ hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
         const u32 ntiles = (u32)((c->bytes + pl.tileBytes - 1) / pl.tileBytes);
         if (t1 >= ntiles) {
             for (const DfaParams &dp : im->engineRuns) {
-                CUDA_TRY(launchEngine(dp, c, s->d_out, s->outCap, s->d_counters, s->smCount, s->maxSmem, stream));
+                if (!s->seg) {
+                    s->seg = new (std::nothrow) SegArea();
+                    if (!s->seg) {
+                        return HS_NOMEM;
+                    }
+                }
+                CUDA_TRY(launchEngine(dp, c, s->d_out, s->outCap, s->d_counters, s->smCount, s->maxSmem, s->seg,
+                                      stream));
             }
         }
     }
@@ -1377,6 +1542,28 @@ hs_error_t hs_b200_last_counters(const hs_scratch_t *scratch, unsigned int out[8
     return HS_SUCCESS;
 }
 
+hs_error_t hs_b200_engine_segment_stats(const hs_scratch_t *scratch, unsigned long long out[4]) {
+    if (!validScratch(scratch) || !out) {
+        return HS_INVALID;
+    }
+    memset(out, 0, 4 * sizeof(unsigned long long));
+    const SegArea *a = scratch->seg;
+    if (!a) {
+        return HS_SUCCESS;
+    }
+    out[0] = a->runs;
+    out[1] = a->segments;
+    if (a->d_stats) {
+        DeviceGuard guard(scratch->device);
+        if (cudaStreamSynchronize(scratch->stream) != cudaSuccess ||
+            cudaMemcpy(out + 2, a->d_stats, SEGSTAT_COUNT * sizeof(unsigned long long), cudaMemcpyDeviceToHost) !=
+                cudaSuccess) {
+            return HS_UNKNOWN_ERROR;
+        }
+    }
+    return HS_SUCCESS;
+}
+
 hs_error_t hs_b200_set_runtime_option(const char *key, int value) {
     initOpts();
     if (!key) {
@@ -1386,7 +1573,8 @@ hs_error_t hs_b200_set_runtime_option(const char *key, int value) {
         {"warps", &g_opts.warps},       {"tile_bytes", &g_opts.tileBytes},
         {"pf_dist", &g_opts.pfDist},    {"chunk_mb", &g_opts.chunkMB},
         {"initial_ring", &g_opts.initialRing}, {"heavy", &g_opts.heavy},
-        {"gram", &g_opts.gram},         {"dfa_ilp", &g_opts.dfaIlp}};
+        {"gram", &g_opts.gram},         {"dfa_ilp", &g_opts.dfaIlp},
+        {"engine_segment", &g_opts.engineSegment}};
     for (auto &x : k) {
         if (!strcmp(key, x.n)) {
             *x.v = value;
@@ -1592,6 +1780,7 @@ hs_error_t hs_free_scratch(hs_scratch_t *s) {
     freeCorpus(s->inlineCorpus);
     cudaFree(s->d_out);
     cudaFree(s->d_order);
+    delete s->seg;
     cudaFree(s->d_counters);
     if (s->h_counters) cudaFreeHost(s->h_counters);
     if (s->h_stage) cudaFreeHost(s->h_stage);
@@ -2174,6 +2363,7 @@ hs_error_t hs_b200_nfa_scan_corpus(const void *nfa, size_t nfa_len, const hs_b20
     u32 *d_ctr = nullptr;
     DevMatch *d_out = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    SegArea seg;
     hs_error_t rv = HS_SUCCESS;
     u32 capDev = (u32)std::min<size_t>(std::max<size_t>(cap, 1u << 16), 0xfffffff0u);
     std::vector<DevMatch> host;
@@ -2188,7 +2378,7 @@ hs_error_t hs_b200_nfa_scan_corpus(const void *nfa, size_t nfa_len, const hs_b20
         if (e != cudaSuccess) break;
         e = cudaMemset(d_ctr, 0, CTR_COUNT * sizeof(u32));
         if (e == cudaSuccess) e = cudaEventRecord(ev0, 0);
-        if (e == cudaSuccess) e = launchEngine(p, corpus, d_out, capDev, d_ctr, smCount, maxSmem, 0);
+        if (e == cudaSuccess) e = launchEngine(p, corpus, d_out, capDev, d_ctr, smCount, maxSmem, &seg, 0);
         if (e == cudaSuccess) e = cudaEventRecord(ev1, 0);
         u32 ctr[CTR_COUNT] = {0};
         if (e == cudaSuccess) e = cudaMemcpy(ctr, d_ctr, sizeof(ctr), cudaMemcpyDeviceToHost);

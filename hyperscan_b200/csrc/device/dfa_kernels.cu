@@ -81,6 +81,7 @@ template <class ST> struct StOps {
     static __device__ __forceinline__ ST zero() { return 0; }
     static __device__ __forceinline__ ST ones() { return ~(ST)0; }
     static __device__ __forceinline__ bool any(ST a) { return a != 0; }
+    static __device__ __forceinline__ bool eq(ST a, ST b) { return a == b; }
     static __device__ __forceinline__ ST band(ST a, ST b) { return a & b; }
     static __device__ __forceinline__ ST bor(ST a, ST b) { return a | b; }
     static __device__ __forceinline__ bool test(ST a, u32 i) { return (a >> i) & 1; }
@@ -117,6 +118,12 @@ template <int W> struct StOps<WideSt<W>> {
 #pragma unroll
         for (int j = 0; j < W; j++) x |= a.w[j];
         return x != 0;
+    }
+    static __device__ __forceinline__ bool eq(const ST &a, const ST &b) {
+        u64 x = 0;
+#pragma unroll
+        for (int j = 0; j < W; j++) x |= a.w[j] ^ b.w[j];
+        return x == 0;
     }
     static __device__ __forceinline__ ST band(const ST &a, const ST &b) {
         ST r;
@@ -290,6 +297,29 @@ __device__ __forceinline__ uint4 load16(const DfaParams &p, const u8 *q) {
     return load16Tail(q, p.corpus + p.readableEnd);
 }
 
+/* 16 corpus bytes at any q inside a block (segments start anywhere): two aligned loads, shifted together */
+__device__ __forceinline__ uint4 load16At(const DfaParams &p, const u8 *q) {
+    const u32 sh = (u32)((uintptr_t)q & 15);
+    if (sh == 0) {
+        return load16(p, q);
+    }
+    const uint4 a = load16(p, q - sh), b = load16(p, q - sh + 16); /* (a block starts 16-byte aligned) */
+    const u32 x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    const u32 first = sh >> 2, sel = 0x3210 + 0x1111 * (sh & 3);
+    u32 o[4];
+#pragma unroll
+    for (u32 i = 0; i < 4; i++) {
+        u32 lo = x[i], hi = x[i + 1];
+#pragma unroll
+        for (u32 d = 1; d < 4; d++) { /* x[first + i], x[first + i + 1] without a dynamically indexed array */
+            lo = first == d ? x[i + d] : lo;
+            hi = first == d ? x[i + d + 1] : hi;
+        }
+        o[i] = __byte_perm(lo, hi, sel);
+    }
+    return make_uint4(o[0], o[1], o[2], o[3]);
+}
+
 __device__ __forceinline__ BlockSpan blockSpan(const DfaParams &p, u32 b) {
     BlockSpan s;
     if (p.uniformPitch && p.uniformLen) {
@@ -398,7 +428,8 @@ __device__ HSB_NOINLINE u32 emitAccept(const DfaParams &p, const u8 *nfa, u32 cu
     return emitReportList(p, nfa, cursor, g32(nfa + what), block, to);
 }
 
-template <int ENGINE, int SMEM_TABLE, int CH, int ILP, bool FUSED>
+/* SEG: the segment mode (p.segs, p.segMode; DESIGN.md section 10f), fused or not */
+template <int ENGINE, int SMEM_TABLE, int CH, int ILP, bool FUSED, bool SEG = false>
 __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(const HSB_GRID_CONSTANT DfaParams p) {
     HSB_DYNAMIC_SMEM(smem);
     typedef DfaTile<CH> Tile;
@@ -407,10 +438,10 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
      * `ctas` CTAs per engine), read once per CTA */
     const u8 *nfa = p.nfa;
     u32 tableBytes = p.tableBytes, squashes = p.squashes;
-    u32 cta = blockIdx.x, ctas = gridDim.x;
-    if constexpr (FUSED) {
+    u32 cta = blockIdx.x, ctas = gridDim.x, which = 0;
+    if (FUSED || (SEG && p.engines != nullptr)) {
         ctas = gridDim.x / p.nengines;
-        const u32 which = blockIdx.x / ctas;
+        which = blockIdx.x / ctas;
         cta = blockIdx.x - which * ctas;
         const DfaEngine *e = p.engines + which;
         nfa = e->nfa;
@@ -462,6 +493,17 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
         k.acceptLimit8 = g16(eng + offsetof(McClellan, accept_limit_8));
         k.auxSize = (u32)sizeof(MStateAux);
         k.stateMask = 0xffffffffu;
+    }
+    /* the state a walk from a later offset starts in: where a segment's guess begins its warm-up */
+    ST segFloat = Ops::zero();
+    if constexpr (SEG) {
+        if constexpr (LIMEX) {
+            segFloat = Ops::load(eng + offsetof(LxNfa, initDS));
+        } else if constexpr (ENGINE == ENG_SHENG) {
+            segFloat = __ldg(eng + offsetof(Sheng, floating));
+        } else {
+            segFloat = g16(eng + offsetof(McClellan, start_floating));
+        }
     }
     u32 tabArea;
     if (LIMEX) {
@@ -578,6 +620,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
         lxShiftAmounts = (u64)g32(eng + offsetof(LxNfa, shiftAmount)) | ((u64)g32(eng + offsetof(LxNfa, shiftAmount) + 4) << 32);
     }
     u32 cursor = 0; /* this lane's next record slot (emitDfaMatch) */
+    const bool segEmit = !SEG || p.segMode == SEG_EMIT; /* the segment passes before SEG_EMIT write no records */
     /* one input byte: byte j of data word w, at block offset pos.  DFAs: returns true when the
      * state entered accepts.  LimEx (LOOP_NOACCEL_FN, limex_runtime_impl.h:209-243): the states
      * that are on BEFORE the byte run their exceptions -- reports at offset pos, except at the
@@ -600,7 +643,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
             }
             Ops::forEach(Ops::band(s, tShift[8]), [&](const u32 bit) {
                 const u32 rep = reinterpret_cast<const u32 *>(smem + T::REP)[bit];
-                if (rep != MO_INVALID_IDX && pos != 0) {
+                if (rep != MO_INVALID_IDX && pos != 0 && segEmit) {
                     cursor = emitLimexReports(p, nfa, cursor, rep, blk, pos);
                 }
                 local = Ops::bor(local, Ops::loadChunks(reinterpret_cast<const uint4 *>(smem + T::LOCAL), T::STATES, bit));
@@ -627,7 +670,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
             Ops::forEach(on, [&](const u32 bit) {
                 const ST *e = lxRows + 4 * bit;
                 const u32 rep = Ops::low32(e[3]);
-                if (rep != MO_INVALID_IDX && pos != 0) {
+                if (rep != MO_INVALID_IDX && pos != 0 && segEmit) {
                     cursor = emitLimexReports(p, nfa, cursor, rep, blk, pos);
                 }
                 lim = Ops::bor(lim, e[0]);
@@ -662,6 +705,265 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
     auto dead = [&](const ST &s) -> bool {
         return ENGINE == ENG_SHENG ? (Ops::low32(s) & SHENG_STATE_DEAD) != 0 : !Ops::any(s);
     };
+    /* reports of a block's last state that fire at end of data (nfaExec*_B), the block `len` bytes long */
+    auto blockEnd = [&](const ST &s, const u32 blk, const u32 len) {
+        if constexpr (LIMEX) {
+            /* STREAM_FN's closing accept check (only if the block had bytes to stream),
+             * then nfaExecLimEx*_testEOD (limex_common_impl.h:192-218) */
+            if (len && Ops::any(Ops::band(s, lxAccept))) {
+                cursor = emitLimexAccepts<ST>(p, nfa, cursor, Ops::band(s, lxAccept), lxAccept,
+                                              g32(eng + offsetof(LxNfa, acceptOffset)), blk, len);
+            }
+            if (Ops::any(Ops::band(s, lxAcceptEod))) {
+                cursor = emitLimexAccepts<ST>(p, nfa, cursor, Ops::band(s, lxAcceptEod), lxAcceptEod,
+                                              g32(eng + offsetof(LxNfa, acceptEodOffset)), blk, len);
+            }
+        } else {
+            const u32 eodOff = ENGINE == ENG_SHENG ? (u32)offsetof(SstateAux, accept_eod)
+                                                   : (u32)offsetof(MStateAux, accept_eod);
+            const u32 eod = g32(nfa + k.auxOffset + k.auxSize * (Ops::low32(s) & k.stateMask) + eodOff);
+            if (eod) {
+                cursor = emitReportList(p, nfa, cursor, eod, blk, len);
+            }
+        }
+    };
+
+    if constexpr (SEG) {
+        /* Segment mode.  A lane's unit is segment p.segs[unit] (SEG_SETTLE: cut block p.cuts[unit] and its chain
+         * of segments); every walk is bytes [from, to) of one block, through the warp's tile as above, from state
+         * s -- and, in the re-walks, from the guess `alt` beside it, until the two states agree: from there on
+         * both walks are the same walk. */
+        static_assert(ILP == 1, "a lane walks one chain in segment mode");
+        ST *const guess = reinterpret_cast<ST *>(p.segStates) + (size_t)which * 2 * p.nsegs;
+        ST *const ends = guess + p.nsegs;
+        const ST init = LIMEX ? lxStart : Ops::fromU32(k.start);
+        const u32 mode = p.segMode;
+        if (mode == SEG_CHECK) {
+            /* the first segment of each block whose guess is not the end of the segment before */
+            for (u32 j = (cta * nwarps + warp) * 32 + lane; j < p.nsegs; j += ctas * nwarps * 32) {
+                const DfaSeg sg = p.segs[j];
+                if (!(sg.flags & SEG_FIRST) && !Ops::eq(ends[j - 1], guess[j])) {
+                    atomicMin(p.segOpen + (size_t)which * p.nblocks + sg.block, j);
+                }
+            }
+            return;
+        }
+        const u32 units = mode == SEG_SETTLE ? p.ncuts : p.nsegs;
+        unsigned long long rewalks = 0, rebytes = 0;
+        for (u32 g = cta * nwarps + warp; g < (units + 31) / 32; g += ctas * nwarps) {
+            const u32 unit = g * 32 + lane;
+            bool more = unit < units; /* this lane has walks left */
+            u32 phase = 0;            /* SEG_SPECULATE: 0 = the warm-up, 1 = the segment */
+            u32 j = unit, jEnd = 0;   /* SEG_SETTLE: the next segment of the chain, and the chain's end */
+            ST s = init, alt = init, t = init; /* t: SEG_JOIN / SEG_SETTLE, the true start of segment j */
+            if (mode == SEG_SETTLE && more) {
+                /* every segment before the first open one starts where the one before it ended, back to the first
+                 * segment, which was walked from the initial state: those starts are true */
+                const uint2 cut = p.cuts[unit];
+                const u32 open = p.segOpen[(size_t)which * p.nblocks + p.segs[cut.x].block];
+                jEnd = cut.x + cut.y;
+                j = min(open, jEnd);
+                more = j < jEnd;
+                if (more) {
+                    t = ends[j - 1];
+                }
+            }
+            for (;;) {
+                /* this lane's next walk */
+                DfaSeg sg = {0, 0, 0, 0};
+                u32 from = 0, to = 0;
+                bool cmp = false, walks = false;
+                if (mode == SEG_SETTLE) {
+                    for (; j < jEnd; j++) { /* segments whose guess was right: their end state is known */
+                        alt = guess[j];
+                        if (!Ops::eq(t, alt)) {
+                            break;
+                        }
+                        t = ends[j];
+                    }
+                    more = j < jEnd;
+                    if (more) {
+                        sg = p.segs[j];
+                        s = t;
+                        cmp = true;
+                    }
+                } else if (more) {
+                    sg = p.segs[unit];
+                    const bool first = (sg.flags & SEG_FIRST) != 0, cut = !first || !(sg.flags & SEG_LAST);
+                    if (mode == SEG_SPECULATE) {
+                        more = cut;
+                        if (phase == 0 && first) {
+                            phase = 1; /* the initial state is no guess */
+                        }
+                        if (phase == 0) {
+                            s = segFloat;
+                            from = sg.start - min(p.warm, sg.start);
+                            to = sg.start;
+                        }
+                    } else if (mode == SEG_JOIN) {
+                        if (first) {
+                            more = false;
+                        } else {
+                            t = ends[unit - 1]; /* (this round's or the last: any state is a guess) */
+                            alt = guess[unit];
+                            s = t;
+                            more = !Ops::eq(t, alt);
+                            cmp = true;
+                        }
+                    } else {
+                        s = first ? init : guess[unit];
+                    }
+                }
+                if (more && !(mode == SEG_SPECULATE && phase == 0)) {
+                    from = sg.start;
+                    to = sg.start + sg.len;
+                }
+                if (!__any_sync(0xffffffffu, more)) {
+                    break;
+                }
+                walks = more;
+                const u64 off = walks ? (u64)(blockSpan(p, sg.block).base - p.corpus) + from : 0;
+                const u32 n = walks ? to - from : 0;
+                bool met = false, live = n != 0 && !dead(s);
+                u32 walked = 0; /* bytes of a re-walk, up to the 16-byte piece where the two walks met */
+                for (u32 r = 0;; r++) {
+                    const u32 done = r * CH;
+                    const bool want = live && done < n;
+                    if (!__any_sync(0xffffffffu, want)) {
+                        break;
+                    }
+                    uint4 v[Tile::PIECES];
+#pragma unroll
+                    for (u32 i = 0; i < Tile::PIECES; i++) {
+                        const u32 src = i * Tile::ROWS_PER_LOAD + lane / Tile::PIECES; /* owning lane */
+                        const u32 rOffLo = __shfl_sync(0xffffffffu, (u32)off, src);
+                        const u32 rOffHi = __shfl_sync(0xffffffffu, (u32)(off >> 32), src);
+                        const u32 rLen = __shfl_sync(0xffffffffu, want ? n : 0u, src);
+                        const u32 pos = done + (lane % Tile::PIECES) * 16;
+                        v[i] = make_uint4(0, 0, 0, 0);
+                        if (pos < rLen) {
+                            v[i] = load16At(p, p.corpus + (((u64)rOffHi << 32) | rOffLo) + pos);
+                        }
+                    }
+#pragma unroll
+                    for (u32 i = 0; i < Tile::PIECES; i++) {
+                        const u32 src = i * Tile::ROWS_PER_LOAD + lane / Tile::PIECES;
+                        *reinterpret_cast<uint4 *>(tile + src * Tile::ROW + (lane % Tile::PIECES) * 16) = v[i];
+                    }
+                    __syncwarp();
+                    const u32 m = want ? min(n - done, (u32)CH) : 0u;
+                    const u32 at = from + done; /* block offset of the tile row's first byte */
+                    if (WIDE) {
+                        /* one byte at a time: the wide models' steps (see above) */
+#pragma unroll 1
+                        for (u32 c = 0; c < m && live; c++) {
+                            const u32 x = myRow[c];
+                            walked++;
+                            if (step(x, 0, s, at + c, sg.block) && segEmit) {
+                                cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s), sg.block, (u64)at + c + 1);
+                            }
+                            if (cmp) {
+                                (void)step(x, 0, alt, at + c, sg.block);
+                                met = Ops::eq(s, alt);
+                            }
+                            live = !met && !dead(s);
+                        }
+                    } else if (cmp) {
+                        /* the re-walks (which write no records): the two chains interleaved in one instruction
+                         * stream, 16 bytes at a time, compared after each piece */
+#pragma unroll 1
+                        for (u32 cc = 0; live && cc * 16 < m; cc++) {
+                            const uint4 x = *reinterpret_cast<const uint4 *>(myRow + cc * 16);
+                            const u32 w[4] = {x.x, x.y, x.z, x.w};
+                            const u32 e = min(m - cc * 16, 16u);
+                            if (e == 16) {
+#pragma unroll
+                                for (u32 jj = 0; jj < 16; jj++) {
+                                    (void)step(w[jj >> 2], jj & 3, s, at + cc * 16 + jj, sg.block);
+                                    (void)step(w[jj >> 2], jj & 3, alt, at + cc * 16 + jj, sg.block);
+                                }
+                            } else {
+#pragma unroll 1
+                                for (u32 jj = 0; jj < e; jj++) {
+                                    (void)step(w[jj >> 2] >> (8 * (jj & 3)), 0, s, at + cc * 16 + jj, sg.block);
+                                    (void)step(w[jj >> 2] >> (8 * (jj & 3)), 0, alt, at + cc * 16 + jj, sg.block);
+                                }
+                            }
+                            walked += e;
+                            met = Ops::eq(s, alt);
+                            live = !met && !dead(s);
+                        }
+                    } else {
+                        u32 cc = 0;
+#pragma unroll 1
+                        for (; live && cc * 16 + 16 <= m; cc++) { /* full pieces: no per-byte checks */
+                            const uint4 x = *reinterpret_cast<const uint4 *>(myRow + cc * 16);
+                            const u32 w[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+                            for (u32 jj = 0; jj < 16; jj++) {
+                                if (step(w[jj >> 2], jj & 3, s, at + cc * 16 + jj, sg.block) && segEmit) {
+                                    cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s), sg.block,
+                                                        (u64)at + cc * 16 + jj + 1);
+                                }
+                            }
+                            live = !dead(s);
+                        }
+                        if (live && cc * 16 < m) { /* the walk's last, partial piece */
+                            const uint4 x = *reinterpret_cast<const uint4 *>(myRow + cc * 16);
+                            const u32 w[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll 1
+                            for (u32 jj = 0; jj < m - cc * 16; jj++) {
+                                if (step(w[jj >> 2] >> (8 * (jj & 3)), 0, s, at + cc * 16 + jj, sg.block) && segEmit) {
+                                    cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s), sg.block,
+                                                        (u64)at + cc * 16 + jj + 1);
+                                }
+                            }
+                            live = !dead(s);
+                        }
+                    }
+                    __syncwarp();
+                }
+                if (!walks) {
+                    continue;
+                }
+                /* what the walk found */
+                if (mode == SEG_SPECULATE) {
+                    if (phase == 0) {
+                        guess[unit] = s;
+                        phase = 1;
+                    } else {
+                        ends[unit] = s;
+                        more = false;
+                    }
+                } else if (mode == SEG_JOIN || mode == SEG_SETTLE) {
+                    const u32 at = mode == SEG_JOIN ? unit : j;
+                    guess[at] = t;
+                    if (!met) { /* (met: from where the walks met, the end state is the guess's) */
+                        ends[at] = s;
+                    }
+                    rewalks++;
+                    rebytes += walked;
+                    if (mode == SEG_SETTLE) {
+                        t = ends[at];
+                        j++;
+                    } else {
+                        more = false;
+                    }
+                } else {
+                    if (sg.flags & SEG_LAST) {
+                        blockEnd(s, sg.block, sg.start + sg.len);
+                    }
+                    more = false;
+                }
+            }
+        }
+        if (rewalks) {
+            atomicAdd(p.segStats + SEGSTAT_WALKS, rewalks);
+            atomicAdd(p.segStats + SEGSTAT_BYTES, rebytes);
+        }
+        padReserved(p, cursor);
+        return;
+    }
 
     /* a warp takes 32 * ILP consecutive blocks at a time; lane t owns blocks t, t + 32, ...
      * of the group: ILP independent state chains in one instruction stream */
@@ -840,15 +1142,17 @@ cudaError_t launchStaged(const DfaParams &p, int smCount, size_t tableBytes, cud
      * ilp 2: two blocks per lane, 64 bytes of each per refill (160 KiB of tiles);
      * ilp 1: one block per lane, 128 bytes per refill (144 KiB) */
     const int threads = StagedThreads<ENGINE>::N;
-    /* (the wide models, and a fused launch, walk one block per lane) */
-    const bool fused = p.engines != nullptr;
-    const bool two = !fused && p.ilp == 2 && ENGINE < ENG_LIMEX128;
+    /* (the wide models, a fused launch and a segmented one walk one block or segment per lane) */
+    const bool fused = p.engines != nullptr, seg = p.segs != nullptr;
+    const bool two = !fused && !seg && p.ilp == 2 && ENGINE < ENG_LIMEX128;
     const size_t tiles = (size_t)(threads / 32) * (two ? 2 * DfaTile<64>::WARP_BYTES : DfaTile<128>::WARP_BYTES);
-    const u64 groups = ((u64)p.nblocks + (two ? 63 : 31)) / (two ? 64 : 32);
+    const u64 units = !seg ? p.nblocks : p.segMode == SEG_SETTLE ? p.ncuts : p.nsegs;
+    const u64 groups = (units + (two ? 63 : 31)) / (two ? 64 : 32);
     /* per engine: `grid` CTAs over all blocks (a fused launch has that many per engine, and the CTAs of every
      * engine share the GPU: a corpus too small to fill it for one engine fills it for several) */
     const int grid = (int)std::min<u64>((u64)smCount, (groups + threads / 32 - 1) / (threads / 32));
-    void (*kern)(const DfaParams) = fused ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, true>
+    void (*kern)(const DfaParams) = seg     ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, true>
+                                    : fused ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, true>
                                     : two ? dfaStagedKernel<ENGINE, SMEM_TABLE, 64, 2, false>
                                           : dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false>;
     const size_t smem = tableBytes + tiles;
@@ -883,7 +1187,7 @@ cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t
     if (!p.nblocks) {
         return cudaSuccess;
     }
-    if (p.toTag) {
+    if (p.toTag && (!p.segs || p.segMode == SEG_EMIT)) { /* (the passes before SEG_EMIT write no records) */
         HSB_LAUNCH(alignSharedRing, 1, 1, 0, stream, p);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) {
@@ -919,6 +1223,39 @@ cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t
                       : launchStaged<ENG_MCC16, 0>(p, smCount, 256, stream);
     }
     return cudaErrorInvalidValue;
+}
+
+u32 dfaResidentLanes(u32 kind, int smCount) {
+    /* one CTA per SM (launchStaged) */
+    const u32 threads = kind == NFA_LIMEX_256 || kind == NFA_LIMEX_512 ? StagedThreads<ENG_LIMEX256>::N
+                                                                       : StagedThreads<ENG_MCC8>::N;
+    return (u32)smCount * threads;
+}
+
+u32 dfaStateBytes(u32 kind) {
+    switch (kind) {
+    case NFA_LIMEX_64: return 8;
+    case NFA_LIMEX_128: return 16;
+    case NFA_LIMEX_256: return 32;
+    case NFA_LIMEX_512: return 64;
+    default: return 4; /* a DFA state id, the 32-state LimEx set */
+    }
+}
+
+cudaError_t launchDfaSegments(const DfaParams &p, int smCount, int maxSmem, u32 rounds, cudaStream_t stream,
+                              unsigned *launches) {
+    DfaParams q = p;
+    *launches = 0;
+    for (u32 i = 0; i < rounds + 4; i++) {
+        q.segMode = i == 0 ? SEG_SPECULATE : i <= rounds ? SEG_JOIN : i == rounds + 1 ? SEG_CHECK
+                  : i == rounds + 2 ? SEG_SETTLE : SEG_EMIT;
+        const cudaError_t e = launchDfa(q, smCount, maxSmem, stream);
+        if (e != cudaSuccess) {
+            return e;
+        }
+        ++*launches;
+    }
+    return cudaSuccess;
 }
 
 } // namespace hsb

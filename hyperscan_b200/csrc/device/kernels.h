@@ -171,6 +171,23 @@ struct DfaEngine {
     u32 pad;
 };
 
+/* A piece of a block walked by one lane (DfaParams.segs): bytes [start, start + len) of block `block`.
+ * A block that is not cut is one segment with both flags. */
+struct DfaSeg {
+    u32 block, start, len, flags;
+};
+enum { SEG_FIRST = 1, SEG_LAST = 2 };
+/* the passes of a segmented engine run (DfaParams.segMode; DESIGN.md section 10f) */
+enum { SEG_SPECULATE = 1, /* every segment j > 0 of a cut block: guess[j] from a warm-up walk, end[j] from guess[j] */
+       SEG_JOIN = 2,      /* (a round) segment j re-walks from end[j - 1] where that is not guess[j] */
+       SEG_CHECK = 5,     /* segment j where end[j - 1] is not guess[j]: the lowest such j per block into segOpen */
+       SEG_SETTLE = 3,    /* one lane per cut block chains its segments from segOpen on: guess[j] becomes the true
+                           * start */
+       SEG_EMIT = 4 };    /* every segment walks from its true start and writes its records */
+/* DfaParams.segStats: segments re-walked by SEG_JOIN / SEG_SETTLE, and the bytes walked again (up to where the
+ * re-walk met the guess's walk) */
+enum { SEGSTAT_WALKS = 0, SEGSTAT_BYTES = 1, SEGSTAT_COUNT = 2 };
+
 /* DFA engines in block mode (dfa_kernels.cu): McClellan 8 / 16, Sheng -- the engine's
  * own bytes (struct NFA first) in device memory, one thread per block. */
 struct DfaParams {
@@ -196,8 +213,30 @@ struct DfaParams {
      * fields above.  tableBytes and states then hold the largest engine's, which size the shared memory. */
     const DfaEngine *engines;
     u32 nengines;
+    /* != null: a segmented run (launchDfaSegments sets the fields below): a lane's unit is segs[i] (the
+     * cut blocks cuts[i] = {first segment, segments} in SEG_SETTLE), walked as pass segMode.  segStates holds
+     * per engine of the launch guess[nsegs] then end[nsegs], states of the engine kind's size. */
+    const DfaSeg *segs;
+    u32 nsegs;
+    u32 segMode;
+    const uint2 *cuts;
+    u32 ncuts;
+    u32 warm;        /* bytes of the warm-up walk in front of a segment (SEG_SPECULATE) */
+    u8 *segStates;
+    unsigned long long *segStats; /* SEGSTAT_COUNT counters, accumulated */
+    u32 *segOpen;    /* per engine of the launch, per block: the first segment whose start is not settled (SEG_CHECK;
+                      * all ones = none), cleared by the caller */
 };
 cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t stream);
+
+/* The segment plan of an engine run: lanes an engine launch keeps resident, and the bytes of one
+ * segment's two states (guess, end) per engine. */
+u32 dfaResidentLanes(u32 kind, int smCount);
+u32 dfaStateBytes(u32 kind);
+/* The segmented walk of p (p.segs ... set, segMode ignored): SEG_SPECULATE, `rounds` SEG_JOIN rounds,
+ * SEG_CHECK, SEG_SETTLE, SEG_EMIT; *launches receives the kernels launched. */
+cudaError_t launchDfaSegments(const DfaParams &p, int smCount, int maxSmem, u32 rounds, cudaStream_t stream,
+                              unsigned *launches);
 
 /* ---- the report rules on the device (order_kernels.h): raw records -> delivered matches ---- */
 

@@ -607,11 +607,23 @@ hs_error_t hs_b200_test_compile_programs(const char *const *lits, const size_t *
  * the library makes from the database: "gram" (class 4-gram first stage for FDR sets:
  * 0 never, 1 from 10 000 prefilter keys, 2 whenever all literals have 4 bytes),
  * "heavy" (class-pair candidate path: per-word queue entries 0 never / 1 and 2
- * always) and "dfa_ilp" (DFA kernels: blocks per lane, 1).  "gram" applies to
- * scratches allocated afterwards.  The defaults are the measured best (DESIGN.md
- * section 3); the others exist for A/B runs (tools/sweep.py) and tests.  Any other
- * key: HS_INVALID. */
+ * always), "dfa_ilp" (DFA kernels: blocks per lane, 1) and "engine_segment"
+ * (engine runs of regular-expression databases and hs_b200_nfa_scan_corpus: 0 = cut
+ * blocks longer than twice the segment length into segments walked by lanes of their
+ * own when the blocks alone leave more than half of the resident lanes idle; N > 0 =
+ * cut every block longer than N bytes into N-byte segments; -1 = never cut, one lane
+ * per block.  The matches are the same in every setting; DESIGN.md section 10f).
+ * "gram" applies to scratches allocated afterwards.  The defaults are the measured
+ * best (DESIGN.md section 3); the others exist for A/B runs (tools/sweep.py) and tests.
+ * Any other key: HS_INVALID. */
 hs_error_t hs_b200_set_runtime_option(const char *key, int value);
+
+/* What the segmented engine runs on this scratch have done since it was allocated:
+ * out[0] engine runs that cut blocks, out[1] segments they walked, out[2] segments
+ * re-walked because the start state guessed for them was wrong, out[3] bytes of those
+ * re-walks, each counted up to the 16-byte piece where it met the walk from the guess.
+ * Waits for the scratch's stream. */
+hs_error_t hs_b200_engine_segment_stats(const hs_scratch_t *scratch, unsigned long long out[4]);
 
 /* Counters of the last finished scan: [0] raw records, [1] error, [2]
  * first-stage candidates, [3] byte-confirmed literals, [4] candidates that
