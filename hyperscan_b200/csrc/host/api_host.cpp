@@ -498,6 +498,13 @@ public:
         if (pos != n) {
             fail("Unmatched parentheses.");
         }
+        if (utf8Mode() && (flags & HS_FLAG_CASELESS)) {
+            for (const std::string &s : out) {
+                if (s.find_first_of("kKsS") != std::string::npos) {
+                    needsRegex("Caseless \"k\" or \"s\" under HS_FLAG_UTF8 (they also match U+212A and U+017F)");
+                }
+            }
+        }
         return std::vector<std::string>(out.begin(), out.end());
     }
 
@@ -516,6 +523,8 @@ private:
                     "finite set of literals only.");
     }
     bool at(char c) const { return pos < n && re[pos] == c; }
+    /* HS_FLAG_UTF8 without HS_FLAG_UCP: a non-ASCII character is its UTF-8 encoding */
+    bool utf8Mode() const { return (flags & HS_FLAG_UTF8) && !(flags & HS_FLAG_UCP); }
 
     static void cap(const std::set<std::string> &s, const FiniteRegex *self) {
         if (s.size() > MAX_STRINGS) {
@@ -649,6 +658,9 @@ private:
             if (h1 < 0 || h2 < 0) {
                 needsRegex("A hex escape other than \\xHH");
             }
+            if (h1 >= 8 && utf8Mode()) {
+                needsRegex("A hex escape above \\x7F under HS_FLAG_UTF8"); /* a code point of two bytes */
+            }
             pos += 2;
             return (unsigned char)(h1 * 16 + h2);
         }
@@ -659,11 +671,17 @@ private:
             if (isalnum(e)) {
                 needsRegex(std::string("Escape sequence \\") + (char)e);
             }
+            if (e >= 0x80 && utf8Mode()) {
+                needsRegex("An escaped non-ASCII character under HS_FLAG_UTF8");
+            }
             return e; /* escaped punctuation */
         }
     }
 
     unsigned char plain(unsigned char c) const {
+        if (c >= 0x80 && utf8Mode()) {
+            needsRegex("A non-ASCII class member under HS_FLAG_UTF8");
+        }
         if (c >= 0x80 && (flags & (HS_FLAG_UTF8 | HS_FLAG_UCP))) {
             fail("Non-ASCII characters under HS_FLAG_UTF8/UCP are not supported by the literal "
                  "compiler.");
@@ -779,6 +797,14 @@ private:
         }
         if (strchr("*+?{", c)) {
             fail("Invalid repeat: nothing to repeat.");
+        }
+        if (c >= 0x80 && utf8Mode()) { /* one character: all the bytes of its (validated) encoding */
+            if (flags & HS_FLAG_CASELESS) {
+                needsRegex("A caseless non-ASCII character");
+            }
+            const size_t len = c < 0xe0 ? 2 : c < 0xf0 ? 3 : 4;
+            pos += len;
+            return {std::string(re + pos - len, len)};
         }
         pos++;
         return {std::string(1, (char)plain(c))};
@@ -945,6 +971,9 @@ static hs_error_t compileCommon(const char *const *expressions,
             if ((f & HS_FLAG_SINGLEMATCH) && (f & HS_FLAG_SOM_LEFTMOST)) {
                 throw CompileError{"HS_FLAG_SINGLEMATCH is not supported in "
                                    "combination with HS_FLAG_SOM_LEFTMOST.", (int)i};
+            }
+            if (!litApi && (f & HS_FLAG_UTF8) && !validUtf8(expressions[i], strlen(expressions[i]))) {
+                throw CompileError{"Expression is not valid UTF-8.", (int)i};
             }
             LitPattern p;
             p.index = i;
@@ -1194,6 +1223,9 @@ static hs_error_t exprInfo(const char *expression, unsigned flags, const hs_expr
     try {
         if (flags & ~0x7ffu) {
             throw CompileError{"Unrecognised flag.", 0};
+        }
+        if ((flags & HS_FLAG_UTF8) && !validUtf8(expression, strlen(expression))) {
+            throw CompileError{"Expression is not valid UTF-8.", 0};
         }
         if (ext && ext->flags != 0) {
             if (ext->flags & ~(HS_EXT_FLAG_MIN_OFFSET | HS_EXT_FLAG_MAX_OFFSET | HS_EXT_FLAG_MIN_LENGTH |

@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <bitset>
 #include <cstring>
+#include <map>
 #include <memory>
 
 #include "../../../include/hs_b200.h"
@@ -17,6 +18,7 @@ typedef std::bitset<256> CharSet;
 struct Node {
     enum Kind { CLASS, CAT, ALT, STAR, PLUS, OPT, EMPTY, ASSERT } kind = EMPTY;
     int assertKind = 0;    /* ASSERT: one of the A_* bits below */
+    bool unit = false;     /* the byte automaton of one UTF-8 character set: never split into top-level arms */
     CharSet cls;
     std::vector<std::shared_ptr<Node>> kids;
 };
@@ -50,13 +52,189 @@ NodeP clone(const NodeP &n) {
     return c;
 }
 
+/* ---- UTF-8 mode ------------------------------------------------------------------------------
+ * A set of code points is a sorted list of disjoint inclusive ranges.  It becomes a byte automaton:
+ * every range is cut into runs whose UTF-8 encodings are a product of byte ranges (one range per
+ * byte, 1 to 4 bytes), and those byte-range sequences form a tree that shares common suffixes,
+ * whose leaves are ordinary character positions of the Glushkov construction. */
+const u32 MAX_UNICODE = 0x10ffff;
+typedef std::vector<std::pair<u32, u32>> Cps;
+
+Cps cpsNorm(Cps s) {
+    std::sort(s.begin(), s.end());
+    Cps out;
+    for (const auto &r : s) {
+        if (!out.empty() && r.first <= out.back().second + 1) {
+            out.back().second = std::max(out.back().second, r.second);
+        } else {
+            out.push_back(r);
+        }
+    }
+    return out;
+}
+
+Cps cpsFlip(const Cps &in) { /* over [0, 0x10ffff], surrogates included, as the reference's CodePointSet::flip */
+    const Cps s = cpsNorm(in);
+    Cps out;
+    u32 next = 0;
+    for (const auto &r : s) {
+        if (r.first > next) {
+            out.push_back({next, r.first - 1});
+        }
+        next = r.second + 1;
+    }
+    if (next <= MAX_UNICODE) {
+        out.push_back({next, MAX_UNICODE});
+    }
+    return out;
+}
+
+Cps cpsOf(const CharSet &c) {
+    Cps s;
+    for (u32 b = 0; b < 256; b++) {
+        if (c[b]) s.push_back({b, b});
+    }
+    return cpsNorm(s);
+}
+
+typedef std::vector<std::pair<u8, u8>> ByteSeq; /* one inclusive byte range per byte of the encoding */
+
+void utf8Encode(u32 c, u8 *out, int len) {
+    static const u8 head[] = {0, 0, 0xc0, 0xe0, 0xf0};
+    for (int i = len - 1; i > 0; i--) {
+        out[i] = (u8)(0x80 | (c & 0x3f));
+        c >>= 6;
+    }
+    out[0] = (u8)(len == 1 ? c : (head[len] | c));
+}
+
+/* the runs of [lo, hi] whose encodings are products of byte ranges */
+void utf8Runs(u32 lo, u32 hi, std::vector<ByteSeq> *out) {
+    static const u32 lim[] = {0x7f, 0x7ff, 0xffff};
+    for (u32 l : lim) {
+        if (lo <= l && hi > l) {
+            utf8Runs(lo, l, out);
+            utf8Runs(l + 1, hi, out);
+            return;
+        }
+    }
+    const int len = lo <= 0x7f ? 1 : lo <= 0x7ff ? 2 : lo <= 0xffff ? 3 : 4;
+    for (int i = 1; i < len; i++) {
+        const u32 m = (1u << (6 * i)) - 1;
+        if ((lo & ~m) != (hi & ~m)) {
+            if (lo & m) {
+                utf8Runs(lo, lo | m, out);
+                utf8Runs((lo | m) + 1, hi, out);
+                return;
+            }
+            if ((hi & m) != m) {
+                utf8Runs(lo, (hi & ~m) - 1, out);
+                utf8Runs(hi & ~m, hi, out);
+                return;
+            }
+        }
+    }
+    u8 a[4], b[4];
+    utf8Encode(lo, a, len);
+    utf8Encode(hi, b, len);
+    ByteSeq s;
+    for (int i = 0; i < len; i++) {
+        s.push_back({a[i], b[i]});
+    }
+    out->push_back(s);
+}
+
+NodeP byteLeaf(u32 lo, u32 hi) {
+    NodeP l = mk(Node::CLASS);
+    for (u32 b = lo; b <= hi; b++) {
+        l->cls[b] = true;
+    }
+    return l;
+}
+
+/* alternation of byte-range sequences (all non-empty), sharing common suffixes: the sequences are grouped by their
+ * last byte range, and the ones whose prefix is used up merge into one position */
+NodeP suffixTree(const std::vector<ByteSeq> &seqs) {
+    std::map<std::pair<u8, u8>, std::vector<ByteSeq>> byLast;
+    for (ByteSeq s : seqs) {
+        const auto last = s.back();
+        s.pop_back();
+        byLast[last].push_back(s);
+    }
+    NodeP alt = mk(Node::ALT);
+    NodeP single; /* the last byte of a sequence that has no prefix left */
+    for (const auto &g : byLast) {
+        std::vector<ByteSeq> rest;
+        bool ends = false;
+        for (const ByteSeq &s : g.second) {
+            if (s.empty()) {
+                ends = true;
+            } else {
+                rest.push_back(s);
+            }
+        }
+        if (ends && rest.empty()) {
+            if (!single) {
+                single = mk(Node::CLASS);
+                alt->kids.push_back(single);
+            }
+            single->cls |= byteLeaf(g.first.first, g.first.second)->cls;
+            continue;
+        }
+        NodeP pre = suffixTree(rest);
+        if (ends) {
+            NodeP o = mk(Node::OPT);
+            o->kids.push_back(pre);
+            pre = o;
+        }
+        NodeP cat = mk(Node::CAT);
+        cat->kids = {pre, byteLeaf(g.first.first, g.first.second)};
+        alt->kids.push_back(cat);
+    }
+    return alt->kids.size() == 1 ? alt->kids[0] : alt;
+}
+
+} // namespace
+
+bool validUtf8(const char *s, size_t len) {
+    const u8 *p = (const u8 *)s;
+    size_t i = 0;
+    while (i < len) {
+        const u8 c = p[i];
+        const int n = c < 0x80 ? 1 : (c & 0xe0) == 0xc0 ? 2 : (c & 0xf0) == 0xe0 ? 3 : (c & 0xf8) == 0xf0 ? 4 : 0;
+        if (!n || i + n > len) {
+            return false;
+        }
+        u32 v = n == 1 ? c : c & (0x7f >> n);
+        for (int k = 1; k < n; k++) {
+            if ((p[i + k] & 0xc0) != 0x80) {
+                return false;
+            }
+            v = (v << 6) | (p[i + k] & 0x3f);
+        }
+        static const u32 least[] = {0, 0, 0x80, 0x800, 0x10000};
+        if (v < least[n] || v > MAX_UNICODE || (v >= 0xd800 && v <= 0xdfff)) {
+            return false; /* overlong, beyond Unicode, or a surrogate */
+        }
+        i += n;
+    }
+    return true;
+}
+
+namespace {
+
 class Parser {
 public:
-    Parser(const char *re_in, unsigned flags_in) : re(re_in), n(strlen(re_in)), flags(flags_in) {}
+    Parser(const char *re_in, unsigned flags_in)
+        : re(re_in), n(strlen(re_in)), flags(flags_in), utf8(flags_in & HS_FLAG_UTF8) {}
 
     NodeP parse() {
-        if (flags & (HS_FLAG_UTF8 | HS_FLAG_UCP)) {
-            fail("HS_FLAG_UTF8 / HS_FLAG_UCP need the reference's Unicode compiler.");
+        if (flags & HS_FLAG_UCP) {
+            fail("HS_FLAG_UCP is not supported: Unicode character classes need the reference's Unicode property "
+                 "tables.");
+        }
+        if (utf8 && !validUtf8(re, n)) {
+            fail("Expression is not valid UTF-8.");
         }
         if (flags & HS_FLAG_SOM_LEFTMOST) {
             fail("HS_FLAG_SOM_LEFTMOST is not supported.");
@@ -76,11 +254,290 @@ private:
     const char *re;
     size_t n, pos = 0;
     unsigned flags;
+    const bool utf8;      /* HS_FLAG_UTF8: characters are code points, encoded in 1 to 4 bytes */
     size_t unrolled = 0;  /* positions made by unrolling bounded repeats so far */
     bool quoting = false; /* between \\Q and \\E: every byte is a literal */
 
     [[noreturn]] void fail(const std::string &m) const { throw RegexError{m}; }
     bool at(char c) const { return pos < n && re[pos] == c; }
+
+    /* the (validated) UTF-8 character at pos; pos moves past it */
+    u32 readChar() {
+        const u8 c = (u8)re[pos];
+        const int len = c < 0x80 ? 1 : c < 0xe0 ? 2 : c < 0xf0 ? 3 : 4;
+        u32 v = len == 1 ? c : c & (0x7f >> len);
+        for (int k = 1; k < len; k++) {
+            v = (v << 6) | ((u8)re[pos + k] & 0x3f);
+        }
+        pos += len;
+        return v;
+    }
+
+    /* UTF-8 mode, a character or range written in the expression under HS_FLAG_CASELESS: ASCII letters take their
+     * other case, and "k" / "s" also the two non-ASCII characters that fold to them, KELVIN SIGN (U+212A) and LATIN
+     * SMALL LETTER LONG S (U+017F), as the reference's case folding does.  Non-ASCII case folding needs Unicode
+     * tables this compiler does not have. */
+    Cps foldU(u32 lo, u32 hi) const {
+        Cps s = {{lo, hi}};
+        if (!(flags & HS_FLAG_CASELESS)) {
+            return s;
+        }
+        if (hi >= 0x80) {
+            fail("HS_FLAG_CASELESS on a non-ASCII character is not supported under HS_FLAG_UTF8: it needs Unicode "
+                 "case folding.");
+        }
+        for (u32 c = lo; c <= hi; c++) {
+            const u32 l = c | 0x20;
+            if (l >= 'a' && l <= 'z') {
+                s.push_back({l, l});
+                s.push_back({l - 32, l - 32});
+                if (l == 'k') s.push_back({0x212a, 0x212a});
+                if (l == 's') s.push_back({0x17f, 0x17f});
+            }
+        }
+        return cpsNorm(s);
+    }
+
+    /* a set of code points as a node: ASCII only, one position; else the byte automaton of the UTF-8 encodings */
+    NodeP unit(const Cps &in) {
+        const Cps s = cpsNorm(in);
+        if (s.empty()) {
+            fail("Empty character class.");
+        }
+        CharSet ascii;
+        std::vector<ByteSeq> multi;
+        for (const auto &r : s) {
+            for (u32 c = r.first; c <= std::min<u32>(r.second, 0x7f); c++) {
+                ascii[c] = true;
+            }
+            if (r.second >= 0x80) {
+                utf8Runs(std::max<u32>(r.first, 0x80), r.second, &multi);
+            }
+        }
+        if (multi.empty()) {
+            return leaf(ascii);
+        }
+        NodeP m = suffixTree(multi);
+        NodeP u = m;
+        if (ascii.any()) {
+            u = mk(Node::ALT);
+            NodeP a = mk(Node::CLASS);
+            a->cls = ascii;
+            u->kids = {a, m};
+        }
+        u->unit = true;
+        return u;
+    }
+
+    /* \\h / \\v under HS_FLAG_UTF8: PCRE's horizontal and vertical white space */
+    static Cps spaceU(bool vertical) {
+        if (vertical) {
+            return {{0x0a, 0x0d}, {0x85, 0x85}, {0x2028, 0x2029}};
+        }
+        return {{0x09, 0x09}, {0x20, 0x20}, {0xa0, 0xa0}, {0x1680, 0x1680}, {0x180e, 0x180e},
+                {0x2000, 0x200a}, {0x202f, 0x202f}, {0x205f, 0x205f}, {0x3000, 0x3000}};
+    }
+
+    /* an escape under HS_FLAG_UTF8: either one code point (*single) or a set; pos is at the backslash */
+    Cps escapeU(bool inClass, long *single) {
+        *single = -1;
+        if (pos + 1 >= n) {
+            fail("Unterminated escape at end of pattern.");
+        }
+        const unsigned char e = (unsigned char)re[pos + 1];
+        switch (e) {
+        case 'p': case 'P':
+            fail("\\p / \\P (Unicode properties) are not supported: they need the reference's Unicode property "
+                 "tables.");
+        case 'X':
+            fail("\\X (an extended grapheme cluster) is not supported: it needs the reference's Unicode property "
+                 "tables.");
+        case 'd': case 'D': case 'w': case 'W': case 's': case 'S': {
+            pos += 2;
+            const Cps s = cpsOf(classEscape((char)(e | 0x20)));
+            return e >= 'a' ? s : cpsFlip(s);
+        }
+        case 'h': case 'H': case 'v': case 'V': {
+            pos += 2;
+            const Cps s = spaceU((e | 0x20) == 'v');
+            return e >= 'a' ? s : cpsFlip(s);
+        }
+        case 'N':
+            pos += 2;
+            return cpsFlip({{'\n', '\n'}});
+        case 'x': case 'o': {
+            pos += 2;
+            const bool hex = e == 'x';
+            if (hex && !at('{')) { /* \\x and up to two hexadecimal digits */
+                u32 v = 0;
+                for (int k = 0; k < 2 && pos < n && hexval(re[pos]) >= 0; k++) {
+                    v = v * 16 + (u32)hexval(re[pos++]);
+                }
+                *single = v;
+                return {{v, v}};
+            }
+            size_t q = pos + 1;
+            u64 v = 0;
+            while (q < n && (hex ? hexval(re[q]) >= 0 : (re[q] >= '0' && re[q] <= '7'))) {
+                v = std::min<u64>(v * (hex ? 16 : 8) + (u64)(hex ? hexval(re[q]) : re[q] - '0'), MAX_UNICODE + 1);
+                q++;
+            }
+            if (!at('{') || q == pos + 1 || q >= n || re[q] != '}') {
+                fail(hex ? "Value in \\x{...} sequence is non-hex or missing }"
+                         : "Value in \\o{...} sequence is non-octal or missing braces");
+            }
+            if (v > MAX_UNICODE) {
+                fail(hex ? "Value in \\x{...} sequence is too large" : "Value in \\o{...} sequence is too large");
+            }
+            pos = q + 1;
+            *single = (long)v;
+            return {{(u32)v, (u32)v}};
+        }
+        default:
+            break;
+        }
+        if (inClass && e >= '1' && e <= '7') { /* octal, up to three digits: a code point up to \\777 */
+            pos += 2;
+            u32 v = e - '0';
+            for (int k = 0; k < 2 && pos < n && re[pos] >= '0' && re[pos] <= '7'; k++) {
+                v = v * 8 + (u32)(re[pos++] - '0');
+            }
+            *single = v;
+            return {{v, v}};
+        }
+        if (e >= 0x80) { /* an escaped non-ASCII character is that character */
+            pos++;
+            const u32 v = readChar();
+            *single = v;
+            return {{v, v}};
+        }
+        int b;
+        escape(inClass, &b); /* the rest name ASCII characters */
+        *single = b;
+        return {{(u32)b, (u32)b}};
+    }
+
+    Cps charClassU() {
+        pos++; /* [ */
+        bool negate = false;
+        if (at('^')) {
+            negate = true;
+            pos++;
+        }
+        Cps set;
+        bool first = true;   /* no member yet: a "]" is a literal */
+        bool quoted = false; /* between \\Q and \\E */
+        long prev = -1;
+        auto add = [&](const Cps &s) { set.insert(set.end(), s.begin(), s.end()); };
+        for (;;) {
+            if (pos >= n) {
+                fail("Unterminated character class.");
+            }
+            const unsigned char c = (unsigned char)re[pos];
+            if (c == '\\' && pos + 1 < n && (re[pos + 1] == 'E' || (re[pos + 1] == 'Q' && !quoted))) {
+                quoted = re[pos + 1] == 'Q';
+                pos += 2;
+                continue;
+            }
+            if (quoted) {
+                prev = readChar();
+                add(foldU((u32)prev, (u32)prev));
+                first = false;
+                continue;
+            }
+            if (c == ']' && !first) {
+                pos++;
+                break;
+            }
+            first = false;
+            if (c == '[' && pos + 1 < n && re[pos + 1] == ':') {
+                const char *close = strstr(re + pos + 2, ":]");
+                if (!close) {
+                    fail("Unterminated POSIX character class.");
+                }
+                std::string name(re + pos + 2, close);
+                bool neg = false;
+                if (!name.empty() && name[0] == '^') {
+                    neg = true;
+                    name.erase(0, 1);
+                }
+                CharSet pc;
+                if (!posixClass(name, &pc)) {
+                    fail("Unknown POSIX character class.");
+                }
+                const Cps s = cpsOf(fold(pc)); /* ASCII classes: ASCII case folding only */
+                add(neg ? cpsFlip(s) : s);
+                pos = (size_t)(close - re) + 2;
+                prev = -1;
+                continue;
+            }
+            if (c == '[' && pos + 1 < n && (re[pos + 1] == '.' || re[pos + 1] == '=')) {
+                fail("POSIX collating elements are not supported.");
+            }
+            if (c == '-' && prev >= 0 && pos + 1 < n && re[pos + 1] != ']') {
+                pos++;
+                long hi;
+                if (re[pos] == '[' && pos + 1 < n && strchr(":.=", re[pos + 1])) {
+                    fail("Invalid range in character class.");
+                }
+                if (re[pos] == '\\') {
+                    if (pos + 1 < n && (re[pos + 1] == 'Q' || re[pos + 1] == 'E')) {
+                        fail("\\Q / \\E as the end of a range is not supported.");
+                    }
+                    escapeU(true, &hi);
+                    if (hi < 0) {
+                        fail("Invalid range in character class.");
+                    }
+                } else {
+                    hi = readChar();
+                }
+                if (hi < prev) {
+                    fail("Invalid range in character class.");
+                }
+                add(foldU((u32)prev, (u32)hi));
+                prev = -1;
+                continue;
+            }
+            if (c == '\\') {
+                long single;
+                const Cps e = escapeU(true, &single);
+                add(single >= 0 ? foldU((u32)single, (u32)single) : e);
+                prev = single;
+            } else {
+                prev = readChar();
+                add(foldU((u32)prev, (u32)prev));
+            }
+        }
+        return negate ? cpsFlip(set) : cpsNorm(set);
+    }
+
+    /* one atom under HS_FLAG_UTF8 that is not a group, a class, an assertion or an option: pos is at it */
+    NodeP atomU() {
+        const unsigned char c = (unsigned char)re[pos];
+        if (quoting) {
+            const u32 v = readChar();
+            return unit(foldU(v, v));
+        }
+        if (c == '\\') {
+            if (pos + 1 < n && re[pos + 1] == 'C') { /* \\C: one byte, whatever it is */
+                pos += 2;
+                CharSet any;
+                return leaf(any.set());
+            }
+            long single;
+            const Cps s = escapeU(false, &single);
+            return unit(single >= 0 ? foldU((u32)single, (u32)single) : s);
+        }
+        if (c == '.') {
+            pos++;
+            return unit(flags & HS_FLAG_DOTALL ? Cps{{0, MAX_UNICODE}} : cpsFlip({{'\n', '\n'}}));
+        }
+        if (strchr("*+?", c) || (c == '{' && startsRepeat(pos))) {
+            fail("Invalid repeat: nothing to repeat.");
+        }
+        const u32 v = readChar();
+        return unit(foldU(v, v));
+    }
 
     CharSet fold(CharSet s) const {
         if (flags & HS_FLAG_CASELESS) {
@@ -573,6 +1030,9 @@ private:
             return mk(Node::EMPTY);
         }
         const unsigned char c = (unsigned char)re[pos];
+        if (quoting && utf8) {
+            return atomU();
+        }
         if (quoting) {
             pos++;
             CharSet s;
@@ -634,7 +1094,7 @@ private:
                     }
                 }
             }
-            return leaf(charClass());
+            return utf8 ? unit(charClassU()) : leaf(charClass());
         }
         if (c == '\\' && pos + 1 < n && strchr("bBAzZ", re[pos + 1])) {
             NodeP a = mk(Node::ASSERT);
@@ -649,6 +1109,9 @@ private:
             a->assertKind = c == '^' ? (ml ? A_BEGIN_LINE : A_BEGIN) : (ml ? A_END_LINE : A_END_LF);
             pos++;
             return a;
+        }
+        if (utf8) {
+            return atomU();
         }
         if (c == '\\') {
             int single;
@@ -914,7 +1377,7 @@ std::vector<NodeP> topArms(const NodeP &root) {
     while (r->kind == Node::CAT && r->kids.size() == 1) {
         r = r->kids[0];
     }
-    if (r->kind == Node::ALT) {
+    if (r->kind == Node::ALT && !r->unit) {
         return r->kids;
     }
     return {root};

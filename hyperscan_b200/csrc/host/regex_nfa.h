@@ -15,10 +15,20 @@
  * data or before a final newline; "$" under HS_FLAG_MULTILINE before any newline or at the end),
  * \z (end of data) -- anywhere the reference takes them: where nothing can have been consumed
  * before a start anchor / can be consumed after an end anchor (ComponentBoundary.cpp:162-185),
- * groups and alternations included.  HS_FLAG_CASELESS folds letters.  Everything else --
- * look-around, back-references, possessive quantifiers, UTF-8 / UCP, SOM, expressions that match
- * the empty string -- is refused with a compile error: those need parts of the reference's
- * compiler and runtime this build does not have.
+ * groups and alternations included.  HS_FLAG_CASELESS folds letters.
+ *
+ * HS_FLAG_UTF8 (src/parser/Utf8ComponentClass.cpp): the expression must be valid UTF-8; a character
+ * is a code point (literal, \x{h..h}, \o{o..o} up to 0x10FFFF) and matches its encoding; ".",
+ * negated classes, classes with non-ASCII members and \W \D \S \H \V \N match whole encoded
+ * characters -- each is a small byte automaton (the encodings of its code-point set as a tree of
+ * byte ranges) whose positions join the Glushkov construction.  \w \d \s, POSIX classes and
+ * \b \B keep their ASCII meaning; \C is one byte.  Case folding is ASCII only (plus KELVIN SIGN
+ * and LONG S, which fold to "k" and "s"); a caseless non-ASCII character, \p \P \X and
+ * HS_FLAG_UCP are refused.
+ *
+ * Everything else -- look-around, back-references, possessive quantifiers, UCP, SOM, expressions
+ * that match the empty string -- is refused with a compile error: those need parts of the
+ * reference's compiler and runtime this build does not have.
  */
 #ifndef HSB200_REGEX_NFA_H
 #define HSB200_REGEX_NFA_H
@@ -46,6 +56,10 @@ struct RegexInfo {
     std::vector<std::pair<u32, u32>> armWidths; /* (shortest, longest) match of every top-level alternative */
     bool anchored = false; /* every way into the expression crosses \A / a non-multiline "^" */
 };
+
+/* Valid UTF-8 (src/parser/utf8_validate.cpp): no overlong form, surrogate, code point above 0x10FFFF or
+ * truncated character. */
+bool validUtf8(const char *s, size_t len);
 
 /* Number of positions / shortest match of one expression (throws RegexError).  forInfo: hs_expression_info also
  * describes expressions that match the empty buffer (hs_compile refuses those without HS_FLAG_ALLOWEMPTY). */

@@ -54,6 +54,12 @@ typedef int hs_error_t;                     /* src/hs_common.h:52 */
 #define HS_FLAG_MULTILINE 4
 #define HS_FLAG_SINGLEMATCH 8
 #define HS_FLAG_ALLOWEMPTY 16
+/* HS_FLAG_UTF8: the expression is UTF-8 (validated; "Expression is not valid UTF-8." otherwise) and its
+ * characters are code points, matched as their 1- to 4-byte encodings ("." and negated classes match whole
+ * encoded characters); \w \d \s, POSIX classes and \b keep their ASCII meaning; widths and offsets count
+ * bytes.  Refused: \p / \P, \X, and HS_FLAG_CASELESS on a non-ASCII character (DESIGN.md section 10b).
+ * HS_FLAG_UCP: refused wherever it could change the meaning (it needs the Unicode property tables); a finite
+ * set of ASCII literals compiles as without it. */
 #define HS_FLAG_UTF8 32
 #define HS_FLAG_UCP 64
 #define HS_FLAG_PREFILTER 128
@@ -139,7 +145,8 @@ typedef int (*match_event_handler)(unsigned int id, unsigned long long from,
  * Where they do not fit only because of expressions that are finite sets of
  * literals, those go to a literal matcher beside that engine instead
  * (ROSE_RUNTIME_FULL_ROSE, block mode) -- DESIGN.md section 10d.
- * Anything else (look-around, back-references, UTF-8 / UCP, larger sets, ...) yields
+ * Expressions in UTF-8 mode (HS_FLAG_UTF8) take either route.
+ * Anything else (look-around, back-references, UCP, larger sets, ...) yields
  * HS_COMPILER_ERROR with an explanatory hs_compile_error_t, exactly as the
  * reference reports unsupported constructs.
  * Logical combinations (HS_FLAG_COMBINATION, with HS_FLAG_QUIET on any expression) are
