@@ -113,6 +113,8 @@ def lib():
         L.hs_b200_streams_scan.argtypes = [vp, vp, vp, vp, vp, BLOCK_CB, vp, u64p]
         L.hs_b200_streams_scan_collect.argtypes = [vp, vp, vp, vp, vp, vp, C.c_size_t, u64p]
         L.hs_b200_streams_close.argtypes = [vp]
+        L.hs_b200_streams_scan_async.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint, vp, vp]
+        L.hs_b200_streams_reset_async.argtypes = [vp, vp, C.c_size_t, vp]
         L.hs_b200_streams_state_bytes.argtypes = [vp]
         L.hs_b200_streams_state_bytes.restype = C.c_size_t
         L.hs_open_stream.argtypes = [vp, C.c_uint, C.POINTER(vp)]
@@ -646,6 +648,29 @@ class StreamSet:
             raise HsError(rc, "streams_scan_collect: %d matches exceed the harness buffer" % n.value)
         _check(rc, "streams_scan_collect")
         return self._out[: int(n.value)].copy()
+
+    def scan_async(self, writes, pitch, lengths, scratch, stream=None):
+        """hs_b200_streams_scan_async: one pass over writes already in device memory -- `writes` a CUDA tensor
+        (a numpy array under the SIMT emulator) of nstreams * pitch bytes, stream i's write at i * pitch + 16 --
+        whose lengths are `lengths` (a device array of nstreams uint32) or, given as an int, all that long.
+        Enqueued on `stream` (a cudaStream_t address; None = the scratch's stream); returns at once.  The
+        records are served by scan_corpus_finish, fetch_matches and order_matches_async(self.db, ...)."""
+        if isinstance(lengths, (int, np.integer)):
+            d_len, uni = None, int(lengths)
+        else:
+            d_len, uni = _dev_ptr(lengths), 0
+        _check(lib().hs_b200_streams_scan_async(self.ptr, _dev_ptr(writes), int(pitch), d_len, uni, scratch.ptr,
+                                                C.c_void_p(stream or 0)), "streams_scan_async")
+
+    def reset_async(self, indices, stream):
+        """hs_b200_streams_reset_async: end the flows of the streams listed in `indices` (a device array of
+        uint32; None = every stream): empty look-behind, offset 0.  `stream` is the cudaStream_t address the
+        passes run on, given explicitly: None is the legacy default stream, which does not order against the
+        scratch's own stream that scan_async(stream=None) uses.  On a set marked by an overflow the reset
+        commits nothing (hs_b200_streams_scan_async)."""
+        n = 0 if indices is None else (indices.numel() if hasattr(indices, "numel") else np.asarray(indices).size)
+        _check(lib().hs_b200_streams_reset_async(self.ptr, _dev_ptr(indices), n, C.c_void_p(stream or 0)),
+               "streams_reset_async")
 
     def close(self):
         if self.ptr:

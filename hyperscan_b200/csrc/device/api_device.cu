@@ -872,6 +872,9 @@ struct hs_scratch {
     /* of the last hs_b200_scan_corpus_async: bounds of its records' block and end offset, for the sort key
      * of hs_b200_order_matches_async */
     u64 lastBlocks, lastMaxLen;
+    /* of the last scan, when it was a stream-set pass: its set's epoch (StreamMark), which finishScan advances
+     * once it has seen the set marked; null otherwise */
+    u32 *streamEpoch;
     /* temporaries of hs_b200_order_*_async (order_kernels.h), grown on demand */
     u8 *d_order;
     size_t orderBytes;
@@ -1320,8 +1323,18 @@ hs_error_t finishScan(hs_scratch *s, u32 *count) {
         return HS_UNKNOWN_ERROR;
     }
     cudaEventElapsedTime(&s->lastMs, s->evStart, s->evStop);
+    const u32 stream = s->h_counters[CTR_STREAM];
+    if (stream && s->streamEpoch) {
+        /* a stream-set pass did not commit: the passes and resets enqueued from now on belong to the next epoch,
+         * which the mark does not hold back (no device work: a reset enqueued before may still be pending) */
+        *s->streamEpoch = *s->streamEpoch + 1 == 0xffffffffu ? 0 : *s->streamEpoch + 1;
+    }
     if (s->h_counters[CTR_ERROR]) {
         return HS_UNKNOWN_ERROR;
+    }
+    if (stream & STREAM_BAD_LENGTH) {
+        s->lastCount = 0;
+        return HS_INVALID;
     }
     *count = s->h_counters[CTR_MATCHES];
     s->lastCount = *count;
@@ -1338,10 +1351,24 @@ struct Upload {
     std::function<hs_error_t(size_t ci, u64 *covered)> chunk;
 };
 
+/* The device half of one stream-set pass over a pitched corpus (hs_b200_streams_*): the set's state and, for
+ * writes whose lengths the caller keeps in device memory, those lengths. */
+struct StreamPass {
+    u8 *hist;
+    u64 *offset;
+    u32 *len;            /* the lengths the scan reads (the corpus's blockLen) */
+    const u32 *srcLen;   /* != null: the caller's, checked and copied into len by the assemble kernel */
+    u32 histReq;
+    StreamMark *mark;
+    u32 *epoch;          /* the set's epoch (host memory), read at enqueue time */
+};
+
 /* Enqueue a scan of the whole corpus on `stream`: reset the counters, launch the tile
- * ranges, read the counters back.  The only place a scan's stream sequence is issued. */
+ * ranges, read the counters back.  The only place a scan's stream sequence is issued.
+ * For a stream-set pass (sp), the look-behind is written in front of every write first,
+ * and the streams advance -- or the set is marked -- before the counters are read back. */
 hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
-                       cudaStream_t stream, const Upload *up = nullptr) {
+                       cudaStream_t stream, const Upload *up = nullptr, const StreamPass *sp = nullptr) {
     if (s->nPeers && (im->rules.shape == SHAPE_LITERALS_OUTFIX || im->rules.shape == SHAPE_OUTFIXES)) {
         /* the engine kernel stores no records into the peers' exchange buffers, and the count it
          * publishes would cover them: an exchange of both halves' records, or of several engines',
@@ -1354,6 +1381,11 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
         return r;
     }
     CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), stream));
+    if (sp) {
+        CUDA_TRY(launchStreamAssemble(c->d_data, sp->hist, (u32)c->nblocks, c->streamPitch, sp->srcLen, sp->len,
+                                      sp->mark, *sp->epoch, stream));
+        g_launches++;
+    }
     CUDA_TRY(cudaEventRecord(s->evStart, stream));
     const u32 ntiles = (u32)((c->bytes + pl.tileBytes - 1) / pl.tileBytes);
     u32 tDone = 0;
@@ -1376,6 +1408,13 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
         return r;
     }
     CUDA_TRY(cudaEventRecord(s->evStop, stream));
+    if (sp) {
+        CUDA_TRY(launchStreamAdvance(c->d_data, sp->hist, sp->offset, sp->len, c->uniformLen, (u32)c->nblocks,
+                                     c->streamPitch, sp->histReq, s->d_counters, s->outCap, sp->mark, *sp->epoch,
+                                     stream));
+        g_launches++;
+    }
+    s->streamEpoch = sp ? sp->epoch : nullptr;
     if (s->nPeers) {
         ScanParams pp;
         fillParams(s, im, c, pl, &pp);
@@ -1409,12 +1448,12 @@ struct ScanTimes {
  * that was resident from the start. */
 hs_error_t scanRecords(hs_scratch *s, DevImage *im, const hs_b200_corpus *c, const Upload *up,
                        bool ordered, std::vector<DevMatch> *matches, ScanTimes *times = nullptr,
-                       const u32 *lengths = nullptr) {
+                       const u32 *lengths = nullptr, const StreamPass *sp = nullptr) {
     ScanTimes unused;
     ScanTimes &t = times ? *times : unused;
     const int passes = up && up->nchunks > 1 ? 4 : 3;
     for (int attempt = 0; attempt < passes; attempt++) {
-        hs_error_t r = enqueueScan(s, im, c, s->stream, attempt == 0 ? up : nullptr);
+        hs_error_t r = enqueueScan(s, im, c, s->stream, attempt == 0 ? up : nullptr, sp);
         if (r != HS_SUCCESS) {
             return r;
         }
@@ -1993,6 +2032,7 @@ hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corp
             scratch->h_counters[CTR_ERROR] = 0;
             scratch->pending = false;
             scratch->lastCount = 0;
+            scratch->streamEpoch = nullptr;
             /* the device count too: the stream-ordered readers of the ring see no records */
             if (cudaMemsetAsync(scratch->d_counters, 0, CTR_COUNT * sizeof(u32), st) != cudaSuccess) {
                 r = HS_UNKNOWN_ERROR;
@@ -2209,13 +2249,16 @@ static DevImage *heldImage(hs_scratch *s, const hs_database_t *db) {
 }
 
 static hs_error_t checkOrderArgs(const hs_database_t *db, hs_scratch_t *scratch, void *d_out, size_t cap,
-                                 void *d_count, DevImage **im) {
+                                 void *d_count, DevImage **im, u32 mode = MODE_BLOCK) {
     if (!db || !scratch || !d_count || (cap && !d_out)) {
         return HS_INVALID;
     }
-    hs_error_t r = checkScanArgs(db, scratch);
+    hs_error_t r = checkDb(db, mode);
     if (r != HS_SUCCESS) {
         return r;
+    }
+    if (!validScratch(scratch)) {
+        return HS_INVALID;
     }
     if (dbRose(db)->ckeyCount) {
         return HS_INVALID; /* combination reports are evaluated per block on the host */
@@ -2296,7 +2339,9 @@ static hs_error_t enqueueOrder(hs_scratch *s, const DevImage *im, const DevMatch
 hs_error_t hs_b200_order_matches_async(const hs_database_t *db, hs_scratch_t *scratch, void *d_out, size_t cap,
                                        void *d_count, void *cuda_stream) {
     DevImage *im = nullptr;
-    hs_error_t r = checkOrderArgs(db, scratch, d_out, cap, d_count, &im);
+    /* the last scan a stream-set pass: its records are a stream database's */
+    const bool streamPass = validScratch(scratch) && scratch->streamEpoch;
+    hs_error_t r = checkOrderArgs(db, scratch, d_out, cap, d_count, &im, streamPass ? MODE_STREAM : MODE_BLOCK);
     if (r != HS_SUCCESS) {
         return r;
     }
@@ -2304,9 +2349,11 @@ hs_error_t hs_b200_order_matches_async(const hs_database_t *db, hs_scratch_t *sc
         return HS_SCRATCH_IN_USE;
     }
     DeviceGuard guard(scratch->device);
-    /* the key needs no more bits than the last scan's block count, its longest block and the id table */
+    /* the key needs no more bits than the last scan's block count, its longest block and the id table; a
+     * stream pass's `to` is a stream offset, which only the device knows (up to 64 bits: the device decides
+     * the passes) */
     const u32 keyBits = bitWidth(im->orderTables.nIds ? im->orderTables.nIds - 1 : 0) +
-                        bitWidth(scratch->lastMaxLen + (u64)std::max(0, im->maxAdjust)) +
+                        (streamPass ? 64 : bitWidth(scratch->lastMaxLen + (u64)std::max(0, im->maxAdjust))) +
                         bitWidth(scratch->lastBlocks ? scratch->lastBlocks - 1 : 0);
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
     r = enqueueOrder(scratch, im, scratch->d_out, scratch->d_counters + CTR_MATCHES, scratch->outCap, 0, d_out, cap,
@@ -2982,7 +3029,11 @@ struct hs_b200_stream_set {
     u8 *d_hist;     /* 8 bytes per stream */
     u64 *d_offset;
     u32 *d_len;     /* per-write lengths when they differ */
-    hs_b200_corpus corpus; /* pitched staging, reused; its block lengths and stream state are the above */
+    StreamMark *d_mark;
+    u32 epoch;      /* of the mark (StreamMark): advanced by finishScan when it has seen the set marked */
+    hs_b200_corpus corpus; /* the pitched corpus of a pass: the set's staging (hs_b200_streams_scan) or the
+                            * caller's buffer (hs_b200_streams_scan_async); its block lengths and stream state
+                            * are the above */
 };
 
 hs_error_t hs_b200_streams_open(const hs_database_t *db, size_t nstreams, int device,
@@ -3014,9 +3065,13 @@ hs_error_t hs_b200_streams_open(const hs_database_t *db, size_t nstreams, int de
     s->d_hist = nullptr;
     s->d_offset = nullptr;
     s->d_len = nullptr;
+    s->d_mark = nullptr;
+    s->epoch = 0;
     cudaError_t e = cudaMalloc(&s->d_hist, nstreams * 8);
     if (e == cudaSuccess) e = cudaMalloc(&s->d_offset, nstreams * 8);
     if (e == cudaSuccess) e = cudaMalloc(&s->d_len, nstreams * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&s->d_mark, sizeof(StreamMark));
+    if (e == cudaSuccess) e = cudaMemset(s->d_mark, 0, sizeof(StreamMark));
     if (e == cudaSuccess) e = cudaMemset(s->d_hist, 0, nstreams * 8);
     if (e == cudaSuccess) e = cudaMemset(s->d_offset, 0, nstreams * 8);
     if (e != cudaSuccess) {
@@ -3039,6 +3094,7 @@ hs_error_t hs_b200_streams_close(hs_b200_stream_set_t *s) {
     cudaFree(s->d_hist);
     cudaFree(s->d_offset);
     cudaFree(s->d_len);
+    cudaFree(s->d_mark);
     cudaFree(s->corpus.d_alloc);
     delete s;
     return HS_SUCCESS;
@@ -3046,9 +3102,36 @@ hs_error_t hs_b200_streams_close(hs_b200_stream_set_t *s) {
 
 size_t hs_b200_streams_state_bytes(const hs_b200_stream_set_t *s) { return s ? s->nstreams * 16 : 0; }
 
-/* Copy one write per stream into the pitched corpus and drop each stream's
- * look-behind in front of it, scan the corpus, and roll history and offsets
- * forward once the scan has succeeded. */
+static StreamPass streamPass(hs_b200_stream_set_t *set, const u32 *srcLen) {
+    StreamPass sp;
+    sp.hist = set->d_hist;
+    sp.offset = set->d_offset;
+    sp.len = set->d_len;
+    sp.srcLen = srcLen;
+    sp.histReq = set->histReq;
+    sp.mark = set->d_mark;
+    sp.epoch = &set->epoch;
+    return sp;
+}
+
+/* The set's corpus over n * pitch bytes at d_data: stream b's write at b * pitch + 16 */
+static hs_b200_corpus *streamCorpus(hs_b200_stream_set_t *set, u8 *d_data, u32 pitch, u32 uniformLen,
+                                    u64 readableEnd) {
+    hs_b200_corpus *c = &set->corpus;
+    c->d_data = d_data;
+    c->nblocks = set->nstreams;
+    c->bytes = (u64)set->nstreams * pitch;
+    c->readableEnd = readableEnd;
+    c->payload = 0;
+    c->uniformPitch = 0;
+    c->uniformLen = uniformLen;
+    c->streamPitch = pitch;
+    return c;
+}
+
+/* Copy one write per stream into the set's pitched staging corpus, then run the pass's device sequence
+ * (enqueueScan with the stream pass: look-behind in front of every write, scan, advance) with the
+ * grow-and-rescan loop and the host ordering of scanRecords. */
 static hs_error_t streamsScanImpl(hs_b200_stream_set_t *set, const char *data,
                                   const unsigned long long *offsets, const unsigned int *lengths,
                                   hs_scratch *s, std::vector<DevMatch> *matches) {
@@ -3101,30 +3184,13 @@ static hs_error_t streamsScanImpl(hs_b200_stream_set_t *set, const char *data,
     if (e == cudaSuccess) {
         e = cudaMemsetAsync(c->d_data + total, 0, 48, st);
     }
-    if (e == cudaSuccess) e = launchStreamAssemble(c->d_data, set->d_hist, (u32)n, pitch, st);
     if (e != cudaSuccess) {
         return HS_UNKNOWN_ERROR;
     }
-    g_launches++;
-    c->nblocks = n;
-    c->bytes = total;
-    c->readableEnd = HSB_ROUNDUP(total, 16) + 16;
-    c->payload = 0;
-    c->uniformPitch = 0;
-    c->uniformLen = uni;
-    c->streamPitch = pitch;
-    r = scanRecords(s, im, c, nullptr, true, matches); /* a rescan reads the assembled corpus again */
-    if (r != HS_SUCCESS) {
-        return r;
-    }
-    e = launchStreamAdvance(c->d_data, set->d_hist, set->d_offset, set->d_len, uni, (u32)n, pitch,
-                            set->histReq, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-        return HS_UNKNOWN_ERROR;
-    }
-    g_launches++;
-    return HS_SUCCESS;
+    c = streamCorpus(set, c->d_data, pitch, uni, HSB_ROUNDUP(total, 16) + 16);
+    const StreamPass sp = streamPass(set, nullptr);
+    /* a rescan reads the staged writes again */
+    return scanRecords(s, im, c, nullptr, true, matches, nullptr, nullptr, &sp);
 }
 
 /* hs_b200_streams_scan and _collect: check the arguments, mark the scratch in use,
@@ -3178,6 +3244,57 @@ hs_error_t hs_b200_streams_scan_collect(hs_b200_stream_set_t *set, const char *d
         /* the stream state HAS advanced; the first cap records are valid */
         return matches.size() > cap ? HS_INSUFFICIENT_SPACE : HS_SUCCESS;
     });
+}
+
+hs_error_t hs_b200_streams_scan_async(hs_b200_stream_set_t *set, void *d_writes, size_t pitch,
+                                      const unsigned int *d_lengths, unsigned int uniform_length,
+                                      hs_scratch_t *scratch, void *cuda_stream) {
+    if (!set || !d_writes || (uintptr_t)d_writes % 16 || pitch < 32 || pitch % 16 || pitch > 0xfffffff0u ||
+        (!d_lengths && uniform_length > pitch - 16) || !validScratch(scratch) || scratch->device != set->device) {
+        return HS_INVALID;
+    }
+    if (markInUse(scratch)) {
+        return HS_SCRATCH_IN_USE;
+    }
+    DeviceGuard guard(set->device);
+    DevImage *im = nullptr;
+    hs_error_t r = findImage(scratch, set->db, &im);
+    if (r == HS_SUCCESS) {
+        cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
+        /* no uniform length and no device lengths: no stream has a write, which the scan reads from the
+         * set's length table */
+        if (!d_lengths && !uniform_length &&
+            cudaMemsetAsync(set->d_len, 0, set->nstreams * sizeof(u32), st) != cudaSuccess) {
+            r = HS_UNKNOWN_ERROR;
+        }
+        /* the caller's buffer as it is: nothing before it and nothing past the last stream is read */
+        const u64 bytes = (u64)set->nstreams * pitch;
+        hs_b200_corpus *c = streamCorpus(set, (u8 *)d_writes, (u32)pitch, d_lengths ? 0 : uniform_length, bytes);
+        const StreamPass sp = streamPass(set, d_lengths);
+        if (r == HS_SUCCESS) {
+            r = enqueueScan(scratch, im, c, st, nullptr, &sp);
+        }
+        scratch->lastCorpus = c;
+        scratch->lastBlocks = set->nstreams;
+        scratch->lastMaxLen = 0;
+    }
+    unmarkInUse(scratch);
+    return r;
+}
+
+hs_error_t hs_b200_streams_reset_async(hs_b200_stream_set_t *set, const unsigned int *d_streams, size_t count,
+                                       void *cuda_stream) {
+    if (!set || (d_streams && count > 0xffffffffu)) {
+        return HS_INVALID;
+    }
+    DeviceGuard guard(set->device);
+    const u32 n = d_streams ? (u32)count : (u32)set->nstreams;
+    if (launchStreamReset(set->d_hist, set->d_offset, d_streams, n, (u32)set->nstreams, set->d_mark, set->epoch,
+                          (cudaStream_t)cuda_stream) != cudaSuccess) {
+        return HS_UNKNOWN_ERROR;
+    }
+    g_launches += n != 0;
+    return HS_SUCCESS;
 }
 
 } /* extern "C" */

@@ -60,6 +60,7 @@ enum ConfirmKind {
 enum { MAX_PEERS = 8 };
 enum { CTR_MATCHES = 0, CTR_ERROR = 1, CTR_CANDIDATES = 2, CTR_CONFIRMED = 3,
        CTR_PREFILTER_PASS = 4, CTR_CANDQ = 5 /* candidates handed to the confirm kernel */,
+       CTR_STREAM = 6 /* a stream-set pass that did not commit: STREAM_MARKED, | STREAM_BAD_LENGTH */,
        CTR_COUNT = 8 };
 
 /* Every scan kernel stops at the prefilter and appends the surviving candidates
@@ -155,11 +156,32 @@ cudaError_t launchConfirm(const LaunchCfg &cfg, const ScanParams &p, cudaStream_
  * region in every peer's exchange buffer (runs after the scan on its stream). */
 cudaError_t launchPublishCount(const ScanParams &p, cudaStream_t stream);
 
-/* stream-set helpers: write every stream's look-behind in front of its write /
- * roll history and offsets forward after a scan */
-cudaError_t launchStreamAssemble(u8 *corpus, const u8 *hist, u32 nstreams, u32 pitch, cudaStream_t stream);
+/* A stream set's pass state in device memory.  A pass whose record ring or candidate list overflowed, or
+ * whose device lengths were bad, does not advance its streams and marks the set; every later pass or reset on
+ * a marked set commits nothing, and a later pass raises its record count above the ring, so that its ordering
+ * reports the overflow.  Marks belong to an epoch of the set: when the host has seen a mark
+ * (hs_b200_scan_corpus_finish) it moves the set to the next epoch, and the passes and resets enqueued from then
+ * on, which carry the new epoch, find the set unmarked -- the passes and resets enqueued before stay without
+ * effect however late they run, and no clear has to be ordered after them. */
+struct StreamMark {
+    u32 marked;  /* epoch + 1 of the mark, 0 = none */
+    u32 need;    /* the largest record count a pass of the mark's epoch reported: what the ring must hold */
+    u32 bad;     /* epoch + 1 of a pass with a write length above pitch - 16, 0 = none */
+    u32 pad;
+};
+enum { STREAM_MARKED = 1, STREAM_BAD_LENGTH = 2 };
+
+/* stream-set helpers, each given the set's epoch at enqueue time: write every stream's look-behind in front of
+ * its write (and, given srcLens, take the caller's device lengths into lens, a length above pitch - 16
+ * becoming 0 and marking the pass bad) / roll history and offsets forward after a scan, only if the pass may
+ * commit / end the flows of the listed streams (idx = null: all), unless the set is marked */
+cudaError_t launchStreamAssemble(u8 *corpus, const u8 *hist, u32 nstreams, u32 pitch, const u32 *srcLens,
+                                 u32 *lens, StreamMark *mark, u32 epoch, cudaStream_t stream);
 cudaError_t launchStreamAdvance(const u8 *corpus, u8 *hist, u64 *offsets, const u32 *lens, u32 uniformLen,
-                                u32 nstreams, u32 pitch, u32 histReq, cudaStream_t stream);
+                                u32 nstreams, u32 pitch, u32 histReq, u32 *counters, u32 outCap, StreamMark *mark,
+                                u32 epoch, cudaStream_t stream);
+cudaError_t launchStreamReset(u8 *hist, u64 *offsets, const u32 *idx, u32 count, u32 nstreams,
+                              const StreamMark *mark, u32 epoch, cudaStream_t stream);
 
 /* one engine of a fused launch (DfaParams.engines): its bytes in device memory and the DfaParams fields
  * that differ from engine to engine */

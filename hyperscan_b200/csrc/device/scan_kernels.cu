@@ -1694,7 +1694,8 @@ __global__ void publishCountKernel(const ScanParams p) {
 } // namespace
 
 namespace {
-__global__ void streamAssembleKernel(u8 *corpus, const u8 *hist, u32 nstreams, u32 pitch) {
+__global__ void streamAssembleKernel(u8 *corpus, const u8 *hist, u32 nstreams, u32 pitch, const u32 *srcLens,
+                                     u32 *lens, StreamMark *mark, u32 epoch) {
     const u32 b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nstreams) {
         return;
@@ -1713,11 +1714,35 @@ __global__ void streamAssembleKernel(u8 *corpus, const u8 *hist, u32 nstreams, u
     out.z = (u32)hi;
     out.w = (u32)(hi >> 32);
     *reinterpret_cast<uint4 *>(corpus + (size_t)b * pitch) = out;
+    if (srcLens) {
+        /* the scan reads the lengths from here: a bad one must not let a block reach past the buffer */
+        u32 l = srcLens[b];
+        if (l > pitch - 16) {
+            l = 0;
+            mark->bad = epoch + 1;
+        }
+        lens[b] = l;
+    }
 }
 
-__global__ void streamAdvanceKernel(const u8 *corpus, u8 *hist, u64 *offsets, const u32 *lens,
-                                    u32 uniformLen, u32 nstreams, u32 pitch, u32 histReq) {
+__global__ void streamAdvanceKernel(const u8 *corpus, u8 *hist, u64 *offsets, const u32 *lens, u32 uniformLen,
+                                    u32 nstreams, u32 pitch, u32 histReq, u32 *counters, u32 outCap,
+                                    StreamMark *mark, u32 epoch) {
     const u32 b = blockIdx.x * blockDim.x + threadIdx.x;
+    /* every thread reaches the same verdict: only thread 0 writes, and only what makes it "no" (a mark of an
+     * earlier epoch is one the host has seen: it counts as none) */
+    const u32 count = counters[CTR_MATCHES];
+    const bool marked = mark->marked == epoch + 1, bad = mark->bad == epoch + 1;
+    if (marked || bad || counters[CTR_ERROR] || count > outCap) {
+        if (b == 0) {
+            const u32 need = max(max(marked ? mark->need : 0u, count), outCap + 1);
+            mark->need = need;
+            mark->marked = epoch + 1;
+            counters[CTR_MATCHES] = need;
+            counters[CTR_STREAM] = STREAM_MARKED | (bad ? (u32)STREAM_BAD_LENGTH : 0u);
+        }
+        return;
+    }
     if (b >= nstreams) {
         return;
     }
@@ -1738,20 +1763,48 @@ __global__ void streamAdvanceKernel(const u8 *corpus, u8 *hist, u64 *offsets, co
     *reinterpret_cast<uint2 *>(hist + (size_t)b * 8) = make_uint2((u32)v, (u32)(v >> 32));
     offsets[b] += wl;
 }
+
+__global__ void streamResetKernel(u8 *hist, u64 *offsets, const u32 *idx, u32 count, u32 nstreams,
+                                  const StreamMark *mark, u32 epoch) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    /* a reset behind a pass that did not commit commits nothing either: the caller enqueues it again with the
+     * passes */
+    if (i >= count || mark->marked == epoch + 1) {
+        return;
+    }
+    const u32 b = idx ? idx[i] : i;
+    if (b >= nstreams) {
+        return;
+    }
+    *reinterpret_cast<uint2 *>(hist + (size_t)b * 8) = make_uint2(0, 0);
+    offsets[b] = 0;
+}
 } // namespace
 
-cudaError_t launchStreamAssemble(u8 *corpus, const u8 *hist, u32 nstreams, u32 pitch, cudaStream_t stream) {
+cudaError_t launchStreamAssemble(u8 *corpus, const u8 *hist, u32 nstreams, u32 pitch, const u32 *srcLens,
+                                 u32 *lens, StreamMark *mark, u32 epoch, cudaStream_t stream) {
     if (nstreams) {
-        HSB_LAUNCH(streamAssembleKernel, (nstreams + 255) / 256, 256, 0, stream, corpus, hist, nstreams, pitch);
+        HSB_LAUNCH(streamAssembleKernel, (nstreams + 255) / 256, 256, 0, stream, corpus, hist, nstreams, pitch,
+                   srcLens, lens, mark, epoch);
     }
     return cudaGetLastError();
 }
 
 cudaError_t launchStreamAdvance(const u8 *corpus, u8 *hist, u64 *offsets, const u32 *lens, u32 uniformLen,
-                                u32 nstreams, u32 pitch, u32 histReq, cudaStream_t stream) {
+                                u32 nstreams, u32 pitch, u32 histReq, u32 *counters, u32 outCap, StreamMark *mark,
+                                u32 epoch, cudaStream_t stream) {
     if (nstreams) {
         HSB_LAUNCH(streamAdvanceKernel, (nstreams + 255) / 256, 256, 0, stream, corpus, hist, offsets, lens,
-                   uniformLen, nstreams, pitch, histReq);
+                   uniformLen, nstreams, pitch, histReq, counters, outCap, mark, epoch);
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t launchStreamReset(u8 *hist, u64 *offsets, const u32 *idx, u32 count, u32 nstreams,
+                              const StreamMark *mark, u32 epoch, cudaStream_t stream) {
+    if (count) {
+        HSB_LAUNCH(streamResetKernel, (count + 255) / 256, 256, 0, stream, hist, offsets, idx, count, nstreams,
+                   mark, epoch);
     }
     return cudaGetLastError();
 }

@@ -466,6 +466,38 @@ hs_error_t hs_b200_streams_scan_collect(hs_b200_stream_set_t *set, const char *d
                                         const unsigned int *lengths, hs_scratch_t *scratch,
                                         hs_b200_match_t *out, size_t cap,
                                         unsigned long long *nmatches);
+/* A pass over writes that are already in device memory, enqueued on cuda_stream (NULL = the scratch's
+ * stream) with no host wait.  Stream i's write is at d_writes + i * pitch + 16, d_lengths[i] bytes long
+ * (device memory), or uniform_length bytes when d_lengths is NULL; length 0 = no write.  d_writes is
+ * 16-byte aligned, pitch a multiple of 16 and at least 32, every length at most pitch - 16.  The 16 bytes
+ * in front of each write belong to the library during the pass (the stream's look-behind is written
+ * there); the bytes after a write may hold anything and take part in no match.  Nothing outside
+ * [d_writes, d_writes + nstreams * pitch) is read or written.  d_writes and d_lengths stay valid until the
+ * pass completes, and all passes of one set go on one CUDA stream.
+ * The records go into the scratch's ring as for hs_b200_scan_corpus_async (block = stream index, to =
+ * stream offset), and hs_b200_scan_corpus_finish, hs_b200_fetch_matches, hs_b200_export_records_async and
+ * hs_b200_order_matches_async serve the pass; the ordered matches equal hs_b200_streams_scan_collect's.
+ * The streams advance on the device, and only when the pass's ring and candidate list did not overflow.
+ * Otherwise the streams stay as they were and the set is marked: every later pass on it commits nothing
+ * and its ordering reports HS_B200_ORDER_RING_OVERFLOW, and every later hs_b200_streams_reset_async on it
+ * commits nothing either, until hs_b200_scan_corpus_finish returns HS_INSUFFICIENT_SPACE and grows the ring
+ * (the set must still be open).  The passes and resets enqueued before that call stay without effect; those
+ * enqueued after it commit.  The caller then enqueues again, in their order, the passes and resets from the
+ * first pass whose ordering reported the overflow on.  A device length above pitch - 16 fails the pass in
+ * the same way, and finish returns HS_INVALID.  HS_INVALID at once: NULL arguments, a misaligned buffer, a
+ * bad pitch, a uniform length above pitch - 16, a scratch on another device than the set. */
+hs_error_t hs_b200_streams_scan_async(hs_b200_stream_set_t *set, void *d_writes, size_t pitch,
+                                      const unsigned int *d_lengths, unsigned int uniform_length,
+                                      hs_scratch_t *scratch, void *cuda_stream);
+/* End the flows of the `count` streams listed in d_streams (device memory; NULL = every stream): their
+ * look-behind becomes empty and their offset 0, in stream order on cuda_stream.  Indices at or above
+ * nstreams are ignored.  Nothing is delivered: a pure-literal stream database has no end-of-data reports.
+ * On a marked set (see hs_b200_streams_scan_async) the reset commits nothing and is enqueued again with the
+ * passes.  cuda_stream is the stream the set's passes run on: NULL here is the legacy default stream, which
+ * does not order against the scratch's own stream (what hs_b200_streams_scan_async takes for NULL).  Before
+ * a hs_b200_streams_scan, the caller synchronises cuda_stream. */
+hs_error_t hs_b200_streams_reset_async(hs_b200_stream_set_t *set, const unsigned int *d_streams, size_t count,
+                                       void *cuda_stream);
 size_t hs_b200_streams_state_bytes(const hs_b200_stream_set_t *set);
 hs_error_t hs_b200_streams_close(hs_b200_stream_set_t *set);
 
