@@ -593,8 +593,8 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
     const RoseEngine *r = dbRose(db);
     const u8 *bc = (const u8 *)r;
     const DbShape shape = dbShape(db);
-    if (shape == SHAPE_UNSUPPORTED) {
-        return HS_ARCH_ERROR;
+    if (shape == SHAPE_UNSUPPORTED || shape == SHAPE_MALFORMED) {
+        return shape == SHAPE_MALFORMED ? HS_INVALID : HS_ARCH_ERROR;
     }
     std::unique_ptr<DevImage, void (*)(DevImage *)> im(new (std::nothrow) DevImage(), freeImage);
     if (!im) {
@@ -1121,16 +1121,21 @@ void fillParams(const hs_scratch *s, const DevImage *im, const hs_b200_corpus *c
     }
 }
 
-/* The segment plan of the default rule (engine_segment = 0; DESIGN.md section 10f): blocks are cut only when
- * they would leave more than half of the lanes an engine launch keeps resident idle, and only blocks longer
- * than twice the segment length, which is at least SEG_MIN and otherwise as long as makes the corpus about fill
- * the resident lanes.  A segment's guess comes from SEG_WARM bytes in front of it; SEG_ROUNDS parallel
- * SEG_JOIN rounds precede the sequential SEG_SETTLE walk. */
+/* The segment plan of the default rule (engine_segment = 0; DESIGN.md section 10f): a run of `engines` engines has
+ * engines x blocks lanes of work, and blocks are cut only when that would leave more than half of the lanes the
+ * run keeps resident idle, and only blocks longer than twice the segment length.  That length is at least SEG_MIN
+ * and otherwise as long as makes engines x segments about fill the resident lanes, so that the segment states
+ * (engines x 2 x segments) stay bounded by the GPU, not by the engine count.  A segment's guess comes from
+ * SEG_WARM bytes in front of it; SEG_ROUNDS parallel SEG_JOIN rounds precede the sequential SEG_SETTLE walk.  A
+ * forced length (engine_segment = N > 0) whose segment area would pass SEG_FORCED_MAX fails the scan with
+ * HS_NOMEM. */
 enum : u32 { SEG_MIN = 4096, SEG_WARM = 256, SEG_ROUNDS = 2 };
+static const size_t SEG_FORCED_MAX = (size_t)1 << 30;
 
-/* Cut the blocks of c for an engine of `kind`?  Fills the segment table (every block, in order: a block not cut
- * is one segment with both flags) and the cut blocks {first segment, segments}; false: one lane per block. */
-bool planSegments(const hs_b200_corpus *c, u32 kind, int smCount, std::vector<DfaSeg> *segs,
+/* Cut the blocks of c for a run of `engines` engines of `kind`?  Fills the segment table (every block, in order: a
+ * block not cut is one segment with both flags) and the cut blocks {first segment, segments}; false: one lane per
+ * block. */
+bool planSegments(const hs_b200_corpus *c, u32 kind, u64 engines, int smCount, std::vector<DfaSeg> *segs,
                   std::vector<uint2> *cuts) {
     const int opt = g_opts.engineSegment;
     if (opt < 0 || c->nblocks == 0 || c->h_len.size() != c->nblocks) {
@@ -1139,10 +1144,10 @@ bool planSegments(const hs_b200_corpus *c, u32 kind, int smCount, std::vector<Df
     u64 segLen = (u64)opt, cutAbove = (u64)opt;
     if (opt == 0) {
         const u64 lanes = dfaResidentLanes(kind, smCount);
-        if ((u64)c->nblocks * 2 > lanes) {
+        if (engines * c->nblocks * 2 > lanes) {
             return false; /* the blocks alone keep half the resident lanes busy or more */
         }
-        segLen = std::max<u64>(SEG_MIN, HSB_ROUNDUP(c->payload / lanes + 1, 16));
+        segLen = std::max<u64>(SEG_MIN, HSB_ROUNDUP(c->payload * engines / lanes + 1, 16));
         cutAbove = 2 * segLen;
     }
     if (*std::max_element(c->h_len.begin(), c->h_len.end()) <= cutAbove) {
@@ -1185,7 +1190,8 @@ cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u
     initOpts();
     std::vector<DfaSeg> segs;
     std::vector<uint2> cuts;
-    if (!planSegments(c, dp.kind, smCount, &segs, &cuts)) {
+    const size_t engines = dp.engines ? dp.nengines : 1;
+    if (!planSegments(c, dp.kind, engines, smCount, &segs, &cuts)) {
         const cudaError_t e = launchDfa(dp, smCount, maxSmem, stream);
         if (e == cudaSuccess) {
             g_launches++;
@@ -1193,12 +1199,14 @@ cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u
         return e;
     }
     /* [segs][cuts][per engine, per block: first open segment][per engine: guess states, end states] */
-    const size_t engines = dp.engines ? dp.nengines : 1;
     const size_t segBytes = HSB_ROUNDUP(segs.size() * sizeof(DfaSeg), 256);
     const size_t planBytes = segBytes + cuts.size() * sizeof(uint2);
     const size_t openBytes = HSB_ROUNDUP(engines * c->nblocks * sizeof(u32), 256);
     const size_t statesAt = HSB_ROUNDUP(planBytes, 256) + openBytes;
     const size_t need = statesAt + engines * 2 * segs.size() * dfaStateBytes(dp.kind);
+    if (g_opts.engineSegment > 0 && need > SEG_FORCED_MAX) {
+        return cudaErrorMemoryAllocation; /* a forced length too short for this corpus and engine count */
+    }
     if (!seg->d_stats) {
         cudaError_t e = cudaMalloc(&seg->d_stats, SEGSTAT_COUNT * sizeof(unsigned long long));
         if (e == cudaSuccess) e = cudaMemset(seg->d_stats, 0, SEGSTAT_COUNT * sizeof(unsigned long long));

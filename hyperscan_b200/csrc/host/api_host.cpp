@@ -19,6 +19,7 @@
 
 #include "../../../include/hs_b200.h"
 #include "api_internal.h"
+#include "db_walk.h"
 #include "rose_build.h"
 #include "dfa_build.h"
 #include "limex_build.h"
@@ -401,6 +402,9 @@ hs_error_t hs_b200_db_info(const hs_database_t *db, hs_b200_db_info_t *out) {
     hs_error_t ret = validDb(db);
     if (ret != HS_SUCCESS) {
         return ret;
+    }
+    if (dbShape(db) == SHAPE_MALFORMED) {
+        return HS_INVALID; /* its engine count does not fit its tables */
     }
     memset(out, 0, sizeof(*out));
     const RoseEngine *r = dbRose(db);

@@ -5,6 +5,7 @@
 #include <cstring>
 
 #include "api_internal.h"
+#include "rose_build.h"
 
 namespace hsb {
 
@@ -392,6 +393,96 @@ void postprocessCombinations(const Combinations &cb, const std::unordered_set<u3
 
 } // namespace
 
+namespace {
+
+/* units[i] at bytes [off, off + count * sizeof(Unit)) of the bytecode, field by field */
+template <class Unit>
+bool unitsAre(const u8 *bc, u32 len, u32 off, u32 count, const std::vector<Unit> &units) {
+    if (count != units.size()) {
+        return false;
+    }
+    if (!count) {
+        return true;
+    }
+    if (off % alignof(Unit) || (u64)off + (u64)count * sizeof(Unit) > len) {
+        return false;
+    }
+    for (u32 i = 0; i < count; i++) {
+        Unit u;
+        memcpy(&u, bc + off + (size_t)i * sizeof(Unit), sizeof(u));
+        if (u.offset != units[i].offset || u.val != units[i].val) {
+            return false;
+        }
+    }
+    return true;
+}
+
+/* The tables that run a set of K = queueCount outfixes, checked against K and the bytecode length `len`: the
+ * NfaInfo table and every engine lie inside the bytecode, the engines' states tile the state and scratch areas in
+ * queue order up to their sizes, the active leaf array has K bits and the state scatter
+ * plan is its clear plan, and the EOD program is there exactly when some engine accepts at end of data, its
+ * sparse iterator over exactly those queues.  (The runtime walks these with no bound of its own.) */
+bool outfixTablesFit(const RoseEngine *r, u32 len) {
+    const u8 *bc = (const u8 *)r;
+    const u32 k = r->queueCount;
+    if (r->nfaInfoOffset % 4 || (u64)r->nfaInfoOffset + (u64)k * sizeof(NfaInfo) > len) {
+        return false;
+    }
+    const StateOffsets &so = r->stateOffsets;
+    std::vector<u32> eod;
+    u64 state = so.nfaStateBegin, full = 0; /* each queue's stream and scratch state follow the one before */
+    for (u32 q = 0; q < k; q++) {
+        NfaInfo ni;
+        memcpy(&ni, bc + r->nfaInfoOffset + (size_t)q * sizeof(NfaInfo), sizeof(ni));
+        if (ni.nfaOffset % 64 || (u64)ni.nfaOffset + sizeof(NFA) > len) {
+            return false;
+        }
+        NFA nh;
+        memcpy(&nh, bc + ni.nfaOffset, sizeof(nh));
+        if ((u64)ni.nfaOffset + nh.length > len || ni.stateOffset != state || ni.fullStateOffset != full) {
+            return false;
+        }
+        if (nh.flags & NFA_ACCEPTS_EOD) {
+            eod.push_back(q);
+        }
+        state += nh.streamStateSize;
+        full = HSB_ROUNDUP(full + nh.scratchStateSize, 64);
+    }
+    if (state != r->stateSize || full != r->scratchStateSize) {
+        return false;
+    }
+    if (so.activeLeafArray_size != mmbitSize(k) || (u64)so.activeLeafArray + so.activeLeafArray_size > r->stateSize) {
+        return false;
+    }
+    const MmbClearPlan p = mmbClearPlan(k, so.activeLeafArray);
+    const ScatterPlan &sp = r->state_init;
+    if (!unitsAre(bc, len, sp.s_u64a_offset, sp.s_u64a_count, p.u64s) ||
+        !unitsAre(bc, len, sp.s_u32_offset, sp.s_u32_count, p.u32s) ||
+        !unitsAre(bc, len, sp.s_u16_offset, sp.s_u16_count, p.u16s) ||
+        !unitsAre(bc, len, sp.s_u8_offset, sp.s_u8_count, p.u8s)) {
+        return false;
+    }
+    if (!r->eodProgramOffset || eod.empty()) {
+        return !r->eodProgramOffset && eod.empty();
+    }
+    InstrEnginesEod ee; /* (inside the bytecode: dbShape) */
+    memcpy(&ee, bc + r->eodProgramOffset, sizeof(ee));
+    const std::vector<MmbSparseIter> want = mmbSparseIterator(eod, k);
+    if (ee.iter_offset % alignof(MmbSparseIter) || (u64)ee.iter_offset + want.size() * sizeof(MmbSparseIter) > len) {
+        return false;
+    }
+    for (size_t i = 0; i < want.size(); i++) {
+        MmbSparseIter it;
+        memcpy(&it, bc + ee.iter_offset + i * sizeof(MmbSparseIter), sizeof(it));
+        if (it.mask != want[i].mask || it.val != want[i].val) {
+            return false;
+        }
+    }
+    return true;
+}
+
+} // namespace
+
 DbShape dbShape(const hs_database_t *db) {
     const DbHeader *h = (const DbHeader *)db;
     const RoseEngine *r = dbRose(db);
@@ -405,12 +496,11 @@ DbShape dbShape(const hs_database_t *db) {
         return SHAPE_SOLE_OUTFIX;
     }
     /* the FULL_ROSE shapes run here: outfixes on queues [0, K) only, beside the floating literal matcher,
-     * whose role-less programs report directly (one outfix, DESIGN.md section 10d), or alone (up to
-     * MAX_OUTFIX_QUEUES, section 10e) -- no anchored, EOD or small-block matcher, no roles, leftfixes,
-     * suffixes, delayed literals, MPV, SOM or long-literal table, and an EOD program that at most checks
-     * the engines' EOD accepts */
+     * whose role-less programs report directly (one outfix, DESIGN.md section 10d), or alone (any K, section
+     * 10e) -- no anchored, EOD or small-block matcher, no roles, leftfixes, suffixes, delayed literals, MPV, SOM
+     * or long-literal table, and an EOD program that at most checks the engines' EOD accepts */
     const u32 k = r->queueCount;
-    if (r->runtimeImpl == RUNTIME_FULL_ROSE && r->mode == MODE_BLOCK && (r->fmatcherOffset ? k == 1 : k <= MAX_OUTFIX_QUEUES) &&
+    if (r->runtimeImpl == RUNTIME_FULL_ROSE && r->mode == MODE_BLOCK && (!r->fmatcherOffset || k == 1) &&
         !r->amatcherOffset && !r->ematcherOffset && !r->sbmatcherOffset && !r->drmatcherOffset && k >= 1 &&
         r->activeArrayCount == k && r->outfixBeginQueue == 0 && r->outfixEndQueue == k &&
         r->leftfixBeginQueue == k && r->nfaInfoOffset && !r->activeLeftCount && !r->rosePrefixCount &&
@@ -422,7 +512,10 @@ DbShape dbShape(const hs_database_t *db) {
          ((size_t)r->eodProgramOffset + 16 <= h->length && r->eodProgramOffset % INSTR_ALIGN == 0 &&
           bc[r->eodProgramOffset] == OP_ENGINES_EOD &&
           bc[r->eodProgramOffset + HSB_ROUNDUP(sizeof(InstrEnginesEod), INSTR_ALIGN)] == OP_END))) {
-        return r->fmatcherOffset ? SHAPE_LITERALS_OUTFIX : SHAPE_OUTFIXES;
+        if (r->fmatcherOffset) {
+            return SHAPE_LITERALS_OUTFIX;
+        }
+        return outfixTablesFit(r, h->length) ? SHAPE_OUTFIXES : SHAPE_MALFORMED;
     }
     return SHAPE_UNSUPPORTED;
 }
@@ -430,8 +523,8 @@ DbShape dbShape(const hs_database_t *db) {
 hs_error_t loadReportRules(const hs_database_t *db, ReportRules *rules, std::vector<LitTail> *tails) {
     const RoseEngine *r = dbRose(db);
     rules->shape = dbShape(db);
-    if (rules->shape == SHAPE_UNSUPPORTED) {
-        return HS_ARCH_ERROR;
+    if (rules->shape == SHAPE_UNSUPPORTED || rules->shape == SHAPE_MALFORMED) {
+        return rules->shape == SHAPE_MALFORMED ? HS_INVALID : HS_ARCH_ERROR;
     }
     rules->bc = (const u8 *)r;
     rules->bcLen = ((const DbHeader *)db)->length;

@@ -77,7 +77,9 @@ enum DbShape {
     SHAPE_PURE_LITERAL,    /* the floating literal matcher alone */
     SHAPE_SOLE_OUTFIX,     /* one engine over the whole block, no literal matcher */
     SHAPE_LITERALS_OUTFIX, /* the floating literal matcher beside one outfix (FULL_ROSE, block mode) */
-    SHAPE_OUTFIXES,        /* up to MAX_OUTFIX_QUEUES outfixes and no literal matcher (FULL_ROSE, block mode) */
+    SHAPE_OUTFIXES,        /* any number of outfixes and no literal matcher (FULL_ROSE, block mode) */
+    SHAPE_MALFORMED,       /* the header of SHAPE_OUTFIXES, but its queue, state or EOD tables do not fit its queue
+                            * count or its bytecode: refused with HS_INVALID */
 };
 DbShape dbShape(const hs_database_t *db);
 

@@ -33,9 +33,87 @@
 #include <map>
 #include <tuple>
 #include <set>
+#include <type_traits>
 #include <stdexcept>
 
 namespace hsb {
+
+/* mmbit_keyshift (src/util/multibit.h:182-186): the shift of the root level's keys, the least multiple of 6 with
+ * 64 << ks >= totalBits */
+static u32 mmbKeyShift(u32 totalBits) {
+    u32 ks = 0;
+    while ((64ull << ks) < totalBits) {
+        ks += 6;
+    }
+    return ks;
+}
+
+std::vector<MmbSparseIter> mmbSparseIterator(const std::vector<u32> &keys, u32 totalBits) {
+    /* level by level from the root, the records of the nodes that hold a key in key order (the breadth-first
+     * layout); a node at shift s is key >> (s + 6), its bit (key >> s) & 63 */
+    std::vector<std::vector<MmbSparseIter>> levels;
+    for (s32 s = (s32)mmbKeyShift(totalBits); s >= 0; s -= 6) {
+        std::vector<MmbSparseIter> lv;
+        u64 node = 0;
+        for (u32 key : keys) {
+            if (lv.empty() || (u64)key >> (s + 6) != node) {
+                node = (u64)key >> (s + 6);
+                MmbSparseIter rec;
+                memset(&rec, 0, sizeof(rec));
+                lv.push_back(rec);
+            }
+            lv.back().mask |= 1ull << ((key >> s) & 63);
+        }
+        levels.push_back(lv);
+    }
+    /* val: above the last level, where the record's children start (the next level's start plus the keys of the
+     * records before it on its level); on the last level, the keys of the records before it there */
+    std::vector<MmbSparseIter> out;
+    u32 next = 0;
+    for (size_t l = 0; l < levels.size(); l++) {
+        next += (u32)levels[l].size();
+        u32 before = l + 1 < levels.size() ? next : 0;
+        for (MmbSparseIter &rec : levels[l]) {
+            rec.val = before;
+            before += (u32)__builtin_popcountll(rec.mask);
+            out.push_back(rec);
+        }
+    }
+    return out;
+}
+
+MmbClearPlan mmbClearPlan(u32 totalBits, u32 at) {
+    MmbClearPlan p;
+    auto unit = [](auto *v, u32 offset) {
+        typename std::remove_reference<decltype(*v)>::type::value_type u;
+        memset(&u, 0, sizeof(u));
+        u.offset = offset;
+        v->push_back(u);
+    };
+    if (totalBits > 256) {
+        unit(&p.u64s, at); /* the tree: clearing its root clears it */
+        return p;
+    }
+    u32 bits = totalBits;
+    for (; bits > 64; bits -= 64, at += 8) {
+        unit(&p.u64s, at);
+    }
+    /* the last word of 1-64 bits */
+    if (bits > 56) {
+        unit(&p.u64s, at);
+        return p;
+    }
+    if (bits > 24) {
+        unit(&p.u32s, at);
+    }
+    if ((bits > 8 && bits <= 24) || bits > 40) {
+        unit(&p.u16s, bits > 24 ? at + 4 : at);
+    }
+    if (bits <= 8 || (bits > 16 && bits <= 24) || (bits > 32 && bits <= 40) || bits > 48) {
+        unit(&p.u8s, bits <= 8 ? at : bits <= 24 ? at + 2 : bits <= 40 ? at + 4 : at + 6);
+    }
+    return p;
+}
 
 namespace {
 
@@ -351,20 +429,20 @@ std::vector<std::pair<u32, NFA>> addEngines(Blob &blob, const std::vector<std::v
 }
 
 /* makeEodProgram (rose_build_bytecode.cpp:3334-3350) with only addEnginesEodProgram: when some engine accepts
- * at end of data, ENGINES_EOD over a sparse iterator of those queues (buildEodNfaIterator, :2276-2294; with
- * at most 64 queues the iterator is one record) and END; requiresEodCheck (hasEodAnchors, :2446-2475). */
+ * at end of data, ENGINES_EOD over a sparse iterator of those queues (buildEodNfaIterator, :2276-2294) and END;
+ * requiresEodCheck (hasEodAnchors, :2446-2475). */
 void addEnginesEodProgram(Blob &blob, RoseEngine *r, const std::vector<std::pair<u32, NFA>> &engines) {
-    u64 eodQueues = 0;
+    std::vector<u32> eodQueues;
     for (u32 q = 0; q < engines.size(); q++) {
         if (engines[q].second.flags & NFA_ACCEPTS_EOD) {
-            eodQueues |= 1ull << q;
+            eodQueues.push_back(q);
         }
     }
-    if (!eodQueues) {
+    if (eodQueues.empty()) {
         return;
     }
-    const MmbSparseIter it = {eodQueues, 0};
-    const u32 iter = blob.add(&it, sizeof(it), alignof(MmbSparseIter));
+    const std::vector<MmbSparseIter> it = mmbSparseIterator(eodQueues, (u32)engines.size());
+    const u32 iter = blob.add(it.data(), it.size() * sizeof(MmbSparseIter), alignof(MmbSparseIter));
     const u32 prog = blob.reserve(instrSize<InstrEnginesEod>() + instrSize<InstrEnd>(), INSTR_ALIGN);
     InstrEnginesEod ee;
     memset(&ee, 0, sizeof(ee));
@@ -377,34 +455,22 @@ void addEnginesEodProgram(Blob &blob, RoseEngine *r, const std::vector<std::pair
 }
 
 /* The state scatter plan of a block-mode database without roles or leftfixes (buildStateScatterPlan,
- * rose_build_scatter.cpp:66-97): the units that clear the active leaf array of `leaves` <= 64 bits, as the
- * flat multibit's clear plan splits them (mmbBuildInitRangePlan, src/util/multibit_build.cpp:216-253), in
- * the order write_out lays them out (u64, u32, u16, u8). */
+ * rose_build_scatter.cpp:66-97): the clear plan of the active leaf array of `leaves` bits, its units laid out
+ * as write_out lays them out (u64, u32, u16, u8). */
 void addStateScatterPlan(Blob &blob, RoseEngine *r, u32 leaves) {
-    const u32 at = r->stateOffsets.activeLeafArray;
+    const MmbClearPlan p = mmbClearPlan(leaves, r->stateOffsets.activeLeafArray);
     ScatterPlan &sp = r->state_init;
-    auto wide = [&](u32 bits, u32 lo) { return leaves > lo && leaves <= bits; };
-    if (leaves > 56) {
-        const ScatterUnitU64 u = {at, 0};
-        sp.s_u64a_offset = blob.add(&u, sizeof(u), alignof(ScatterUnitU64));
-        sp.s_u64a_count = 1;
-        return;
-    }
-    if (leaves > 24) {
-        const ScatterUnitU32 u = {at, 0};
-        sp.s_u32_offset = blob.add(&u, sizeof(u), alignof(ScatterUnitU32));
-        sp.s_u32_count = 1;
-    }
-    if (wide(16, 8) || wide(24, 16) || wide(48, 40) || wide(56, 48)) {
-        const ScatterUnitU16 u = {leaves > 24 ? at + 4 : at, 0};
-        sp.s_u16_offset = blob.add(&u, sizeof(u), alignof(ScatterUnitU16));
-        sp.s_u16_count = 1;
-    }
-    if (leaves <= 8 || wide(24, 16) || wide(40, 32) || wide(56, 48)) {
-        const ScatterUnitU8 u = {leaves <= 8 ? at : leaves <= 24 ? at + 2 : leaves <= 40 ? at + 4 : at + 6, 0};
-        sp.s_u8_offset = blob.add(&u, sizeof(u), alignof(ScatterUnitU8));
-        sp.s_u8_count = 1;
-    }
+    auto add = [&](const auto &units, u32 *offset, u32 *count) {
+        if (!units.empty()) {
+            typedef typename std::remove_reference<decltype(units)>::type::value_type Unit;
+            *offset = blob.add(units.data(), units.size() * sizeof(Unit), alignof(Unit));
+            *count = (u32)units.size();
+        }
+    };
+    add(p.u64s, &sp.s_u64a_offset, &sp.s_u64a_count);
+    add(p.u32s, &sp.s_u32_offset, &sp.s_u32_count);
+    add(p.u16s, &sp.s_u16_offset, &sp.s_u16_count);
+    add(p.u8s, &sp.s_u8_offset, &sp.s_u8_count);
 }
 
 /* header + blob, the header's size field set */
@@ -1112,10 +1178,6 @@ std::vector<u8> buildMultiOutfixRose(const std::vector<RegexPattern> &pats, cons
     std::map<u32, u32> ekeys, dkeys;
     const bool allHighlander = assignRegexKeys(pats, &highlander, &ekeys, &dkeys);
     const std::vector<std::vector<RegexPattern>> groups = packEngineGroups(pats);
-    if (groups.size() > MAX_OUTFIX_QUEUES) {
-        throw CompileError{"Pattern set is too large: it needs more than " + std::to_string(MAX_OUTFIX_QUEUES) +
-                               " engines.", -1};
-    }
     Blob blob((u32)HSB_ROUNDUP(sizeof(RoseEngine), 64));
     std::vector<std::vector<u8>> engines;
     u32 minLen = ~0u;

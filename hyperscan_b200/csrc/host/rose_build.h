@@ -5,7 +5,7 @@
  * (src/rose/rose_build_bytecode.cpp:3609-3888, src/compiler/compiler.cpp:476-
  * 536), restricted to databases whose runtimeImpl is ROSE_RUNTIME_PURE_LITERAL,
  * ROSE_RUNTIME_SINGLE_OUTFIX, or ROSE_RUNTIME_FULL_ROSE with only the floating
- * literal matcher and one outfix.
+ * literal matcher and one outfix, or with any number of outfixes and no literal matcher.
  */
 #ifndef HSB200_ROSE_BUILD_H
 #define HSB200_ROSE_BUILD_H
@@ -87,10 +87,26 @@ std::vector<u8> buildMixedRose(const std::vector<LitPattern> &lits, const std::v
 
 /** Expressions too many for one engine (ROSE_RUNTIME_FULL_ROSE without a literal matcher): the
  * expressions packed greedily, in order, into groups whose automaton fits one engine, and each group's
- * engine (McClellan-8 / 16 or LimEx, as buildRegexRose picks it) as the outfix on its own queue, at most
- * MAX_OUTFIX_QUEUES.  Report ids share their exhaustion and dedupe keys across all engines.  Block mode
- * only; no logical combinations.  Throws CompileError, also when one expression alone does not fit. */
+ * engine (McClellan-8 / 16 or LimEx, as buildRegexRose picks it) as the outfix on its own queue, as many
+ * queues as there are groups.  Report ids share their exhaustion and dedupe keys across all engines.  Block
+ * mode only; no logical combinations.  Throws CompileError, also when one expression alone does not fit. */
 std::vector<u8> buildMultiOutfixRose(const std::vector<RegexPattern> &pats, const CompileOpts &opts);
+
+/** The sparse iterator over `keys` (ascending, each < totalBits) of a multibit of totalBits bits, as
+ * mmbBuildSparseIterator lays it out (src/util/multibit_build.cpp:158-206): one record per node of the key
+ * tree that holds a key, breadth first; one record while totalBits <= 64. */
+std::vector<MmbSparseIter> mmbSparseIterator(const std::vector<u32> &keys, u32 totalBits);
+
+/** The scatter units that clear a multibit of totalBits bits at state offset `at` (mmbBuildClearPlan,
+ * src/util/multibit_build.cpp:208-325): the flat form (<= 256 bits) as 64-bit words and a last word of 1-64
+ * bits split into u64 / u32 / u16 / u8 units; the tree form (> 256 bits) as its root word. */
+struct MmbClearPlan {
+    std::vector<ScatterUnitU64> u64s;
+    std::vector<ScatterUnitU32> u32s;
+    std::vector<ScatterUnitU16> u16s;
+    std::vector<ScatterUnitU8> u8s;
+};
+MmbClearPlan mmbClearPlan(u32 totalBits, u32 at);
 
 /** Test hook: pure-literal block database from raw literal programs (`area`
  * is placed at programAreaBase(); lits[i].id = its program's offset in area). */

@@ -375,10 +375,6 @@ struct ScatterUnitU32 { u32 offset; u32 val; };
 struct ScatterUnitU16 { u32 offset; u16 val; };
 struct ScatterUnitU8 { u32 offset; u8 val; };
 
-/* Not a reference limit: the most outfix queues a database built and run here has.  Up to 64, the active
- * leaf array is one flat multibit word and a sparse iterator over it is one record. */
-static const u32 MAX_OUTFIX_QUEUES = 64;
-
 /* ---- logical combinations: src/util/logical.h:42-72 -------------------- */
 
 static const u32 INVALID_LKEY = 0xffffffffu;

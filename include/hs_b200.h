@@ -515,6 +515,8 @@ typedef struct hs_b200_db_info {
     unsigned int engine_count;   /* engines run as outfixes (RoseEngine.queueCount): 0 for a pure-literal database,
                                   * 1 beside or without a literal matcher, K for a set split over K engines */
 } hs_b200_db_info_t;
+/* HS_INVALID also for a database of several outfixes whose queue table, state scatter plan or EOD iterator
+ * does not fit its engine count or its bytecode (such a database is refused at scratch allocation too). */
 hs_error_t hs_b200_db_info(const hs_database_t *db, hs_b200_db_info_t *info);
 
 /* Process-wide build tunable (the analogue of the reference tools' -G Grey
@@ -649,9 +651,11 @@ hs_error_t hs_b200_test_compile_programs(const char *const *lits, const size_t *
  * always), "dfa_ilp" (DFA kernels: blocks per lane, 1) and "engine_segment"
  * (engine runs of regular-expression databases and hs_b200_nfa_scan_corpus: 0 = cut
  * blocks longer than twice the segment length into segments walked by lanes of their
- * own when the blocks alone leave more than half of the resident lanes idle; N > 0 =
- * cut every block longer than N bytes into N-byte segments; -1 = never cut, one lane
- * per block.  The matches are the same in every setting; DESIGN.md section 10f).
+ * own when the blocks, times the engines of the run, leave more than half of the
+ * resident lanes idle; N > 0 = cut every block longer than N bytes into N-byte
+ * segments, and a scan whose segment area (engines x segments x two states, with the
+ * plan) would pass 1 GiB fails with HS_NOMEM; -1 = never cut, one lane per block.  The
+ * matches are the same in every setting; DESIGN.md section 10f).
  * "gram" applies to scratches allocated afterwards.  The defaults are the measured
  * best (DESIGN.md section 3); the others exist for A/B runs (tools/sweep.py) and tests.
  * Any other key: HS_INVALID. */
