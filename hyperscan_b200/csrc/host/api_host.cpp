@@ -822,6 +822,9 @@ static std::vector<std::string> regexToLiterals(const char *re, unsigned flags, 
 static hs_error_t exprInfo(const char *expression, unsigned flags, const hs_expr_ext_t *ext,
                            hs_expr_info_t **info, hs_compile_error_t **error);
 
+/* src/compiler/compiler.cpp:191-195 */
+static const char PREFILTER_SOM[] = "HS_FLAG_PREFILTER is not supported in combination with HS_FLAG_SOM_LEFTMOST.";
+
 /* What a combination may name (validateSubIDs, src/parser/logical_combination.cpp:116-159): the
  * first expression with each named id is an ordinary one, without SOM or PREFILTER, whose matches
  * arrive in order. */
@@ -975,6 +978,9 @@ static hs_error_t compileCommon(const char *const *expressions,
             if ((f & HS_FLAG_SINGLEMATCH) && (f & HS_FLAG_SOM_LEFTMOST)) {
                 throw CompileError{"HS_FLAG_SINGLEMATCH is not supported in "
                                    "combination with HS_FLAG_SOM_LEFTMOST.", (int)i};
+            }
+            if ((f & HS_FLAG_PREFILTER) && (f & HS_FLAG_SOM_LEFTMOST) && !litApi) {
+                throw CompileError{PREFILTER_SOM, (int)i};
             }
             if (!litApi && (f & HS_FLAG_UTF8) && !validUtf8(expressions[i], strlen(expressions[i]))) {
                 throw CompileError{"Expression is not valid UTF-8.", (int)i};
@@ -1231,6 +1237,9 @@ static hs_error_t exprInfo(const char *expression, unsigned flags, const hs_expr
         if ((flags & HS_FLAG_UTF8) && !validUtf8(expression, strlen(expression))) {
             throw CompileError{"Expression is not valid UTF-8.", 0};
         }
+        if ((flags & HS_FLAG_PREFILTER) && (flags & HS_FLAG_SOM_LEFTMOST)) {
+            throw CompileError{PREFILTER_SOM, 0};
+        }
         if (ext && ext->flags != 0) {
             if (ext->flags & ~(HS_EXT_FLAG_MIN_OFFSET | HS_EXT_FLAG_MAX_OFFSET | HS_EXT_FLAG_MIN_LENGTH |
                                HS_EXT_FLAG_EDIT_DISTANCE | HS_EXT_FLAG_HAMMING_DISTANCE)) {
@@ -1263,7 +1272,8 @@ static hs_error_t exprInfo(const char *expression, unsigned flags, const hs_expr
                 throw;
             }
             try { /* not a finite set of literals: the NFA route's parser knows the widths */
-                ri = regexInfo(expression, flags, true);
+                ri = regexInfo(expression, flags, true,
+                               ext && (ext->flags & HS_EXT_FLAG_MIN_LENGTH) ? ext->min_length : 0);
                 minW = ri.minLen;
                 maxW = ri.maxLen; /* 0xffffffff = unbounded, as in the reference (src/hs.cpp:398-403) */
             } catch (const RegexError &re) {
@@ -1276,7 +1286,7 @@ static hs_error_t exprInfo(const char *expression, unsigned flags, const hs_expr
             return HS_COMPILER_ERROR;
         }
         memset(out, 0, sizeof(*out));
-        if (ext && (ext->flags & HS_EXT_FLAG_MIN_LENGTH) && ext->min_length <= 0xfffffffeull) {
+        if (ext && (ext->flags & HS_EXT_FLAG_MIN_LENGTH) && ext->min_length <= 0xfffffffeull && !ri.minLengthDropped) {
             /* a min_length is a lower bound for the match width (checkVertex, src/nfagraph/ng_expr_info.cpp:104-109) */
             minW = std::max<size_t>(minW, (size_t)ext->min_length);
             maxW = std::max<size_t>(maxW, (size_t)ext->min_length);

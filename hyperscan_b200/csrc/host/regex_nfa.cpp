@@ -6,6 +6,7 @@
 #include <cstring>
 #include <map>
 #include <memory>
+#include <tuple>
 
 #include "../../../include/hs_b200.h"
 
@@ -19,6 +20,9 @@ struct Node {
     enum Kind { CLASS, CAT, ALT, STAR, PLUS, OPT, EMPTY, ASSERT } kind = EMPTY;
     int assertKind = 0;    /* ASSERT: one of the A_* bits below */
     bool unit = false;     /* the byte automaton of one UTF-8 character set: never split into top-level arms */
+    unsigned ref = 0;      /* EMPTY standing for a back-reference (HS_FLAG_PREFILTER) to this group number ... */
+    std::string refName;   /* ... or to this group name, until Parser::resolve replaces it */
+    bool caseless = false; /* that back-reference is under HS_FLAG_CASELESS */
     CharSet cls;
     std::vector<std::shared_ptr<Node>> kids;
 };
@@ -223,10 +227,21 @@ bool validUtf8(const char *s, size_t len) {
 
 namespace {
 
+/* HS_FLAG_PREFILTER: a bounded repeat the size reduction may widen, in parse order */
+struct Repeat {
+    size_t positions; /* what its copies contribute */
+    unsigned lo;
+};
+
 class Parser {
 public:
-    Parser(const char *re_in, unsigned flags_in)
-        : re(re_in), n(strlen(re_in)), flags(flags_in), utf8(flags_in & HS_FLAG_UTF8) {}
+    /* widen (HS_FLAG_PREFILTER): per Repeat in parse order, -1 or the m' that x{m,n} becomes x{m',} with */
+    Parser(const char *re_in, unsigned flags_in, const std::vector<long> *widen_in = nullptr)
+        : re(re_in), n(strlen(re_in)), flags(flags_in), utf8(flags_in & HS_FLAG_UTF8),
+          prefilter(flags_in & HS_FLAG_PREFILTER), widen(widen_in) {}
+
+    std::vector<Repeat> repeats; /* HS_FLAG_PREFILTER: the repeats the reduction may widen */
+    bool overflow = false;       /* HS_FLAG_PREFILTER: unrolling stopped early, the tree is too large */
 
     NodeP parse() {
         if (flags & HS_FLAG_UCP) {
@@ -243,6 +258,18 @@ public:
         if (pos != n) {
             fail("Unmatched parentheses.");
         }
+        /* references are checked once every group is known, as the reference's checkReferences does */
+        for (unsigned c : condNums) {
+            if (c >= groups) {
+                fail("Invalid conditional reference to expression " + std::to_string(c) + ".");
+            }
+        }
+        for (const std::string &c : condNames) {
+            if (c != "DEFINE" && !names.count(c)) {
+                fail("Invalid conditional reference to label '" + c + "'.");
+            }
+        }
+        resolve(r);
         /* anchors only where the reference takes them (ComponentBoundary::checkEmbeddedStartAnchor / EndAnchor,
          * src/parser/ComponentBoundary.cpp:162-185, and the callers' rules in ComponentSequence / Alternation / Repeat) */
         embeddedStart(r, true);
@@ -255,8 +282,247 @@ private:
     size_t n, pos = 0;
     unsigned flags;
     const bool utf8;      /* HS_FLAG_UTF8: characters are code points, encoded in 1 to 4 bytes */
+    const bool prefilter; /* HS_FLAG_PREFILTER: back-references, look-around, atomic and conditional groups and
+                           * possessive quantifiers are rewritten into a superset (src/parser/prefilter.cpp) */
+    const std::vector<long> *widen;
     size_t unrolled = 0;  /* positions made by unrolling bounded repeats so far */
     bool quoting = false; /* between \\Q and \\E: every byte is a literal */
+    unsigned groups = 1;  /* the number the next capturing group gets */
+    std::vector<NodeP> referent = {nullptr}; /* per group: a copy of it when it is one position, else null */
+    std::map<std::string, unsigned> names;   /* named groups */
+    size_t refsSeen = 0;  /* back-references and conditionals so far: a group with one is no safe referent */
+    std::vector<unsigned> condNums;
+    std::vector<std::string> condNames;
+
+    /* a back-reference becomes a copy of its group when that group is a single character position
+     * (MAX_REFERENT_POSITIONS = 1 in the reference), else any byte sequence -- the reference's ".*" with DOTALL,
+     * which under HS_FLAG_UTF8 is any sequence of whole characters.  Unlike the reference, a group that is one
+     * assertion (its copy would assert again where PCRE asserts nothing) is no referent, and a copy under
+     * HS_FLAG_CASELESS at the reference is folded (PCRE then compares the text caselessly), so the result is
+     * always a superset. */
+    void resolve(NodeP &x) {
+        if (x->kind == Node::EMPTY && (x->ref || !x->refName.empty())) {
+            unsigned g = x->ref;
+            if (g && g >= groups) {
+                fail("Invalid back reference to expression " + std::to_string(g) + ".");
+            }
+            if (!g) {
+                const auto it = names.find(x->refName);
+                if (it == names.end()) {
+                    fail("Invalid back reference to label '" + x->refName + "'.");
+                }
+                g = it->second;
+            }
+            if (referent[g]) {
+                NodeP copy = clone(referent[g]);
+                if (x->caseless) {
+                    foldTree(copy);
+                }
+                x = copy;
+            } else {
+                CharSet any;
+                x = repeat(leaf(any.set()), 0, -1);
+            }
+            return;
+        }
+        for (NodeP &k : x->kids) {
+            resolve(k);
+        }
+    }
+
+    void foldTree(const NodeP &x) {
+        const unsigned saved = flags;
+        flags |= HS_FLAG_CASELESS;
+        if (x->kind == Node::CLASS) {
+            x->cls = fold(x->cls);
+        }
+        for (const NodeP &k : x->kids) {
+            foldTree(k);
+        }
+        flags = saved;
+    }
+
+    NodeP backRef(unsigned g, const std::string &name = std::string()) {
+        refsSeen++;
+        NodeP b = mk(Node::EMPTY);
+        b->ref = g;
+        b->refName = name;
+        b->caseless = flags & HS_FLAG_CASELESS;
+        return b;
+    }
+
+    /* [A-Za-z0-9_]+ and then `term` at pos (pos moves past the terminator); false and pos unchanged if not */
+    bool readName(char term, std::string *out) {
+        size_t q = pos;
+        while (q < n && (isalnum((unsigned char)re[q]) || re[q] == '_')) q++;
+        if (q == pos || q >= n || re[q] != term) {
+            return false;
+        }
+        out->assign(re + pos, q - pos);
+        pos = q + 1;
+        return true;
+    }
+
+    /* up to three decimal digits at pos */
+    bool readNumber(unsigned *v) {
+        size_t q = pos;
+        unsigned x = 0;
+        while (q < n && q < pos + 3 && isdigit((unsigned char)re[q])) x = x * 10 + (unsigned)(re[q++] - '0');
+        if (q == pos) {
+            return false;
+        }
+        pos = q;
+        *v = x;
+        return true;
+    }
+
+    /* HS_FLAG_PREFILTER, an escape at pos that is a back-reference (\\1..\\99 as PCRE reads them, \\g, \\k) or
+     * \\X: its node; null (pos unchanged) for every other escape */
+    NodeP prefilterEscape() {
+        const size_t at0 = pos;
+        const char e = re[pos + 1];
+        if (e == 'X') { /* an extended grapheme cluster: one or more of any character */
+            pos += 2;
+            CharSet any;
+            return repeat(utf8 ? unit({{0, MAX_UNICODE}}) : leaf(any.set()), 1, -1);
+        }
+        if (e >= '1' && e <= '9') {
+            size_t q = pos + 1;
+            u64 v = 0;
+            while (q < n && isdigit((unsigned char)re[q])) v = std::min<u64>(v * 10 + (u64)(re[q++] - '0'), 1u << 20);
+            if (q == pos + 2) { /* one digit: \\1..\\7 refer to a group, forward ones too; \\8 \\9 are not read here */
+                if (e > '7') {
+                    return nullptr;
+                }
+                pos = q;
+                return backRef((unsigned)v);
+            }
+            if (v < groups) {
+                pos = q;
+                return backRef((unsigned)v);
+            }
+            /* not that many groups yet: up to three octal digits, then literal digits */
+            pos++;
+            u32 oct = 0;
+            int digits = 0;
+            while (digits < 3 && pos < q && re[pos] <= '7') oct = oct * 8 + (u32)(re[pos++] - '0'), digits++;
+            NodeP s = mk(Node::CAT);
+            auto lit = [&](u32 c) {
+                CharSet one;
+                one[c & 0xff] = true;
+                s->kids.push_back(utf8 ? unit(foldU(c, c)) : leaf(fold(one)));
+            };
+            if (digits) lit(oct);
+            while (pos < q) lit((u32)re[pos++]);
+            return s;
+        }
+        std::string name;
+        unsigned v = 0;
+        if (e == 'g') {
+            pos += 2;
+            const bool brace = at('{');
+            if (brace) pos++;
+            const bool neg = at('-');
+            if (neg) pos++;
+            const size_t digits = pos;
+            if (readNumber(&v) && (!brace || at('}'))) {
+                pos += brace;
+                if (v == 0) {
+                    fail("Numbered reference cannot be zero.");
+                }
+                if (neg) {
+                    if (v >= groups) {
+                        fail("Invalid reference.");
+                    }
+                    v = groups - v;
+                }
+                return backRef(v);
+            }
+            pos = digits; /* \\g{name}: the name may begin with digits, as "12abc" */
+            if (brace && !neg && readName('}', &name)) {
+                return backRef(0, name);
+            }
+            pos = at0;
+            fail("Invalid reference after \\g.");
+        }
+        if (e == 'k' && pos + 2 < n && strchr("<'{", re[pos + 2])) {
+            pos += 3;
+            const char open = re[pos - 1];
+            if (readName(open == '<' ? '>' : open == '{' ? '}' : '\'', &name)) {
+                return backRef(0, name);
+            }
+            pos = at0;
+        }
+        return nullptr;
+    }
+
+    /* HS_FLAG_PREFILTER, "(?(" at pos: a conditional group becomes the alternation of its branches (one branch
+     * only: that branch or nothing) */
+    NodeP conditional(unsigned saved) {
+        pos += 2;
+        refsSeen++;
+        if (at('R') && pos + 1 < n && (isdigit((unsigned char)re[pos + 1]) || re[pos + 1] == '&' || re[pos + 1] == ')')) {
+            fail("Pattern recursion not supported.");
+        }
+        std::string name;
+        unsigned v = 0;
+        bool define = false;
+        if (isdigit((unsigned char)re[pos])) {
+            size_t q = pos;
+            while (q < n && isdigit((unsigned char)re[q])) v = std::min(v * 10 + (unsigned)(re[q++] - '0'), 1u << 20);
+            if (q >= n || re[q] != ')') {
+                fail("Conditional subpattern unsupported.");
+            }
+            if (v == 0) {
+                fail("Numbered reference cannot be zero.");
+            }
+            pos = q + 1;
+            condNums.push_back(v);
+        } else if (at('?') && pos + 1 < n && (strchr("=!", re[pos + 1]) || (re[pos + 1] == '<' && pos + 2 < n && strchr("=!", re[pos + 2])))) {
+            pos += re[pos + 1] == '<' ? 3 : 2; /* an assertion as the condition: it asserts nothing here */
+            alt();
+            if (!at(')')) {
+                fail("Missing close parenthesis.");
+            }
+            pos++;
+        } else {
+            /* (?(<name>)...), (?('name')...), (?(name)...) */
+            const char open = re[pos];
+            const char close = open == '<' ? '>' : open == '\'' ? '\'' : ')';
+            if (close != ')') pos++;
+            if (!readName(close, &name) || (close != ')' && !at(')'))) {
+                fail("Conditional subpattern unsupported.");
+            }
+            if (close != ')') pos++;
+            define = name == "DEFINE";
+            condNames.push_back(name);
+        }
+        std::vector<NodeP> arms = {seq()};
+        while (at('|')) {
+            pos++;
+            arms.push_back(seq());
+        }
+        if (arms.size() > 2) {
+            fail("Conditional with more than two branches.");
+        }
+        if (define && arms.size() == 2) {
+            fail("DEFINE conditional group with more than one branch.");
+        }
+        if (!at(')')) {
+            fail("Missing close parenthesis.");
+        }
+        pos++;
+        flags = saved;
+        if (arms.size() == 1 && arms[0]->kids.empty()) {
+            return mk(Node::EMPTY);
+        }
+        if (arms.size() == 1) {
+            arms.push_back(mk(Node::CAT));
+        }
+        NodeP a = mk(Node::ALT);
+        a->kids = arms;
+        return a;
+    }
 
     [[noreturn]] void fail(const std::string &m) const { throw RegexError{m}; }
     bool at(char c) const { return pos < n && re[pos] == c; }
@@ -648,6 +914,16 @@ private:
         return false;
     }
 
+    static bool hasAssert(const NodeP &x) {
+        if (x->kind == Node::ASSERT) {
+            return true;
+        }
+        for (const NodeP &k : x->kids) {
+            if (hasAssert(k)) return true;
+        }
+        return false;
+    }
+
     static size_t leaves(const NodeP &x) {
         size_t c = x->kind == Node::CLASS || x->kind == Node::ASSERT;
         for (const NodeP &k : x->kids) {
@@ -657,9 +933,24 @@ private:
     }
 
     NodeP repeat(const NodeP &a, unsigned lo, long hi /* -1 = unbounded */) {
+        const size_t copies = hi < 0 ? std::max<size_t>(lo, 1) : (size_t)hi;
+        if (prefilter && copies > 1) { /* the size reduction may widen this one to x{m',} */
+            const size_t i = repeats.size();
+            repeats.push_back({leaves(a) * copies, lo});
+            if (widen && i < widen->size() && (*widen)[i] >= 0) {
+                lo = (unsigned)(*widen)[i];
+                hi = -1;
+            }
+        }
         /* repeats are unrolled: refuse before copying what cannot fit the largest model anyway */
-        unrolled += leaves(a) * std::max<size_t>(hi < 0 ? lo + 1 : (size_t)hi, 1);
+        /* (under HS_FLAG_PREFILTER a copy without positions, of a look-around or a reference, still costs a node:
+         * the repeats may be 65 535 long there) */
+        unrolled += std::max<size_t>(leaves(a), prefilter) * std::max<size_t>(hi < 0 ? lo + 1 : (size_t)hi, 1);
         if (unrolled > 4 * MAX_NFA_STATES) {
+            if (prefilter) { /* the reduction widens repeats until the expression fits */
+                overflow = true;
+                return mk(Node::EMPTY);
+            }
             fail("Pattern is too large.");
         }
         NodeP s = mk(Node::CAT);
@@ -751,7 +1042,8 @@ private:
             if (comma && haveY && y < x) {
                 fail("Bounded repeat is invalid: min > max.");
             }
-            if (x > 1000 || (haveY && y > 1000)) {
+            const unsigned long most = prefilter ? 65535 : 1000; /* PCRE's own limit, when repeats can be widened */
+            if (x > most || (haveY && y > most)) {
                 fail("Pattern is too large.");
             }
             pos = q + 1;
@@ -763,7 +1055,10 @@ private:
         if (pos < n && re[pos] == '?') {
             pos++; /* lazy: same set of match ends */
         } else if (pos < n && re[pos] == '+') {
-            fail("Possessive quantifiers are not supported.");
+            if (!prefilter) {
+                fail("Possessive quantifiers are not supported.");
+            }
+            pos++; /* the greedy form: the same match ends and more */
         }
         if (lo == 1 && hi == 1) {
             return a;
@@ -1042,7 +1337,41 @@ private:
         if (c == '(') {
             pos++;
             const unsigned saved = flags; /* an option change lasts to the end of the group it is in */
-            if (at('?')) {
+            unsigned capture = 0;         /* the group's number; 0: not a capturing group */
+            bool lookAround = false;
+            std::string name;
+            const char q1 = pos + 1 < n ? re[pos + 1] : 0, q2 = pos + 2 < n ? re[pos + 2] : 0;
+            if (at('?') && (q1 == '\'' || (q1 == '<' && q2 != '=' && q2 != '!') || (q1 == 'P' && q2 == '<'))) {
+                /* a named group, (?<name>...), (?'name'...), (?P<name>...): a capturing group in every mode */
+                const size_t start = pos - 1;
+                pos += q1 == 'P' ? 3 : 2;
+                if (!readName(q1 == '\'' ? '\'' : '>', &name)) {
+                    fail("Look-around, named groups, comments and the other (?...) groups are not supported.");
+                }
+                if (isdigit((unsigned char)name[0])) {
+                    pos = start;
+                    fail("Group name cannot begin with a digit.");
+                }
+                if (!names.emplace(name, groups).second) {
+                    fail("Two named subpatterns use the name '" + name + "'.");
+                }
+                capture = groups++;
+            } else if (prefilter && at('?') && (q1 == '=' || q1 == '!' || (q1 == '<' && (q2 == '=' || q2 == '!')))) {
+                pos += q1 == '<' ? 3 : 2; /* look-around: an empty sequence */
+                lookAround = true;
+            } else if (prefilter && at('?') && q1 == '>') {
+                pos += 2; /* an atomic group: a plain group */
+            } else if (prefilter && at('?') && q1 == '(') {
+                return conditional(saved);
+            } else if (prefilter && at('?') && q1 == 'P' && q2 == '=') {
+                pos += 3;
+                if (!readName(')', &name)) {
+                    fail("Look-around, named groups, comments and the other (?...) groups are not supported.");
+                }
+                return backRef(0, name);
+            } else if (!at('?')) {
+                capture = groups++;
+            } else {
                 /* (?ims-ims) and (?ims-ims: ... ) */
                 size_t q = pos + 1;
                 unsigned on = 0, off = 0;
@@ -1071,13 +1400,20 @@ private:
                     fail("Look-around, named groups, comments and the other (?...) groups are not supported.");
                 }
             }
+            if (capture) {
+                referent.push_back(nullptr);
+            }
+            const size_t refsBefore = refsSeen;
             NodeP r = alt();
             if (!at(')')) {
                 fail("Missing close parenthesis.");
             }
             pos++;
             flags = saved;
-            return r;
+            if (capture && refsSeen == refsBefore && leaves(r) <= 1 && !hasAssert(r)) {
+                referent[capture] = clone(r);
+            }
+            return lookAround ? mk(Node::EMPTY) : r;
         }
         if (c == '[') {
             /* "[:name:]", "[.x.]", "[=x=]" where a class should start: PCRE's check_posix_syntax */
@@ -1109,6 +1445,11 @@ private:
             a->assertKind = c == '^' ? (ml ? A_BEGIN_LINE : A_BEGIN) : (ml ? A_END_LINE : A_END_LF);
             pos++;
             return a;
+        }
+        if (prefilter && c == '\\' && pos + 1 < n) {
+            if (NodeP b = prefilterEscape()) {
+                return b;
+            }
         }
         if (utf8) {
             return atomU();
@@ -1383,11 +1724,113 @@ std::vector<NodeP> topArms(const NodeP &root) {
     return {root};
 }
 
+void addTree(RawNfa *nfa, const NodeP &root, u32 report, u32 reportBeforeNewline, u64 minLength);
+
+/* The expression's tree, and the min_length its automaton keeps.  Under HS_FLAG_PREFILTER an expression whose own
+ * automaton would be too large is reduced to a superset that fits (the role of src/nfagraph/ng_prefilter.cpp):
+ * bounded repeats x{m,n} become x{m',}, the largest contribution first, each with the largest m' <= m that fits;
+ * if that is not enough, min_length goes and the repeats are reduced again.  An expression that fits without a
+ * reduction keeps its tree, so its database is the one it has without the flag. */
+struct Parsed {
+    NodeP root;
+    u64 minLength;
+};
+
+/* what the reduction chose for one expression: the widened repeats and the min_length kept, or its error */
+struct Reduction {
+    std::vector<long> widen;
+    u64 minLength;
+    std::string error;
+};
+
+Reduction reduce(const char *re, unsigned flags, u64 minLength) {
+    std::vector<long> widen;
+    std::vector<Repeat> repeats;
+    std::string tooLarge;
+    /* does its own automaton fit?  Syntax and other errors are thrown as they are */
+    auto fits = [&](u64 ml) -> bool {
+        Parser p(re, flags, &widen);
+        NodeP r = p.parse();
+        repeats = p.repeats;
+        if (p.overflow) {
+            tooLarge = tooLarge.empty() ? "Pattern is too large." : tooLarge;
+            return false;
+        }
+        try {
+            RawNfa own;
+            regexNfaInit(&own);
+            addTree(&own, r, 1, 2, ml);
+        } catch (const RegexError &e) {
+            if (e.msg.find("too large") == std::string::npos) {
+                return true; /* (not a size error: the real build reports it) */
+            }
+            tooLarge = tooLarge.empty() ? e.msg : tooLarge;
+            return false;
+        }
+        return true;
+    };
+    for (const u64 ml : {minLength, (u64)0}) {
+        widen.clear();
+        if (fits(ml)) {
+            return {widen, ml, ""};
+        }
+        const std::vector<Repeat> all = repeats;
+        std::vector<size_t> order(all.size());
+        for (size_t i = 0; i < order.size(); i++) order[i] = i;
+        std::stable_sort(order.begin(), order.end(),
+                         [&](size_t a, size_t b) { return all[a].positions > all[b].positions; });
+        widen.assign(all.size(), -1);
+        for (const size_t i : order) {
+            const long least = std::min<long>(all[i].lo, 1); /* x{1,} is x+, as small as x* and not nullable */
+            widen[i] = least;
+            if (!fits(ml)) {
+                continue; /* too large even so: this one stays at its least, and the next one widens too */
+            }
+            long good = least, tooBig = (long)all[i].lo + 1;
+            while (tooBig - good > 1) {
+                const long mid = (good + tooBig) / 2;
+                widen[i] = mid;
+                (fits(ml) ? good : tooBig) = mid;
+            }
+            widen[i] = good;
+            return {widen, ml, ""};
+        }
+        if (!minLength) {
+            break;
+        }
+    }
+    return {{}, 0, tooLarge};
+}
+
+Parsed parseExpr(const char *re, unsigned flags, u64 minLength) {
+    if (!(flags & HS_FLAG_PREFILTER)) {
+        return {Parser(re, flags).parse(), minLength};
+    }
+    /* one compile asks for the same expression several times (widths, the "can never match" check, the build):
+     * the reduction's search runs once per expression and thread */
+    thread_local std::map<std::tuple<std::string, unsigned, u64>, Reduction> cache;
+    const auto key = std::make_tuple(std::string(re), flags, minLength);
+    auto it = cache.find(key);
+    if (it == cache.end()) {
+        if (cache.size() >= 4096) {
+            cache.clear();
+        }
+        it = cache.emplace(key, reduce(re, flags, minLength)).first;
+    }
+    const Reduction &red = it->second;
+    if (!red.error.empty()) {
+        throw RegexError{red.error};
+    }
+    return {Parser(re, flags, &red.widen).parse(), red.minLength};
+}
+
 } // namespace
 
-RegexInfo regexInfo(const char *re, unsigned flags, bool forInfo) {
-    const NodeP root = Parser(re, flags).parse();
+RegexInfo regexInfo(const char *re, unsigned flags, bool forInfo, u64 minLength) {
+    const Parsed parsed = parseExpr(re, flags, minLength);
+    const NodeP &root = parsed.root;
     RegexInfo info;
+    info.minLengthDropped = parsed.minLength != minLength;
     info.minLen = ~0u;
     bool someOtherExit = false, someFloatingEntry = false;
     /* one way out of the expression: the assertions crossed after the last character, and whether that character
@@ -1484,7 +1927,13 @@ void regexNfaInit(RawNfa *nfa) {
 }
 
 void regexNfaAdd(RawNfa *nfa, const char *re, unsigned flags, u32 report, u32 reportBeforeNewline, u64 minLength) {
-    const NodeP root = Parser(re, flags).parse();
+    const Parsed p = parseExpr(re, flags, minLength);
+    addTree(nfa, p.root, report, reportBeforeNewline, p.minLength);
+}
+
+namespace {
+
+void addTree(RawNfa *nfa, const NodeP &root, u32 report, u32 reportBeforeNewline, u64 minLength) {
     const CharSet W = Glushkov::wordSet();
     auto newState = [&]() -> u32 {
         if (nfa->nstates >= MAX_NFA_STATES) {
@@ -1687,5 +2136,7 @@ void regexNfaAdd(RawNfa *nfa, const char *re, unsigned flags, u32 report, u32 re
         }
     }
 }
+
+} // namespace
 
 } // namespace hsb

@@ -26,7 +26,16 @@
  * and LONG S, which fold to "k" and "s"); a caseless non-ASCII character, \p \P \X and
  * HS_FLAG_UCP are refused.
  *
- * Everything else -- look-around, back-references, possessive quantifiers, UCP, SOM, expressions
+ * Named groups (?<n>...) (?'n'...) (?P<n>...) are capturing groups in every mode.
+ *
+ * HS_FLAG_PREFILTER (src/parser/prefilter.cpp): the expression is rewritten into one whose matches are
+ * a superset of its own -- a back-reference (\1..\99, \g, \k, (?P=n)) becomes a copy of its group when
+ * that group is one character position (folded where the reference is caseless), else any byte
+ * sequence; look-around becomes nothing, an atomic group a plain group, a possessive quantifier the
+ * greedy one, a conditional group the alternation of its branches, \X ".+" -- and an expression whose automaton would be too large is widened until it fits
+ * (bounded repeats x{m,n} become x{m',}; then min_length goes).
+ *
+ * Everything else -- look-around and the rest without HS_FLAG_PREFILTER, UCP, SOM, expressions
  * that match the empty string -- is refused with a compile error: those need parts of the
  * reference's compiler and runtime this build does not have.
  */
@@ -55,6 +64,7 @@ struct RegexInfo {
     bool unordered = false, atEod = false, onlyAtEod = false;
     std::vector<std::pair<u32, u32>> armWidths; /* (shortest, longest) match of every top-level alternative */
     bool anchored = false; /* every way into the expression crosses \A / a non-multiline "^" */
+    bool minLengthDropped = false; /* HS_FLAG_PREFILTER: the automaton fits only without the min_length */
 };
 
 /* Valid UTF-8 (src/parser/utf8_validate.cpp): no overlong form, surrogate, code point above 0x10FFFF or
@@ -62,8 +72,9 @@ struct RegexInfo {
 bool validUtf8(const char *s, size_t len);
 
 /* Number of positions / shortest match of one expression (throws RegexError).  forInfo: hs_expression_info also
- * describes expressions that match the empty buffer (hs_compile refuses those without HS_FLAG_ALLOWEMPTY). */
-RegexInfo regexInfo(const char *re, unsigned flags, bool forInfo = false);
+ * describes expressions that match the empty buffer (hs_compile refuses those without HS_FLAG_ALLOWEMPTY).
+ * minLength: as for regexNfaAdd, so that a prefiltered expression is described as the same reduction. */
+RegexInfo regexInfo(const char *re, unsigned flags, bool forInfo = false, u64 minLength = 0);
 
 /* Add the expression's position automaton to `nfa`: its accepting positions raise `report`.
  * State 0 of `nfa` is the floating start (always on), state 1 the anchored start (on at

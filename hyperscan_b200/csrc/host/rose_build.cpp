@@ -881,7 +881,7 @@ std::vector<u8> buildRegexEngine(Blob &blob, const std::vector<RegexPattern> &pa
     };
     for (const RegexPattern &p : pats) {
         try {
-            const RegexInfo ri = regexInfo(p.re.c_str(), p.flags);
+            const RegexInfo ri = regexInfo(p.re.c_str(), p.flags, false, p.minLength);
             /* extended parameters no match can satisfy (src/nfagraph/ng_extparam.cpp:820-880) */
             if (p.minLength && ri.maxLen != 0xffffffffu && p.minLength > ri.maxLen) {
                 throw CompileError{"Expression has min_length=" + std::to_string(p.minLength) + " but can only produce matches of length " +
@@ -959,7 +959,7 @@ std::vector<std::vector<RegexPattern>> packEngineGroups(const std::vector<RegexP
     RawNfa last; /* the automaton of the last group */
     for (const RegexPattern &p : pats) {
         try {
-            const RegexInfo ri = regexInfo(p.re.c_str(), p.flags);
+            const RegexInfo ri = regexInfo(p.re.c_str(), p.flags, false, p.minLength);
             /* the reports do not change the positions: placeholders stand in for the report programs */
             auto add = [&](RawNfa *n) { regexNfaAdd(n, p.re.c_str(), p.flags, 1, ri.needsAdjust ? 2 : 0, p.minLength); };
             if (!groups.empty()) {

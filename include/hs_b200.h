@@ -62,6 +62,13 @@ typedef int hs_error_t;                     /* src/hs_common.h:52 */
  * set of ASCII literals compiles as without it. */
 #define HS_FLAG_UTF8 32
 #define HS_FLAG_UCP 64
+/* HS_FLAG_PREFILTER: the expression is rewritten into one whose matches are a superset of its own, to be
+ * confirmed by the application (with PCRE, say): a back-reference becomes a copy of its group when that group is
+ * one character position (caseless where the reference is), else any byte sequence; look-around becomes nothing; atomic groups, possessive quantifiers and
+ * conditional groups become their plain forms; an expression whose automaton would be too large has its bounded
+ * repeats widened, then its min_length dropped, until it fits.  An expression with none of these compiles to the
+ * same database as without the flag.  Refused with HS_FLAG_SOM_LEFTMOST, in a combination's sub-expression and
+ * by hs_compile_lit* (DESIGN.md section 10b, "Prefilter mode"). */
 #define HS_FLAG_PREFILTER 128
 #define HS_FLAG_SOM_LEFTMOST 256
 #define HS_FLAG_COMBINATION 512
@@ -146,7 +153,7 @@ typedef int (*match_event_handler)(unsigned int id, unsigned long long from,
  * literals, those go to a literal matcher beside that engine instead
  * (ROSE_RUNTIME_FULL_ROSE, block mode) -- DESIGN.md section 10d.
  * Expressions in UTF-8 mode (HS_FLAG_UTF8) take either route.
- * Anything else (look-around, back-references, UCP, larger sets, ...) yields
+ * Anything else (look-around, back-references without HS_FLAG_PREFILTER, UCP, ...) yields
  * HS_COMPILER_ERROR with an explanatory hs_compile_error_t, exactly as the
  * reference reports unsupported constructs.
  * Logical combinations (HS_FLAG_COMBINATION, with HS_FLAG_QUIET on any expression) are
