@@ -148,6 +148,7 @@ def lib():
         L.hs_b200_fetch_matches.argtypes = [vp, vp, vp, C.c_size_t, u64p]
         L.hs_b200_order_matches_async.argtypes = [vp, vp, vp, C.c_size_t, vp, vp]
         L.hs_b200_order_records_async.argtypes = [vp, vp, vp, C.c_size_t, vp, C.c_size_t, vp, vp]
+        L.hs_b200_scan_rows_async.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, vp]
         L.hs_b200_db_info.argtypes = [vp, C.POINTER(DbInfo)]
         L.hs_b200_set_build_option.argtypes = [cp, C.c_int]
         L.hs_b200_set_runtime_option.argtypes = [cp, C.c_int]
@@ -503,6 +504,24 @@ def order_records_async(db, scratch, recs, n, out, count, stream=None, cap=None)
     cap = _capacity(out) if cap is None else int(cap)
     _check(lib().hs_b200_order_records_async(db.ptr, scratch.ptr, _dev_ptr(recs), int(n), _dev_ptr(out), cap,
                                              _dev_ptr(count), C.c_void_p(stream or 0)), "order_records_async")
+
+
+def scan_rows_async(db, chars, offsets, scratch, stream=None):
+    """hs_b200_scan_rows_async: one pass over the rows of a column already in device memory -- `chars` a uint8
+    CUDA tensor, `offsets` an int64 CUDA tensor of nrows + 1 entries, row i = chars[offsets[i]:offsets[i + 1]]
+    (numpy arrays under the SIMT emulator) -- enqueued on `stream` (a cudaStream_t address; None = the scratch's
+    stream).  Returns at once; the records are served by scan_corpus_finish, fetch_matches and
+    order_matches_async."""
+    for x, dt in ((chars, "uint8"), (offsets, "int64")):
+        name = str(x.dtype).replace("torch.", "")
+        if name != dt and not (dt == "int64" and name == "uint64"):
+            raise ValueError("expected %s, got %s" % (dt, name))
+    nrows = (offsets.numel() if hasattr(offsets, "numel") else offsets.size) - 1
+    if nrows < 0:
+        raise ValueError("offsets needs nrows + 1 entries")
+    nbytes = chars.numel() if hasattr(chars, "numel") else chars.size
+    _check(lib().hs_b200_scan_rows_async(db.ptr, _dev_ptr(chars) if nbytes else None, nbytes, _dev_ptr(offsets),
+                                         nrows, scratch.ptr, C.c_void_p(stream or 0)), "scan_rows_async")
 
 
 def scan_corpus(db, corpus, scratch, fetch=True):

@@ -35,6 +35,7 @@
 #include "../host/pair_table.h"
 #include "kernels.h"
 #include "order_kernels.h"
+#include "rows_kernels.h"
 
 using namespace hsb;
 
@@ -840,6 +841,9 @@ struct hs_b200_corpus {
     const u64 *streamOffset = nullptr;
     std::vector<u32> h_len;  /* block lengths, for the end-of-block evaluation of logical combinations */
     u32 maxLen = 0;          /* the longest block (resident corpora): bounds a match's end offset */
+    /* a row scan's staging corpus (hs_b200_scan_rows_async): its block table is filled on the device, h_len is
+     * empty, `bytes` is the host's bound and `payload` the size of the rows' chars, which bounds their sum */
+    bool deviceTables = false;
 };
 
 /* ---- scratch ------------------------------------------------------------------ */
@@ -878,6 +882,10 @@ struct hs_scratch {
     /* temporaries of hs_b200_order_*_async (order_kernels.h), grown on demand */
     u8 *d_order;
     size_t orderBytes;
+    /* of hs_b200_scan_rows_async: the staging corpus, and the plan's temporaries (rows_kernels.h), grown on demand */
+    hs_b200_corpus *rowsCorpus;
+    u8 *d_rows;
+    size_t rowsBytes;
     SegArea *seg;            /* of the engine runs, created on first use */
     float lastMs;
     int smCount, maxSmem;
@@ -1132,23 +1140,33 @@ void fillParams(const hs_scratch *s, const DevImage *im, const hs_b200_corpus *c
 enum : u32 { SEG_MIN = 4096, SEG_WARM = 256, SEG_ROUNDS = 2 };
 static const size_t SEG_FORCED_MAX = (size_t)1 << 30;
 
-/* Cut the blocks of c for a run of `engines` engines of `kind`?  Fills the segment table (every block, in order: a
- * block not cut is one segment with both flags) and the cut blocks {first segment, segments}; false: one lane per
- * block. */
-bool planSegments(const hs_b200_corpus *c, u32 kind, u64 engines, int smCount, std::vector<DfaSeg> *segs,
-                  std::vector<uint2> *cuts) {
+/* The rule from the block count and the payload alone: may blocks of c be cut for a run of `engines` engines of
+ * `kind`, and if so, into segments of *segLen bytes, the blocks longer than *cutAbove. */
+bool segmentRule(const hs_b200_corpus *c, u32 kind, u64 engines, int smCount, u64 *segLen, u64 *cutAbove) {
     const int opt = g_opts.engineSegment;
-    if (opt < 0 || c->nblocks == 0 || c->h_len.size() != c->nblocks) {
+    if (opt < 0 || c->nblocks == 0) {
         return false;
     }
-    u64 segLen = (u64)opt, cutAbove = (u64)opt;
+    *segLen = *cutAbove = (u64)opt;
     if (opt == 0) {
         const u64 lanes = dfaResidentLanes(kind, smCount);
         if (engines * c->nblocks * 2 > lanes) {
             return false; /* the blocks alone keep half the resident lanes busy or more */
         }
-        segLen = std::max<u64>(SEG_MIN, HSB_ROUNDUP(c->payload * engines / lanes + 1, 16));
-        cutAbove = 2 * segLen;
+        *segLen = std::max<u64>(SEG_MIN, HSB_ROUNDUP(c->payload * engines / lanes + 1, 16));
+        *cutAbove = 2 * *segLen;
+    }
+    return true;
+}
+
+/* Cut the blocks of c for a run of `engines` engines of `kind`?  Fills the segment table (every block, in order: a
+ * block not cut is one segment with both flags) and the cut blocks {first segment, segments}; false: one lane per
+ * block. */
+bool planSegments(const hs_b200_corpus *c, u32 kind, u64 engines, int smCount, std::vector<DfaSeg> *segs,
+                  std::vector<uint2> *cuts) {
+    u64 segLen = 0, cutAbove = 0;
+    if (c->h_len.size() != c->nblocks || !segmentRule(c, kind, engines, smCount, &segLen, &cutAbove)) {
+        return false;
     }
     if (*std::max_element(c->h_len.begin(), c->h_len.end()) <= cutAbove) {
         return false;
@@ -1174,7 +1192,9 @@ bool planSegments(const hs_b200_corpus *c, u32 kind, u64 engines, int smCount, s
 
 /* Run an engine (dp from engineParams, dp.nfa its bytes in device memory), or a fused launch of several
  * (dp.engines), over every block of corpus c, into the record ring out[0, outCap) and its counters.  Long
- * blocks are cut into segments walked by lanes of their own (planSegments); `seg` holds their plan and states. */
+ * blocks are cut into segments walked by lanes of their own (planSegments); `seg` holds their plan and states.
+ * A corpus whose block lengths only the device knows (deviceTables) gets its plan from launchRowSegments, in
+ * lists sized by the bound the payload sets: no block may be cut when the payload is no longer than cutAbove. */
 cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u32 outCap,
                          u32 *counters, int smCount, int maxSmem, SegArea *seg, cudaStream_t stream) {
     dp.corpus = c->d_data;
@@ -1191,19 +1211,33 @@ cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u
     std::vector<DfaSeg> segs;
     std::vector<uint2> cuts;
     const size_t engines = dp.engines ? dp.nengines : 1;
-    if (!planSegments(c, dp.kind, engines, smCount, &segs, &cuts)) {
+    u64 segLen = 0, cutAbove = 0, nsegs = 0, ncuts = 0;
+    const bool devicePlan = c->deviceTables && segmentRule(c, dp.kind, engines, smCount, &segLen, &cutAbove) &&
+                            c->payload > cutAbove;
+    if (devicePlan) {
+        nsegs = c->nblocks + c->payload / segLen + 1;
+        ncuts = std::min<u64>(c->nblocks, c->payload / (cutAbove + 1));
+        if (nsegs > 0xfffffff0ull) {
+            return cudaErrorMemoryAllocation;
+        }
+    } else if (planSegments(c, dp.kind, engines, smCount, &segs, &cuts)) {
+        nsegs = segs.size();
+        ncuts = cuts.size();
+    } else {
         const cudaError_t e = launchDfa(dp, smCount, maxSmem, stream);
         if (e == cudaSuccess) {
             g_launches++;
         }
         return e;
     }
-    /* [segs][cuts][per engine, per block: first open segment][per engine: guess states, end states] */
-    const size_t segBytes = HSB_ROUNDUP(segs.size() * sizeof(DfaSeg), 256);
-    const size_t planBytes = segBytes + cuts.size() * sizeof(uint2);
+    /* [segs][cuts][device plans: the first segment of every block][per engine, per block: first open segment]
+     * [per engine: guess states, end states] */
+    const size_t segBytes = HSB_ROUNDUP(nsegs * sizeof(DfaSeg), 256);
+    const size_t cutBytes = HSB_ROUNDUP(ncuts * sizeof(uint2), 256);
+    const size_t planBytes = segBytes + (devicePlan ? cutBytes + (c->nblocks + 1) * sizeof(u32) : ncuts * sizeof(uint2));
     const size_t openBytes = HSB_ROUNDUP(engines * c->nblocks * sizeof(u32), 256);
     const size_t statesAt = HSB_ROUNDUP(planBytes, 256) + openBytes;
-    const size_t need = statesAt + engines * 2 * segs.size() * dfaStateBytes(dp.kind);
+    const size_t need = statesAt + engines * 2 * nsegs * dfaStateBytes(dp.kind);
     if (g_opts.engineSegment > 0 && need > SEG_FORCED_MAX) {
         return cudaErrorMemoryAllocation; /* a forced length too short for this corpus and engine count */
     }
@@ -1226,13 +1260,35 @@ cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u
         }
         seg->bytes = need + need / 4;
     }
+    cudaError_t e = cudaSuccess;
+    if (devicePlan) {
+        RowSegParams rp;
+        rp.blockLen = c->d_len;
+        rp.nrows = (u32)c->nblocks;
+        rp.segLen = (u32)segLen;
+        rp.cutAbove = (u32)std::min<u64>(cutAbove, 0xffffffffull);
+        rp.segs = reinterpret_cast<DfaSeg *>(seg->d);
+        rp.segCap = (u32)nsegs;
+        rp.cuts = reinterpret_cast<uint2 *>(seg->d + segBytes);
+        rp.cutCap = (u32)ncuts;
+        rp.segFirst = reinterpret_cast<u32 *>(seg->d + segBytes + cutBytes);
+        seg->plan.clear(); /* what is in device memory is no host plan's image */
+        unsigned launched = 0;
+        e = launchRowSegments(rp, smCount, stream, &launched);
+        g_launches += launched;
+        if (e != cudaSuccess) {
+            return e;
+        }
+    }
     /* the plan's image; copied only when it differs from the one in device memory (a scan of the same corpus
      * again, or the next engine kind of the same scan, reuses it) */
-    std::vector<u8> image(planBytes, 0);
-    memcpy(image.data(), segs.data(), segs.size() * sizeof(DfaSeg));
-    memcpy(image.data() + segBytes, cuts.data(), cuts.size() * sizeof(uint2));
-    cudaError_t e = cudaSuccess;
-    if (image != seg->plan) {
+    std::vector<u8> image;
+    if (!devicePlan) {
+        image.assign(planBytes, 0);
+        memcpy(image.data(), segs.data(), segs.size() * sizeof(DfaSeg));
+        memcpy(image.data() + segBytes, cuts.data(), cuts.size() * sizeof(uint2));
+    }
+    if (!devicePlan && image != seg->plan) {
         e = cudaEventSynchronize(seg->copied); /* the last copy out of the pinned buffer has been made */
         if (e == cudaSuccess && planBytes > seg->hBytes) {
             cudaFreeHost(seg->h);
@@ -1260,9 +1316,9 @@ cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u
         return e;
     }
     dp.segs = reinterpret_cast<const DfaSeg *>(seg->d);
-    dp.nsegs = (u32)segs.size();
+    dp.nsegs = (u32)nsegs;
     dp.cuts = reinterpret_cast<const uint2 *>(seg->d + segBytes);
-    dp.ncuts = (u32)cuts.size();
+    dp.ncuts = (u32)ncuts;
     dp.warm = SEG_WARM;
     dp.segOpen = open;
     dp.segStates = seg->d + statesAt;
@@ -1272,7 +1328,7 @@ cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u
     g_launches += launches;
     if (e == cudaSuccess) {
         seg->runs++;
-        seg->segments += segs.size();
+        seg->segments += nsegs;
     }
     return e;
 }
@@ -1374,9 +1430,11 @@ struct StreamPass {
 /* Enqueue a scan of the whole corpus on `stream`: reset the counters, launch the tile
  * ranges, read the counters back.  The only place a scan's stream sequence is issued.
  * For a stream-set pass (sp), the look-behind is written in front of every write first,
- * and the streams advance -- or the set is marked -- before the counters are read back. */
+ * and the streams advance -- or the set is marked -- before the counters are read back.
+ * For a row scan (rows), the row plan fills c's block table and packs the rows into it first. */
 hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
-                       cudaStream_t stream, const Upload *up = nullptr, const StreamPass *sp = nullptr) {
+                       cudaStream_t stream, const Upload *up = nullptr, const StreamPass *sp = nullptr,
+                       const RowsParams *rows = nullptr) {
     if (s->nPeers && (im->rules.shape == SHAPE_LITERALS_OUTFIX || im->rules.shape == SHAPE_OUTFIXES)) {
         /* the engine kernel stores no records into the peers' exchange buffers, and the count it
          * publishes would cover them: an exchange of both halves' records, or of several engines',
@@ -1393,6 +1451,11 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
         CUDA_TRY(launchStreamAssemble(c->d_data, sp->hist, (u32)c->nblocks, c->streamPitch, sp->srcLen, sp->len,
                                       sp->mark, *sp->epoch, stream));
         g_launches++;
+    }
+    if (rows) {
+        unsigned launched = 0;
+        CUDA_TRY(launchRowPlan(*rows, s->smCount, stream, &launched));
+        g_launches += launched;
     }
     CUDA_TRY(cudaEventRecord(s->evStart, stream));
     const u32 ntiles = (u32)((c->bytes + pl.tileBytes - 1) / pl.tileBytes);
@@ -1794,6 +1857,9 @@ hs_error_t hs_scratch_size(const hs_scratch_t *scratch, size_t *size) {
     if (scratch->inlineCorpus) {
         n += scratch->inlineCorpus->capData;
     }
+    if (scratch->rowsCorpus) {
+        n += scratch->rowsCorpus->capData;
+    }
     *size = n;
     return HS_SUCCESS;
 }
@@ -1827,6 +1893,8 @@ hs_error_t hs_free_scratch(hs_scratch_t *s) {
     freeCorpus(s->inlineCorpus);
     cudaFree(s->d_out);
     cudaFree(s->d_order);
+    freeCorpus(s->rowsCorpus);
+    cudaFree(s->d_rows);
     delete s->seg;
     cudaFree(s->d_counters);
     if (s->h_counters) cudaFreeHost(s->h_counters);
@@ -2018,6 +2086,17 @@ static hs_error_t checkScanArgs(const hs_database_t *db, hs_scratch_t *scratch) 
     return validScratch(scratch) ? HS_SUCCESS : HS_INVALID;
 }
 
+/* A pass over no bytes: no records, on the host and, for the stream-ordered readers of the ring, on the device */
+static hs_error_t emptyPass(hs_scratch *s, cudaStream_t st) {
+    s->h_counters[CTR_MATCHES] = 0;
+    s->h_counters[CTR_ERROR] = 0;
+    s->pending = false;
+    s->lastCount = 0;
+    s->streamEpoch = nullptr;
+    return cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), st) == cudaSuccess ? HS_SUCCESS
+                                                                                          : HS_UNKNOWN_ERROR;
+}
+
 hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corpus_t *corpus,
                                      hs_scratch_t *scratch, void *cuda_stream) {
     if (!scratch || !corpus) {
@@ -2036,15 +2115,7 @@ hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corp
     if (r == HS_SUCCESS) {
         cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
         if (corpus->bytes == 0 || corpus->nblocks == 0) {
-            scratch->h_counters[CTR_MATCHES] = 0;
-            scratch->h_counters[CTR_ERROR] = 0;
-            scratch->pending = false;
-            scratch->lastCount = 0;
-            scratch->streamEpoch = nullptr;
-            /* the device count too: the stream-ordered readers of the ring see no records */
-            if (cudaMemsetAsync(scratch->d_counters, 0, CTR_COUNT * sizeof(u32), st) != cudaSuccess) {
-                r = HS_UNKNOWN_ERROR;
-            }
+            r = emptyPass(scratch, st);
         } else {
             r = enqueueScan(scratch, im, corpus, st);
         }
@@ -2387,6 +2458,104 @@ hs_error_t hs_b200_order_records_async(const hs_database_t *db, hs_scratch_t *sc
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
     r = enqueueOrder(scratch, im, (const DevMatch *)d_recs, nullptr, 0, (u32)n, d_out, cap, d_count,
                      ORDER_MAX_PASSES, st);
+    unmarkInUse(scratch);
+    return r;
+}
+
+/* ---- row scans: a column of rows in device memory -------------------------------------------------------------- */
+
+/* The staging corpus of a row scan (`bound` bytes packed, nrows blocks) and the row plan's temporaries */
+static hs_error_t reserveRows(hs_scratch *s, u64 bound, size_t nrows) {
+    if (!s->rowsCorpus) {
+        s->rowsCorpus = new (std::nothrow) hs_b200_corpus();
+        if (!s->rowsCorpus) {
+            return HS_NOMEM;
+        }
+        s->rowsCorpus->device = s->device;
+        s->rowsCorpus->deviceTables = true;
+    }
+    const u8 *before = s->rowsCorpus->d_alloc;
+    hs_error_t r = reserveCorpus(s->rowsCorpus, bound, nrows);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    if (s->rowsCorpus->d_alloc != before) {
+        /* the front pad of a new allocation is zeroed on the legacy stream: done before any pass reads it */
+        CUDA_TRY(cudaDeviceSynchronize());
+    }
+    const size_t ntiles = (nrows + ROWS_TILE - 1) / ROWS_TILE;
+    const size_t need = 256 + HSB_ROUNDUP(ntiles * sizeof(u64), 256) + ntiles * sizeof(u32);
+    if (need > s->rowsBytes) {
+        cudaFree(s->d_rows); /* (synchronises with any pass still using it) */
+        s->d_rows = nullptr;
+        s->rowsBytes = 0;
+        CUDA_TRY(cudaMalloc(&s->d_rows, need + need / 8));
+        s->rowsBytes = need + need / 8;
+    }
+    return HS_SUCCESS;
+}
+
+hs_error_t hs_b200_scan_rows_async(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
+                                   const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch,
+                                   void *cuda_stream) {
+    if (!db || !scratch || !d_offsets || (uintptr_t)d_offsets % 8 || (!d_chars && chars_bytes) ||
+        nrows > 0xfffffff0u) {
+        return HS_INVALID;
+    }
+    hs_error_t r = checkScanArgs(db, scratch);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    if (dbRose(db)->ckeyCount) {
+        return HS_INVALID; /* combination reports are evaluated per block on the host, from the block lengths */
+    }
+    DevImage *im = heldImage(scratch, db);
+    if (!im) {
+        return HS_INVALID;
+    }
+    if (scratch->nPeers) {
+        return HS_ARCH_ERROR;
+    }
+    if (markInUse(scratch)) {
+        return HS_SCRATCH_IN_USE;
+    }
+    DeviceGuard guard(scratch->device);
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
+    /* the packed rows take at most their bytes plus 16 per row (a row's pad, or an empty row's 16 bytes) */
+    const u64 bound = (u64)chars_bytes + 16 * (u64)nrows;
+    if (nrows == 0) {
+        r = emptyPass(scratch, st);
+    } else {
+        r = reserveRows(scratch, bound, nrows);
+    }
+    hs_b200_corpus *c = scratch->rowsCorpus;
+    if (r == HS_SUCCESS && nrows) {
+        c->nblocks = nrows;
+        c->bytes = bound;
+        c->readableEnd = HSB_ROUNDUP(bound, 16) + 16;
+        c->payload = chars_bytes;
+        c->uniformPitch = 0;
+        c->uniformLen = 0;
+        RowsParams rp;
+        rp.chars = (const u8 *)d_chars;
+        rp.charsBytes = chars_bytes;
+        rp.offsets = (const u64 *)d_offsets;
+        rp.nrows = (u32)nrows;
+        rp.corpus = c->d_data;
+        rp.zeroEnd = HSB_ROUNDUP(bound, 16) + 32;
+        rp.blockOff = c->d_off;
+        rp.blockLen = c->d_len;
+        rp.bad = reinterpret_cast<u32 *>(scratch->d_rows);
+        rp.tilePad = reinterpret_cast<u64 *>(scratch->d_rows + 256);
+        rp.tileBad = reinterpret_cast<u32 *>(scratch->d_rows + 256 +
+                                             HSB_ROUNDUP((nrows + ROWS_TILE - 1) / ROWS_TILE * sizeof(u64), 256));
+        rp.counters = scratch->d_counters;
+        rp.outCap = scratch->outCap;
+        r = enqueueScan(scratch, im, c, st, nullptr, nullptr, &rp);
+    }
+    scratch->lastCorpus = c;
+    scratch->lastBlocks = nrows;
+    scratch->lastMaxLen = chars_bytes; /* no row is longer; the device decides the radix passes the records need */
     unmarkInUse(scratch);
     return r;
 }

@@ -60,7 +60,8 @@ enum ConfirmKind {
 enum { MAX_PEERS = 8 };
 enum { CTR_MATCHES = 0, CTR_ERROR = 1, CTR_CANDIDATES = 2, CTR_CONFIRMED = 3,
        CTR_PREFILTER_PASS = 4, CTR_CANDQ = 5 /* candidates handed to the confirm kernel */,
-       CTR_STREAM = 6 /* a stream-set pass that did not commit: STREAM_MARKED, | STREAM_BAD_LENGTH */,
+       CTR_STREAM = 6 /* a stream-set pass that did not commit: STREAM_MARKED, | STREAM_BAD_LENGTH; a row scan
+                       * whose row table is bad: STREAM_BAD_LENGTH */,
        CTR_COUNT = 8 };
 
 /* Every scan kernel stops at the prefilter and appends the surviving candidates
@@ -322,6 +323,48 @@ struct OrderParams {
 /* Enqueue the whole ordering on `stream`, with at most maxPasses radix passes (the key needs no more for
  * the input at hand); *launches receives the number of kernels launched. */
 cudaError_t launchOrder(const OrderParams &p, u32 maxPasses, cudaStream_t stream, unsigned *launches);
+
+/* ---- row scans (rows_kernels.h): rows at any byte of a device column -> a packed corpus and its plan ---- */
+
+enum { ROWS_THREADS = 256, ROWS_ITEMS = 8, ROWS_TILE = ROWS_THREADS * ROWS_ITEMS,
+       ROWS_SPAN = 4096 /* packed bytes per warp of the repack */ };
+
+struct RowsParams {
+    /* row i = chars[offsets[i], offsets[i + 1]) */
+    const u8 *chars;
+    u64 charsBytes;
+    const u64 *offsets;
+    u32 nrows;
+    /* the packed corpus (position 0; bytes [0, zeroEnd) are written, pads and slack zero) and its block table */
+    u8 *corpus;
+    u64 zeroEnd;
+    u64 *blockOff;
+    u32 *blockLen;
+    /* temporaries: per tile of ROWS_TILE rows its padded bytes (then their exclusive prefix) and a bad row */
+    u64 *tilePad;
+    u32 *tileBad;
+    u32 *bad;        /* the verdict: the table is bad */
+    /* the pass's counters: a bad table sets STREAM_BAD_LENGTH in CTR_STREAM and raises CTR_MATCHES above outCap */
+    u32 *counters;
+    u32 outCap;
+};
+/* Enqueue the plan and the repack (after the counters are cleared, before the scan); *launches: kernels launched */
+cudaError_t launchRowPlan(const RowsParams &p, int smCount, cudaStream_t stream, unsigned *launches);
+
+/* The segment plan of an engine run over a packed row corpus whose lengths only the device knows: every row longer
+ * than cutAbove is cut into segLen-byte segments.  segs[segCap] and cuts[cutCap] are sized by the host's bound,
+ * segFirst has nrows + 1 entries. */
+struct RowSegParams {
+    const u32 *blockLen;
+    u32 nrows;
+    u32 segLen, cutAbove;
+    DfaSeg *segs;
+    u32 segCap;
+    uint2 *cuts;
+    u32 cutCap;
+    u32 *segFirst;
+};
+cudaError_t launchRowSegments(const RowSegParams &p, int smCount, cudaStream_t stream, unsigned *launches);
 
 /* accel primitives (src/nfa/shufti.c, truffle.c, vermicelli.h): first
  * position in [0,len) whose byte is in the class, or len. */

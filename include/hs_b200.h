@@ -448,6 +448,27 @@ hs_error_t hs_b200_order_records_async(const hs_database_t *db, hs_scratch_t *sc
                                        const void *d_recs, size_t n, void *d_out, size_t cap,
                                        void *d_count, void *cuda_stream);
 
+/* Scan a column of rows that is already in device memory, such as a torch jagged tensor or an Arrow large_string
+ * column: row i is d_chars[d_offsets[i], d_offsets[i + 1]), with nrows + 1 offsets in device memory (8-byte
+ * aligned); d_offsets[0] may be above 0, and neither d_chars nor any row needs an alignment.  The pass is enqueued
+ * on cuda_stream (NULL = the scratch's stream) and returns without a host wait: the device checks the offsets,
+ * packs the rows into staging memory of the scratch (grown in the call) and scans them, for every database shape
+ * hs_b200_scan_corpus_async takes.  Nothing outside [d_chars, d_chars + chars_bytes) and the offsets is read, and
+ * neither is written; both stay valid until the pass completes.  d_chars may be NULL when chars_bytes is 0.
+ * The records go into the scratch's ring as for hs_b200_scan_corpus_async (block = row index, to = end offset
+ * within the row), and hs_b200_scan_corpus_finish, hs_b200_fetch_matches, hs_b200_export_records_async and
+ * hs_b200_order_matches_async serve the pass: the delivered matches equal hs_b200_scan_blocks_collect's over the
+ * same rows from host memory.  A ring overflow is as for a corpus scan: finish returns HS_INSUFFICIENT_SPACE and
+ * grows the ring, and the caller enqueues the pass again.  A row table that decreases, ends past chars_bytes or
+ * holds a row of 4 GiB or more fails the pass: no records, the ordering reports HS_B200_ORDER_RING_OVERFLOW and
+ * finish returns HS_INVALID; the next pass is unaffected.  Refused at once: HS_INVALID for NULL arguments,
+ * misaligned offsets, nrows above 0xfffffff0, a scratch that holds no image of `db` and a database with logical
+ * combinations (their reports need the row lengths on the host); HS_DB_MODE_ERROR for a database not in block
+ * mode; HS_ARCH_ERROR for a scratch with a peer exchange registered. */
+hs_error_t hs_b200_scan_rows_async(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
+                                   const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch,
+                                   void *cuda_stream);
+
 /* Stream sets: `nstreams` streams of one HS_MODE_STREAM literal database whose
  * state (7 look-behind bytes + count, 64-bit offset: 16 bytes per stream) stays
  * in HBM between calls.  hs_b200_streams_scan() gives every stream one write
@@ -672,6 +693,8 @@ hs_error_t hs_b200_set_runtime_option(const char *key, int value);
  * out[0] engine runs that cut blocks, out[1] segments they walked, out[2] segments
  * re-walked because the start state guessed for them was wrong, out[3] bytes of those
  * re-walks, each counted up to the 16-byte piece where it met the walk from the guess.
+ * The segments of a run over rows scanned by hs_b200_scan_rows_async are its segment table's size, which
+ * the host bounds from the row count and the chars' size: at least the segments walked.
  * Waits for the scratch's stream. */
 hs_error_t hs_b200_engine_segment_stats(const hs_scratch_t *scratch, unsigned long long out[4]);
 
