@@ -149,6 +149,9 @@ def lib():
         L.hs_b200_order_matches_async.argtypes = [vp, vp, vp, C.c_size_t, vp, vp]
         L.hs_b200_order_records_async.argtypes = [vp, vp, vp, C.c_size_t, vp, C.c_size_t, vp, vp]
         L.hs_b200_scan_rows_async.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, vp]
+        L.hs_b200_report_ids.argtypes = [vp, vp, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.hs_b200_scan_corpus_mask_async.argtypes = [vp, vp, vp, vp, C.c_size_t, vp, vp]
+        L.hs_b200_scan_rows_mask_async.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, vp, C.c_size_t, vp, vp]
         L.hs_b200_db_info.argtypes = [vp, C.POINTER(DbInfo)]
         L.hs_b200_set_build_option.argtypes = [cp, C.c_int]
         L.hs_b200_set_runtime_option.argtypes = [cp, C.c_int]
@@ -401,9 +404,10 @@ def scan_blocks_collect(db, data, offsets, lengths, scratch, out):
 class Corpus:
     """Device-resident corpus (hs_b200_corpus_upload / hs_b200_corpus_wrap)."""
 
-    def __init__(self, ptr, keep=None):
+    def __init__(self, ptr, keep=None, nblocks=0):
         self.ptr = ptr
         self._keep = keep
+        self.nblocks = nblocks
 
     @staticmethod
     def upload(data, offsets, lengths, device=0):
@@ -412,7 +416,7 @@ class Corpus:
         out = C.c_void_p()
         _check(lib().hs_b200_corpus_upload(a.ctypes.data, off.ctypes.data, ln.ctypes.data, off.size,
                                            device, C.byref(out)), "corpus_upload")
-        return Corpus(out)
+        return Corpus(out, nblocks=off.size)
 
     @staticmethod
     def wrap(dev_ptr, nbytes, offsets, lengths, device=0, keep=None):
@@ -420,7 +424,7 @@ class Corpus:
         out = C.c_void_p()
         _check(lib().hs_b200_corpus_wrap(C.c_void_p(dev_ptr), nbytes, off.ctypes.data, ln.ctypes.data,
                                          off.size, device, C.byref(out)), "corpus_wrap")
-        return Corpus(out, keep)
+        return Corpus(out, keep, nblocks=off.size)
 
     def payload_bytes(self):
         return int(lib().hs_b200_corpus_bytes(self.ptr))
@@ -522,6 +526,46 @@ def scan_rows_async(db, chars, offsets, scratch, stream=None):
     nbytes = chars.numel() if hasattr(chars, "numel") else chars.size
     _check(lib().hs_b200_scan_rows_async(db.ptr, _dev_ptr(chars) if nbytes else None, nbytes, _dev_ptr(offsets),
                                          nrows, scratch.ptr, C.c_void_p(stream or 0)), "scan_rows_async")
+
+
+def report_ids(db):
+    """hs_b200_report_ids: the report ids the database can deliver, ascending (uint32); column r of a match mask is
+    report_ids(db)[r].  No GPU needed."""
+    n = C.c_size_t()
+    _check(lib().hs_b200_report_ids(db.ptr, None, 0, C.byref(n)), "report_ids count")
+    ids = np.zeros(int(n.value), dtype=np.uint32)
+    if ids.size:
+        _check(lib().hs_b200_report_ids(db.ptr, ids.ctypes.data, ids.size, C.byref(n)), "report_ids")
+    return ids
+
+
+def _words_per_block(mask, nblocks, words_per_block):
+    if words_per_block is not None:
+        return int(words_per_block)
+    nbytes = mask.numel() * mask.element_size() if hasattr(mask, "numel") else mask.nbytes
+    return nbytes // 4 // nblocks if nblocks else 0
+
+
+def scan_corpus_mask_async(db, corpus, scratch, mask, words_per_block=None, status=None, stream=None):
+    """hs_b200_scan_corpus_mask_async: one pass over the corpus that writes the match mask `mask` (a CUDA tensor of
+    nblocks x words_per_block 32-bit words, e.g. torch.empty((nblocks, words), dtype=torch.int32); numpy under the
+    SIMT emulator) and, given `status` (one 32-bit element), its status, on `stream`.  words_per_block defaults to
+    the mask's size over the block count.  Returns at once; hs_b200_scan_corpus_finish serves the pass."""
+    wpb = _words_per_block(mask, corpus.nblocks, words_per_block)
+    _check(lib().hs_b200_scan_corpus_mask_async(db.ptr, corpus.ptr, scratch.ptr, _dev_ptr(mask), wpb,
+                                                _dev_ptr(status), C.c_void_p(stream or 0)), "scan_corpus_mask_async")
+
+
+def scan_rows_mask_async(db, chars, offsets, scratch, mask, words_per_block=None, status=None, stream=None):
+    """hs_b200_scan_rows_mask_async: the same for the rows of a column in device memory (as scan_rows_async)."""
+    nrows = (offsets.numel() if hasattr(offsets, "numel") else offsets.size) - 1
+    if nrows < 0:
+        raise ValueError("offsets needs nrows + 1 entries")
+    nbytes = chars.numel() if hasattr(chars, "numel") else chars.size
+    wpb = _words_per_block(mask, nrows, words_per_block)
+    _check(lib().hs_b200_scan_rows_mask_async(db.ptr, _dev_ptr(chars) if nbytes else None, nbytes,
+                                              _dev_ptr(offsets), nrows, scratch.ptr, _dev_ptr(mask), wpb,
+                                              _dev_ptr(status), C.c_void_p(stream or 0)), "scan_rows_mask_async")
 
 
 def scan_corpus(db, corpus, scratch, fetch=True):

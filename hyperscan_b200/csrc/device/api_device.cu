@@ -622,28 +622,18 @@ hs_error_t buildImage(const hs_database_t *db, DevImage **out) {
          * a literal matcher beside it (roseBlockExec's outfix), the engine's records are tagged so
          * that the host can tell them from the literals'.  Several outfixes without a literal matcher
          * (roseBlockExec over several outfix queues) all run over every block, into one record ring */
-        const u32 k = r->queueCount;
-        if ((size_t)r->nfaInfoOffset + (size_t)k * sizeof(NfaInfo) > h->length) {
+        std::vector<EngineBytes> engines;
+        if (!outfixEngines(db, &engines)) {
             return HS_INVALID;
         }
-        for (u32 q = 0; q < k; q++) {
-            NfaInfo ni;
-            memcpy(&ni, bc + r->nfaInfoOffset + q * sizeof(NfaInfo), sizeof(ni));
-            if (ni.nfaOffset % 64 || (size_t)ni.nfaOffset + sizeof(NFA) > h->length) {
-                return HS_INVALID;
-            }
-            NFA nh;
-            memcpy(&nh, bc + ni.nfaOffset, sizeof(nh));
-            if ((size_t)ni.nfaOffset + nh.length > h->length) {
-                return HS_INVALID;
-            }
+        for (const EngineBytes &e : engines) {
             DfaParams dp;
-            const hs_error_t er = engineParams(bc + ni.nfaOffset, nh.length, &dp);
+            const hs_error_t er = engineParams(e.nfa, e.len, &dp);
             if (er != HS_SUCCESS) {
                 return er;
             }
             dp.toTag = shape == SHAPE_LITERALS_OUTFIX ? ENGINE_RECORD : 0;
-            im->engines.push_back({ni.nfaOffset, nh.length});
+            im->engines.push_back({(u32)(e.nfa - bc), e.len});
             im->engineRuns.push_back(dp);
         }
     }
@@ -1334,15 +1324,18 @@ cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u
 }
 
 /* Launch over tiles [t0, t1) of the corpus on `stream`; t0 == 0 is the first range of a
- * scan, whose counters were all cleared just before. */
+ * scan, whose counters were all cleared just before.  mask != null: a mask pass. */
 hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
-                       const ScanPlan &pl, u32 t0, u32 t1, cudaStream_t stream) {
+                       const ScanPlan &pl, u32 t0, u32 t1, cudaStream_t stream, const MaskOut *mask) {
     if (t1 <= t0) {
         return HS_SUCCESS;
     }
     if (im->kind != FK_OUTFIX) {
         ScanParams p;
         fillParams(s, im, c, pl, &p);
+        if (mask) {
+            p.mask = *mask;
+        }
         p.tileFirst = t0;
         p.ntiles = t1 - t0;
         LaunchCfg cfg = pl.cfg;
@@ -1363,7 +1356,10 @@ hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
          * alignSharedRing between them) */
         const u32 ntiles = (u32)((c->bytes + pl.tileBytes - 1) / pl.tileBytes);
         if (t1 >= ntiles) {
-            for (const DfaParams &dp : im->engineRuns) {
+            for (DfaParams dp : im->engineRuns) {
+                if (mask) {
+                    dp.mask = *mask;
+                }
                 if (!s->seg) {
                     s->seg = new (std::nothrow) SegArea();
                     if (!s->seg) {
@@ -1431,10 +1427,12 @@ struct StreamPass {
  * ranges, read the counters back.  The only place a scan's stream sequence is issued.
  * For a stream-set pass (sp), the look-behind is written in front of every write first,
  * and the streams advance -- or the set is marked -- before the counters are read back.
- * For a row scan (rows), the row plan fills c's block table and packs the rows into it first. */
+ * For a row scan (rows), the row plan fills c's block table and packs the rows into it first.
+ * For a mask pass (mask), the caller's mask is zeroed before the scan, which sets bits instead of writing records,
+ * and *status (if given) receives the pass's verdict after it. */
 hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
                        cudaStream_t stream, const Upload *up = nullptr, const StreamPass *sp = nullptr,
-                       const RowsParams *rows = nullptr) {
+                       const RowsParams *rows = nullptr, const MaskOut *mask = nullptr, u32 *status = nullptr) {
     if (s->nPeers && (im->rules.shape == SHAPE_LITERALS_OUTFIX || im->rules.shape == SHAPE_OUTFIXES)) {
         /* the engine kernel stores no records into the peers' exchange buffers, and the count it
          * publishes would cover them: an exchange of both halves' records, or of several engines',
@@ -1447,6 +1445,10 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
         return r;
     }
     CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), stream));
+    if (mask) {
+        CUDA_TRY(launchMaskClear(mask->bits, (u64)c->nblocks * mask->words, s->smCount, stream));
+        g_launches++;
+    }
     if (sp) {
         CUDA_TRY(launchStreamAssemble(c->d_data, sp->hist, (u32)c->nblocks, c->streamPitch, sp->srcLen, sp->len,
                                       sp->mark, *sp->epoch, stream));
@@ -1468,13 +1470,13 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
         }
         /* tiles wholly inside the copied prefix (plus look-ahead) */
         const u32 tEnd = covered >= c->bytes ? ntiles : covered > 16 ? (u32)((covered - 16) / pl.tileBytes) : 0;
-        r = launchRange(s, im, c, pl, tDone, tEnd, stream);
+        r = launchRange(s, im, c, pl, tDone, tEnd, stream, mask);
         if (r != HS_SUCCESS) {
             return r;
         }
         tDone = std::max(tDone, tEnd);
     }
-    r = launchRange(s, im, c, pl, tDone, ntiles, stream);
+    r = launchRange(s, im, c, pl, tDone, ntiles, stream, mask);
     if (r != HS_SUCCESS) {
         return r;
     }
@@ -1486,6 +1488,10 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
         g_launches++;
     }
     s->streamEpoch = sp ? sp->epoch : nullptr;
+    if (status) {
+        CUDA_TRY(launchMaskStatus(s->d_counters, s->outCap, status, stream));
+        g_launches++;
+    }
     if (s->nPeers) {
         ScanParams pp;
         fillParams(s, im, c, pl, &pp);
@@ -2097,34 +2103,12 @@ static hs_error_t emptyPass(hs_scratch *s, cudaStream_t st) {
                                                                                           : HS_UNKNOWN_ERROR;
 }
 
+static hs_error_t corpusPass(const hs_database_t *db, const hs_b200_corpus_t *corpus, hs_scratch_t *scratch,
+                             void *cuda_stream, bool mask, void *d_mask, size_t words_per_block, void *d_status);
+
 hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corpus_t *corpus,
                                      hs_scratch_t *scratch, void *cuda_stream) {
-    if (!scratch || !corpus) {
-        return HS_INVALID;
-    }
-    hs_error_t r = checkScanArgs(db, scratch);
-    if (r != HS_SUCCESS) {
-        return r;
-    }
-    if (markInUse(scratch)) {
-        return HS_SCRATCH_IN_USE;
-    }
-    DeviceGuard guard(scratch->device);
-    DevImage *im = nullptr;
-    r = findImage(scratch, db, &im);
-    if (r == HS_SUCCESS) {
-        cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
-        if (corpus->bytes == 0 || corpus->nblocks == 0) {
-            r = emptyPass(scratch, st);
-        } else {
-            r = enqueueScan(scratch, im, corpus, st);
-        }
-        scratch->lastCorpus = corpus;
-        scratch->lastBlocks = corpus->nblocks;
-        scratch->lastMaxLen = corpus->maxLen;
-    }
-    unmarkInUse(scratch);
-    return r;
+    return corpusPass(db, corpus, scratch, cuda_stream, false, nullptr, 0, nullptr);
 }
 
 hs_error_t hs_b200_scan_corpus_finish(hs_scratch_t *scratch, unsigned long long *nrecords,
@@ -2495,9 +2479,91 @@ static hs_error_t reserveRows(hs_scratch *s, u64 bound, size_t nrows) {
     return HS_SUCCESS;
 }
 
-hs_error_t hs_b200_scan_rows_async(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
-                                   const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch,
-                                   void *cuda_stream) {
+/* The checks of a mask pass over nblocks blocks (after those of its ordinary form), and its MaskOut: the caller's
+ * buffer (NULL only without blocks, as an empty torch tensor's) and the image's tables, uploaded with it
+ * (uploadOrderTables). */
+static hs_error_t maskArgs(const DevImage *im, size_t nblocks, void *d_mask, size_t words_per_block, void *d_status,
+                           MaskOut *m) {
+    if (im->orderStatus != HS_SUCCESS) {
+        return im->orderStatus; /* an engine program the tables cannot hold */
+    }
+    const OrderParams &t = im->orderTables;
+    if ((!d_mask && nblocks) || (uintptr_t)d_mask % 4 || (uintptr_t)d_status % 4 || words_per_block < (t.nIds + 31) / 32 ||
+        words_per_block > 0xffffffffu) {
+        return HS_INVALID;
+    }
+    m->bits = (u32 *)d_mask;
+    m->words = (u32)words_per_block;
+    m->nIds = t.nIds;
+    m->ids = t.ids;
+    m->progOff = t.progOff;
+    m->progStart = t.progStart;
+    m->reps = t.reps;
+    m->nProg = t.nProg;
+    return HS_SUCCESS;
+}
+
+/* A mask pass over no bytes: no records, every word of the mask zero, status 0 */
+static hs_error_t emptyMaskPass(hs_scratch *s, cudaStream_t st, const MaskOut &m, size_t nblocks, u32 *status) {
+    hs_error_t r = emptyPass(s, st);
+    if (r == HS_SUCCESS && (launchMaskClear(m.bits, (u64)nblocks * m.words, s->smCount, st) != cudaSuccess ||
+                            (status && launchMaskStatus(s->d_counters, s->outCap, status, st) != cudaSuccess))) {
+        r = HS_UNKNOWN_ERROR;
+    }
+    return r;
+}
+
+/* hs_b200_scan_corpus_mask_async / hs_b200_scan_rows_mask_async when mask is set, else their ordinary forms */
+static hs_error_t corpusPass(const hs_database_t *db, const hs_b200_corpus_t *corpus, hs_scratch_t *scratch,
+                             void *cuda_stream, bool mask, void *d_mask, size_t words_per_block, void *d_status) {
+    if (!scratch || !corpus) {
+        return HS_INVALID;
+    }
+    hs_error_t r = checkScanArgs(db, scratch);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    MaskOut m;
+    DevImage *im = nullptr;
+    if (mask) {
+        if (dbRose(db)->ckeyCount) {
+            return HS_INVALID; /* a combination's reports depend on the order within a block */
+        }
+        im = heldImage(scratch, db);
+        if (!im) {
+            return HS_INVALID;
+        }
+        if (scratch->nPeers) {
+            return HS_ARCH_ERROR;
+        }
+        r = maskArgs(im, corpus->nblocks, d_mask, words_per_block, d_status, &m);
+        if (r != HS_SUCCESS) {
+            return r;
+        }
+    }
+    if (markInUse(scratch)) {
+        return HS_SCRATCH_IN_USE;
+    }
+    DeviceGuard guard(scratch->device);
+    r = mask ? HS_SUCCESS : findImage(scratch, db, &im);
+    if (r == HS_SUCCESS) {
+        cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
+        if (corpus->bytes == 0 || corpus->nblocks == 0) {
+            r = mask ? emptyMaskPass(scratch, st, m, corpus->nblocks, (u32 *)d_status) : emptyPass(scratch, st);
+        } else {
+            r = enqueueScan(scratch, im, corpus, st, nullptr, nullptr, nullptr, mask ? &m : nullptr, (u32 *)d_status);
+        }
+        scratch->lastCorpus = corpus;
+        scratch->lastBlocks = corpus->nblocks;
+        scratch->lastMaxLen = corpus->maxLen;
+    }
+    unmarkInUse(scratch);
+    return r;
+}
+
+static hs_error_t rowsPass(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
+                           const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch, void *cuda_stream,
+                           bool mask, void *d_mask, size_t words_per_block, void *d_status) {
     if (!db || !scratch || !d_offsets || (uintptr_t)d_offsets % 8 || (!d_chars && chars_bytes) ||
         nrows > 0xfffffff0u) {
         return HS_INVALID;
@@ -2516,6 +2582,13 @@ hs_error_t hs_b200_scan_rows_async(const hs_database_t *db, const void *d_chars,
     if (scratch->nPeers) {
         return HS_ARCH_ERROR;
     }
+    MaskOut m;
+    if (mask) {
+        r = maskArgs(im, nrows, d_mask, words_per_block, d_status, &m);
+        if (r != HS_SUCCESS) {
+            return r;
+        }
+    }
     if (markInUse(scratch)) {
         return HS_SCRATCH_IN_USE;
     }
@@ -2524,7 +2597,7 @@ hs_error_t hs_b200_scan_rows_async(const hs_database_t *db, const void *d_chars,
     /* the packed rows take at most their bytes plus 16 per row (a row's pad, or an empty row's 16 bytes) */
     const u64 bound = (u64)chars_bytes + 16 * (u64)nrows;
     if (nrows == 0) {
-        r = emptyPass(scratch, st);
+        r = mask ? emptyMaskPass(scratch, st, m, 0, (u32 *)d_status) : emptyPass(scratch, st);
     } else {
         r = reserveRows(scratch, bound, nrows);
     }
@@ -2551,13 +2624,32 @@ hs_error_t hs_b200_scan_rows_async(const hs_database_t *db, const void *d_chars,
                                              HSB_ROUNDUP((nrows + ROWS_TILE - 1) / ROWS_TILE * sizeof(u64), 256));
         rp.counters = scratch->d_counters;
         rp.outCap = scratch->outCap;
-        r = enqueueScan(scratch, im, c, st, nullptr, nullptr, &rp);
+        r = enqueueScan(scratch, im, c, st, nullptr, nullptr, &rp, mask ? &m : nullptr, (u32 *)d_status);
     }
     scratch->lastCorpus = c;
     scratch->lastBlocks = nrows;
     scratch->lastMaxLen = chars_bytes; /* no row is longer; the device decides the radix passes the records need */
     unmarkInUse(scratch);
     return r;
+}
+
+hs_error_t hs_b200_scan_rows_async(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
+                                   const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch,
+                                   void *cuda_stream) {
+    return rowsPass(db, d_chars, chars_bytes, d_offsets, nrows, scratch, cuda_stream, false, nullptr, 0, nullptr);
+}
+
+hs_error_t hs_b200_scan_corpus_mask_async(const hs_database_t *db, const hs_b200_corpus_t *corpus,
+                                          hs_scratch_t *scratch, void *d_mask, size_t words_per_block,
+                                          void *d_status, void *cuda_stream) {
+    return corpusPass(db, corpus, scratch, cuda_stream, true, d_mask, words_per_block, d_status);
+}
+
+hs_error_t hs_b200_scan_rows_mask_async(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
+                                        const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch,
+                                        void *d_mask, size_t words_per_block, void *d_status, void *cuda_stream) {
+    return rowsPass(db, d_chars, chars_bytes, d_offsets, nrows, scratch, cuda_stream, true, d_mask, words_per_block,
+                    d_status);
 }
 
 /* ---- DFA engines in block mode ------------------------------------------------------

@@ -27,6 +27,7 @@
 #include <type_traits>
 
 #include "kernels.h"
+#include "resolve.h"
 
 namespace hsb {
 
@@ -42,7 +43,20 @@ __device__ __forceinline__ u16 g16(const u8 *p) { return __ldg(reinterpret_cast<
  * counts reserved slots. */
 enum : u32 { DFA_SLOTS = 8, DFA_NO_RECORD = 0xffffffffu };
 
+/* A mask pass: the reports of the engine's report program `prog` whose bounds admit `to` set their bits, as the
+ * ordering resolves the record (resolve.h) */
+__device__ __forceinline__ void maskEngineRecord(const DfaParams &p, u32 prog, u32 block, u64 to) {
+    programReports(p.mask.progStart, p.mask.reps, indexOf(p.mask.progOff, p.mask.nProg, prog), to,
+                   [&](const OrderRep &rp) { maskReport(p.mask, rp.onmatch, block); });
+}
+
+/* MASK: the walk of a mask pass (dfaStagedKernel) */
+template <bool MASK>
 __device__ __forceinline__ u32 emitDfaMatch(const DfaParams &p, u32 cursor, u32 id, u32 block, u64 to) {
+    if (MASK) {
+        maskEngineRecord(p, id, block, to);
+        return cursor;
+    }
     if ((cursor & (DFA_SLOTS - 1)) == 0) {
         cursor = atomicAdd(p.counters + CTR_MATCHES, (u32)DFA_SLOTS);
     }
@@ -57,10 +71,11 @@ __device__ __forceinline__ u32 emitDfaMatch(const DfaParams &p, u32 cursor, u32 
 }
 
 /* struct report_list {u32 count; ReportID report[]} at offset `off` of the engine at `nfa` */
+template <bool MASK>
 __device__ u32 emitReportList(const DfaParams &p, const u8 *nfa, u32 cursor, u32 off, u32 block, u64 to) {
     const u32 n = g32(nfa + off);
     for (u32 i = 0; i < n; i++) {
-        cursor = emitDfaMatch(p, cursor, g32(nfa + off + 4 + 4 * i), block, to);
+        cursor = emitDfaMatch<MASK>(p, cursor, g32(nfa + off + 4 + 4 * i), block, to);
     }
     return cursor;
 }
@@ -230,6 +245,7 @@ template <int W> struct StOps<WideSt<W>> {
 };
 
 /* LimEx report list: ReportID[] terminated by MO_INVALID_IDX (limexRunReports, limex_runtime.h:90-103) */
+template <bool MASK>
 __device__ HSB_NOINLINE u32 emitLimexReports(const DfaParams &p, const u8 *nfa, u32 cursor, u32 listOff, u32 block,
                                              u64 to) {
     const u8 *lx = nfa + sizeof(NFA);
@@ -238,14 +254,14 @@ __device__ HSB_NOINLINE u32 emitLimexReports(const DfaParams &p, const u8 *nfa, 
         if (id == MO_INVALID_IDX) {
             break;
         }
-        cursor = emitDfaMatch(p, cursor, id, block, to);
+        cursor = emitDfaMatch<MASK>(p, cursor, id, block, to);
     }
     return cursor;
 }
 
 /* accepts of the states in `found` through an NFAAccept table (PROCESS_ACCEPTS_IMPL_FN,
  * limex_common_impl.h:116-163; the squash of PROCESS_ACCEPTS_FN is dead code there) */
-template <class ST>
+template <class ST, bool MASK>
 __device__ HSB_NOINLINE u32 emitLimexAccepts(const DfaParams &p, const u8 *nfa, u32 cursor, ST found, ST mask,
                                              u32 tableOff, u32 block, u64 to) {
     const u8 *lx = nfa + sizeof(NFA);
@@ -254,9 +270,9 @@ __device__ HSB_NOINLINE u32 emitLimexAccepts(const DfaParams &p, const u8 *nfa, 
         const u8 *a = lx + tableOff + idx * (u32)sizeof(NFAAccept);
         const u32 reports = g32(a + offsetof(NFAAccept, reports));
         if (__ldg(a + offsetof(NFAAccept, single_report))) {
-            cursor = emitDfaMatch(p, cursor, reports, block, to);
+            cursor = emitDfaMatch<MASK>(p, cursor, reports, block, to);
         } else {
-            cursor = emitLimexReports(p, nfa, cursor, reports, block, to);
+            cursor = emitLimexReports<MASK>(p, nfa, cursor, reports, block, to);
         }
     });
     return cursor;
@@ -420,16 +436,19 @@ struct DfaConsts {
 /* reports of a state that was just entered at offset `to` (doComplexReport, mcclellan.c:43-91;
  * fireReports, sheng_impl.h:116-155).  what = the one report of a single-report engine, else
  * the offset of the state's aux record.  Returns the lane's record cursor. */
+template <bool MASK>
 __device__ HSB_NOINLINE u32 emitAccept(const DfaParams &p, const u8 *nfa, u32 cursor, u32 single, u32 what, u32 block,
                                        u64 to) {
     if (single) {
-        return emitDfaMatch(p, cursor, what, block, to);
+        return emitDfaMatch<MASK>(p, cursor, what, block, to);
     }
-    return emitReportList(p, nfa, cursor, g32(nfa + what), block, to);
+    return emitReportList<MASK>(p, nfa, cursor, g32(nfa + what), block, to);
 }
 
-/* SEG: the segment mode (p.segs, p.segMode; DESIGN.md section 10f), fused or not */
-template <int ENGINE, int SMEM_TABLE, int CH, int ILP, bool FUSED, bool SEG = false>
+/* SEG: the segment mode (p.segs, p.segMode; DESIGN.md section 10f), fused or not.  MASK: a mask pass (p.mask), whose
+ * accepts set bits instead of writing records: instantiations of their own, so that the record walks stay as they
+ * are */
+template <int ENGINE, int SMEM_TABLE, int CH, int ILP, bool FUSED, bool SEG = false, bool MASK = false>
 __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(const HSB_GRID_CONSTANT DfaParams p) {
     HSB_DYNAMIC_SMEM(smem);
     typedef DfaTile<CH> Tile;
@@ -644,7 +663,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
             Ops::forEach(Ops::band(s, tShift[8]), [&](const u32 bit) {
                 const u32 rep = reinterpret_cast<const u32 *>(smem + T::REP)[bit];
                 if (rep != MO_INVALID_IDX && pos != 0 && segEmit) {
-                    cursor = emitLimexReports(p, nfa, cursor, rep, blk, pos);
+                    cursor = emitLimexReports<MASK>(p, nfa, cursor, rep, blk, pos);
                 }
                 local = Ops::bor(local, Ops::loadChunks(reinterpret_cast<const uint4 *>(smem + T::LOCAL), T::STATES, bit));
                 if (squashes) {
@@ -671,7 +690,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                 const ST *e = lxRows + 4 * bit;
                 const u32 rep = Ops::low32(e[3]);
                 if (rep != MO_INVALID_IDX && pos != 0 && segEmit) {
-                    cursor = emitLimexReports(p, nfa, cursor, rep, blk, pos);
+                    cursor = emitLimexReports<MASK>(p, nfa, cursor, rep, blk, pos);
                 }
                 lim = Ops::bor(lim, e[0]);
                 local = Ops::bor(local, e[1]);
@@ -711,11 +730,11 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
             /* STREAM_FN's closing accept check (only if the block had bytes to stream),
              * then nfaExecLimEx*_testEOD (limex_common_impl.h:192-218) */
             if (len && Ops::any(Ops::band(s, lxAccept))) {
-                cursor = emitLimexAccepts<ST>(p, nfa, cursor, Ops::band(s, lxAccept), lxAccept,
+                cursor = emitLimexAccepts<ST, MASK>(p, nfa, cursor, Ops::band(s, lxAccept), lxAccept,
                                               g32(eng + offsetof(LxNfa, acceptOffset)), blk, len);
             }
             if (Ops::any(Ops::band(s, lxAcceptEod))) {
-                cursor = emitLimexAccepts<ST>(p, nfa, cursor, Ops::band(s, lxAcceptEod), lxAcceptEod,
+                cursor = emitLimexAccepts<ST, MASK>(p, nfa, cursor, Ops::band(s, lxAcceptEod), lxAcceptEod,
                                               g32(eng + offsetof(LxNfa, acceptEodOffset)), blk, len);
             }
         } else {
@@ -723,7 +742,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                                                    : (u32)offsetof(MStateAux, accept_eod);
             const u32 eod = g32(nfa + k.auxOffset + k.auxSize * (Ops::low32(s) & k.stateMask) + eodOff);
             if (eod) {
-                cursor = emitReportList(p, nfa, cursor, eod, blk, len);
+                cursor = emitReportList<MASK>(p, nfa, cursor, eod, blk, len);
             }
         }
     };
@@ -860,7 +879,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                             const u32 x = myRow[c];
                             walked++;
                             if (step(x, 0, s, at + c, sg.block) && segEmit) {
-                                cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s), sg.block, (u64)at + c + 1);
+                                cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s), sg.block, (u64)at + c + 1);
                             }
                             if (cmp) {
                                 (void)step(x, 0, alt, at + c, sg.block);
@@ -902,7 +921,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll
                             for (u32 jj = 0; jj < 16; jj++) {
                                 if (step(w[jj >> 2], jj & 3, s, at + cc * 16 + jj, sg.block) && segEmit) {
-                                    cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s), sg.block,
+                                    cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s), sg.block,
                                                         (u64)at + cc * 16 + jj + 1);
                                 }
                             }
@@ -914,7 +933,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll 1
                             for (u32 jj = 0; jj < m - cc * 16; jj++) {
                                 if (step(w[jj >> 2] >> (8 * (jj & 3)), 0, s, at + cc * 16 + jj, sg.block) && segEmit) {
-                                    cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s), sg.block,
+                                    cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s), sg.block,
                                                         (u64)at + cc * 16 + jj + 1);
                                 }
                             }
@@ -1052,7 +1071,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll
                         for (int u = 0; u < ILP; u++) {
                             if (step(w[u][j >> 2], j & 3, s[u], done + c * 16 + j, b[u])) {
-                                cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + c * 16 + j + 1);
+                                cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + c * 16 + j + 1);
                             }
                         }
                     }
@@ -1086,7 +1105,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll
                         for (u32 j = 0; j < 16; j++) {
                             if (step(w[j >> 2], j & 3, s[u], done + cc * 16 + j, b[u])) {
-                                cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
+                                cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
                             }
                         }
                         live[u] = !dead(s[u]);
@@ -1098,7 +1117,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll 1
                         for (u32 j = 0; j < m; j++) {
                             if (step(w[j >> 2] >> (8 * (j & 3)), 0, s[u], done + cc * 16 + j, b[u])) {
-                                cursor = emitAccept(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
+                                cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
                             }
                         }
                         live[u] = !dead(s[u]);
@@ -1115,11 +1134,11 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                     /* STREAM_FN's closing accept check (only if the block had bytes to stream),
                      * then nfaExecLimEx*_testEOD (limex_common_impl.h:192-218) */
                     if (len[u] && Ops::any(Ops::band(s[u], lxAccept))) {
-                        cursor = emitLimexAccepts<ST>(p, nfa, cursor, Ops::band(s[u], lxAccept), lxAccept,
+                        cursor = emitLimexAccepts<ST, MASK>(p, nfa, cursor, Ops::band(s[u], lxAccept), lxAccept,
                                                       g32(eng + offsetof(LxNfa, acceptOffset)), b[u], len[u]);
                     }
                     if (Ops::any(Ops::band(s[u], lxAcceptEod))) {
-                        cursor = emitLimexAccepts<ST>(p, nfa, cursor, Ops::band(s[u], lxAcceptEod), lxAcceptEod,
+                        cursor = emitLimexAccepts<ST, MASK>(p, nfa, cursor, Ops::band(s[u], lxAcceptEod), lxAcceptEod,
                                                       g32(eng + offsetof(LxNfa, acceptEodOffset)), b[u], len[u]);
                     }
                 }
@@ -1128,7 +1147,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                                                        : (u32)offsetof(MStateAux, accept_eod);
                 const u32 eod = g32(nfa + k.auxOffset + k.auxSize * (Ops::low32(s[u]) & k.stateMask) + eodOff);
                 if (eod) {
-                    cursor = emitReportList(p, nfa, cursor, eod, b[u], len[u]);
+                    cursor = emitReportList<MASK>(p, nfa, cursor, eod, b[u], len[u]);
                 }
             }
         }
@@ -1144,17 +1163,22 @@ cudaError_t launchStaged(const DfaParams &p, int smCount, size_t tableBytes, cud
     const int threads = StagedThreads<ENGINE>::N;
     /* (the wide models, a fused launch and a segmented one walk one block or segment per lane) */
     const bool fused = p.engines != nullptr, seg = p.segs != nullptr;
-    const bool two = !fused && !seg && p.ilp == 2 && ENGINE < ENG_LIMEX128;
+    const bool mask = p.mask.bits != nullptr; /* (a mask pass walks one block or segment per lane) */
+    const bool two = !fused && !seg && !mask && p.ilp == 2 && ENGINE < ENG_LIMEX128;
     const size_t tiles = (size_t)(threads / 32) * (two ? 2 * DfaTile<64>::WARP_BYTES : DfaTile<128>::WARP_BYTES);
     const u64 units = !seg ? p.nblocks : p.segMode == SEG_SETTLE ? p.ncuts : p.nsegs;
     const u64 groups = (units + (two ? 63 : 31)) / (two ? 64 : 32);
     /* per engine: `grid` CTAs over all blocks (a fused launch has that many per engine, and the CTAs of every
      * engine share the GPU: a corpus too small to fill it for one engine fills it for several) */
     const int grid = (int)std::min<u64>((u64)smCount, (groups + threads / 32 - 1) / (threads / 32));
-    void (*kern)(const DfaParams) = seg     ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, true>
-                                    : fused ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, true>
-                                    : two ? dfaStagedKernel<ENGINE, SMEM_TABLE, 64, 2, false>
-                                          : dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false>;
+    void (*kern)(const DfaParams) =
+        mask ? (seg     ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, true, true>
+                : fused ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, true, false, true>
+                        : dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, false, true>)
+             : seg     ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, true>
+             : fused   ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, true>
+             : two     ? dfaStagedKernel<ENGINE, SMEM_TABLE, 64, 2, false>
+                       : dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false>;
     const size_t smem = tableBytes + tiles;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) {
@@ -1187,7 +1211,8 @@ cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t
     if (!p.nblocks) {
         return cudaSuccess;
     }
-    if (p.toTag && (!p.segs || p.segMode == SEG_EMIT)) { /* (the passes before SEG_EMIT write no records) */
+    if (p.toTag && !p.mask.bits && (!p.segs || p.segMode == SEG_EMIT)) { /* (the passes before SEG_EMIT and a mask
+                                                                           * pass write no records) */
         HSB_LAUNCH(alignSharedRing, 1, 1, 0, stream, p);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) {

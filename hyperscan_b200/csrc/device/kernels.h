@@ -76,6 +76,29 @@ struct DevCand {
 };
 enum { ERR_BAD_OPCODE = 1, ERR_INTERNAL = 2 };
 
+/* a report instruction an engine's program reaches (db_walk.h ProgReport) */
+struct OrderRep {
+    u32 onmatch;
+    s32 adjust;
+    u64 lo, hi;    /* CHECK_BOUNDS on the record's end offset */
+    u32 logical;   /* SET_LOGICAL: the record becomes a logical-key record */
+    u32 pad;
+};
+
+/* A match-mask pass (hs_b200_scan_corpus_mask_async / hs_b200_scan_rows_mask_async): where a record would be
+ * written, the match sets bit r % 32 of bits[block * words + r / 32] instead, r = the rank of its report id in
+ * ids[0, nIds) (DeviceRules.ids).  An engine's record (a report program) first becomes the reports its program
+ * raises, through the program tables the ordering uses (resolve.h). */
+struct MaskOut {
+    u32 *bits;       /* null: the pass writes records */
+    u32 words;       /* per block */
+    u32 nIds;
+    const u32 *ids;
+    const u32 *progOff, *progStart;
+    const OrderRep *reps;
+    u32 nProg;
+};
+
 struct ScanParams {
     /* corpus: position 0 = first byte of the packed corpus; bytes
      * [-16, paddedBytes + 16) are readable; blocks start 16-byte aligned */
@@ -130,6 +153,7 @@ struct ScanParams {
     u32 peerCap;
     u32 blockBase;           /* added to block indices in exchanged records */
     DevMatch *peers[MAX_PEERS];
+    MaskOut mask;            /* mask.bits != null: a mask pass (the confirm kernel sets bits, writes no records) */
 };
 
 struct LaunchCfg {
@@ -156,6 +180,12 @@ cudaError_t launchConfirm(const LaunchCfg &cfg, const ScanParams &p, cudaStream_
 /* Publish the record count of a finished scan into slot 0 of this rank's
  * region in every peer's exchange buffer (runs after the scan on its stream). */
 cudaError_t launchPublishCount(const ScanParams &p, cudaStream_t stream);
+
+/* The two ends of a mask pass: zero the n words of the caller's mask (after the counters are cleared, before the
+ * scan), and write its status from the pass's counters (after the scan): 0 when the mask is valid, 1 when
+ * hs_b200_scan_corpus_finish will not return HS_SUCCESS (an error, a bad row table or a candidate-list overflow). */
+cudaError_t launchMaskClear(u32 *bits, u64 n, int smCount, cudaStream_t stream);
+cudaError_t launchMaskStatus(const u32 *counters, u32 outCap, u32 *status, cudaStream_t stream);
 
 /* A stream set's pass state in device memory.  A pass whose record ring or candidate list overflowed, or
  * whose device lengths were bad, does not advance its streams and marks the set; every later pass or reset on
@@ -249,6 +279,7 @@ struct DfaParams {
     unsigned long long *segStats; /* SEGSTAT_COUNT counters, accumulated */
     u32 *segOpen;    /* per engine of the launch, per block: the first segment whose start is not settled (SEG_CHECK;
                       * all ones = none), cleared by the caller */
+    MaskOut mask;    /* mask.bits != null: a mask pass (the accepts set bits, no slot is reserved or written) */
 };
 cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t stream);
 
@@ -262,15 +293,6 @@ cudaError_t launchDfaSegments(const DfaParams &p, int smCount, int maxSmem, u32 
                               unsigned *launches);
 
 /* ---- the report rules on the device (order_kernels.h): raw records -> delivered matches ---- */
-
-/* a report instruction an engine's program reaches (db_walk.h ProgReport) */
-struct OrderRep {
-    u32 onmatch;
-    s32 adjust;
-    u64 lo, hi;    /* CHECK_BOUNDS on the record's end offset */
-    u32 logical;   /* SET_LOGICAL: the record becomes a logical-key record */
-    u32 pad;
-};
 
 enum { ORDER_THREADS = 256, ORDER_ITEMS = 8, ORDER_TILE = ORDER_THREADS * ORDER_ITEMS,
        ORDER_MAX_PASSES = 16 /* 8-bit digits of a key of 32 (block) + 64 (to) + 32 (id) bits */ };

@@ -32,6 +32,7 @@
 
 #include "../host/db_walk.h"
 #include "kernels.h"
+#include "resolve.h"
 
 namespace hsb {
 
@@ -96,40 +97,10 @@ __device__ u32 blockExclusive(u32 v, u32 *sm, u32 *total) {
 }
 
 /* index of program `off` in the table, or -1 */
-__device__ int findProgram(const OrderParams &p, u32 off) {
-    u32 lo = 0, hi = p.nProg;
-    while (lo < hi) {
-        const u32 mid = (lo + hi) >> 1;
-        const u32 v = __ldg(p.progOff + mid);
-        if (v == off) {
-            return (int)mid;
-        }
-        if (v < off) {
-            lo = mid + 1;
-        } else {
-            hi = mid;
-        }
-    }
-    return -1;
-}
+__device__ int findProgram(const OrderParams &p, u32 off) { return indexOf(p.progOff, p.nProg, off); }
 
 /* dense rank of report id `id`, or -1 */
-__device__ int rankOf(const OrderParams &p, u32 id) {
-    u32 lo = 0, hi = p.nIds;
-    while (lo < hi) {
-        const u32 mid = (lo + hi) >> 1;
-        const u32 v = __ldg(p.ids + mid);
-        if (v == id) {
-            return (int)mid;
-        }
-        if (v < id) {
-            lo = mid + 1;
-        } else {
-            hi = mid;
-        }
-    }
-    return -1;
-}
+__device__ int rankOf(const OrderParams &p, u32 id) { return indexOf(p.ids, p.nIds, id); }
 
 /* What one raw record becomes (ReportRules::deliver): *prog = -1 and 1 record as it is (a literal's), or
  * the program whose reports replace it (0 records for a padding slot or a program not in the table). */
@@ -160,14 +131,7 @@ __device__ Resolved resolveOne(const OrderParams &p, DevMatch r) {
         return x;
     }
     x.prog = findProgram(p, r.id);
-    if (x.prog < 0) {
-        return x;
-    }
-    const u32 e = __ldg(p.progStart + x.prog + 1);
-    for (u32 k = __ldg(p.progStart + x.prog); k < e; k++) {
-        const OrderRep &rp = p.reps[k];
-        x.count += r.to >= rp.lo && r.to <= rp.hi;
-    }
+    x.count = programReports(p.progStart, p.reps, x.prog, r.to, [](const OrderRep &) {});
     return x;
 }
 
@@ -291,17 +255,12 @@ __global__ void __launch_bounds__(ORDER_THREADS) resolveScatterKernel(const Orde
         if (x.count && x.prog < 0) {
             emit(x.r);
         } else if (x.count) {
-            const u32 e = __ldg(p.progStart + x.prog + 1);
-            for (u32 q = __ldg(p.progStart + x.prog); q < e; q++) {
-                const OrderRep rp = p.reps[q];
-                if (x.r.to < rp.lo || x.r.to > rp.hi) {
-                    continue;
-                }
+            programReports(p.progStart, p.reps, x.prog, x.r.to, [&](const OrderRep &rp) {
                 DevMatch o = x.r;
                 o.id = rp.onmatch;
                 o.to = (u64)((long long)x.r.to + rp.adjust) | (rp.logical ? LKEY_RECORD : 0);
                 emit(o);
-            }
+            });
         }
     }
     warpMax(maxBlock);

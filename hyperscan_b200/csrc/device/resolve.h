@@ -1,0 +1,75 @@
+/*
+ * resolve.h -- the report tables of a database on the device (DeviceRules, uploaded with its image), and what one
+ * match becomes through them: the look-ups the ordering (order_kernels.h) and the match mask (scan_kernels.cu,
+ * dfa_kernels.cu) share.  Each translation unit that includes it gets its own copy of these inline functions.
+ */
+#ifndef HSB200_RESOLVE_H
+#define HSB200_RESOLVE_H
+
+#include "kernels.h"
+
+namespace hsb {
+
+namespace {
+
+/* index of v in the ascending table[0, n), or -1 (a program offset in progOff, a report id in ids) */
+__device__ __forceinline__ int indexOf(const u32 *table, u32 n, u32 v) {
+    u32 lo = 0, hi = n;
+    while (lo < hi) {
+        const u32 mid = (lo + hi) >> 1;
+        const u32 t = __ldg(table + mid);
+        if (t == v) {
+            return (int)mid;
+        }
+        if (t < v) {
+            lo = mid + 1;
+        } else {
+            hi = mid;
+        }
+    }
+    return -1;
+}
+
+/* The reports an engine's record raises (ReportRules::deliver): f(rep) for each report instruction of program k
+ * (its index in progOff; -1 = none) whose CHECK_BOUNDS admits the record's end offset `to`.  Returns how many. */
+template <class F>
+__device__ __forceinline__ u32 programReports(const u32 *progStart, const OrderRep *reps, int k, u64 to, F f) {
+    if (k < 0) {
+        return 0;
+    }
+    u32 n = 0;
+    const u32 e = __ldg(progStart + k + 1);
+    for (u32 q = __ldg(progStart + k); q < e; q++) {
+        const OrderRep &rp = reps[q];
+        const bool in = to >= rp.lo && to <= rp.hi;
+        if (in) {
+            f(rp);
+        }
+        n += in;
+    }
+    return n;
+}
+
+/* A mask pass: set the bit of report id `id` in row `block` (an id outside the table sets none).  The word is
+ * read first, so that an id that fires again in the same block costs a load, not an atomic: bits only go from 0
+ * to 1 during the pass, so a stale read can only send a match to the atomic. */
+__device__ __forceinline__ void maskReport(const MaskOut &m, u32 id, u32 block) {
+    const int r = indexOf(m.ids, m.nIds, id);
+    if (r < 0) {
+        return;
+    }
+    u32 *w = m.bits + (u64)block * m.words + ((u32)r >> 5);
+    const u32 bit = 1u << ((u32)r & 31);
+    if (!(*w & bit)) {
+#ifdef HSB_HOST_EMU /* the SIMT emulator of tests/emu runs one thread at a time between its barriers */
+        *w |= bit;
+#else
+        atomicOr(w, bit);
+#endif
+    }
+}
+
+} // namespace
+
+} // namespace hsb
+#endif

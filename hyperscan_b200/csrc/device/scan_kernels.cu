@@ -39,7 +39,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 #include "kernels.h"
+#include "resolve.h"
 
 namespace hsb {
 
@@ -156,6 +159,10 @@ __device__ bool findBlock(const ScanParams &p, u64 g, BlockRef *out) {
 }
 
 __device__ __forceinline__ void emitMatch(const ScanParams &p, u32 id, u32 block, u64 to) {
+    if (p.mask.bits) {
+        maskReport(p.mask, id, block); /* (no logical-key record: a database with combinations is refused) */
+        return;
+    }
     const u32 i = atomicAdd(p.counters + CTR_MATCHES, 1u);
     if (i < p.outCap) {
         DevMatch m;
@@ -1692,6 +1699,33 @@ __global__ void publishCountKernel(const ScanParams p) {
     }
 }
 } // namespace
+
+namespace {
+__global__ void maskClearKernel(u32 *bits, u64 n) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+        bits[i] = 0;
+    }
+}
+
+/* the verdict hs_b200_scan_corpus_finish reaches from the same counters (finishScan) */
+__global__ void maskStatusKernel(const u32 *counters, u32 outCap, u32 *status) {
+    *status = counters[CTR_ERROR] || (counters[CTR_STREAM] & STREAM_BAD_LENGTH) || counters[CTR_MATCHES] > outCap;
+}
+} // namespace
+
+cudaError_t launchMaskClear(u32 *bits, u64 n, int smCount, cudaStream_t stream) {
+    if (!n) {
+        return cudaSuccess;
+    }
+    const u64 blocks = std::min<u64>((n + 255) / 256, (u64)std::max(1, smCount) * 8);
+    HSB_LAUNCH(maskClearKernel, (unsigned)blocks, 256, 0, stream, bits, n);
+    return cudaGetLastError();
+}
+
+cudaError_t launchMaskStatus(const u32 *counters, u32 outCap, u32 *status, cudaStream_t stream) {
+    HSB_LAUNCH(maskStatusKernel, 1, 1, 0, stream, counters, outCap, status);
+    return cudaGetLastError();
+}
 
 namespace {
 __global__ void streamAssembleKernel(u8 *corpus, const u8 *hist, u32 nstreams, u32 pitch, const u32 *srcLens,

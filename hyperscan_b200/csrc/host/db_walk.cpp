@@ -687,6 +687,31 @@ bool enginePrograms(const u8 *nfa, u32 len, std::vector<u32> *out) {
 
 } // namespace
 
+bool outfixEngines(const hs_database_t *db, std::vector<EngineBytes> *out) {
+    const DbHeader *h = (const DbHeader *)db;
+    const RoseEngine *r = dbRose(db);
+    const u8 *bc = (const u8 *)r;
+    const u32 k = r->queueCount;
+    out->clear();
+    if ((size_t)r->nfaInfoOffset + (size_t)k * sizeof(NfaInfo) > h->length) {
+        return false;
+    }
+    for (u32 q = 0; q < k; q++) {
+        NfaInfo ni;
+        memcpy(&ni, bc + r->nfaInfoOffset + q * sizeof(NfaInfo), sizeof(ni));
+        if (ni.nfaOffset % 64 || (size_t)ni.nfaOffset + sizeof(NFA) > h->length) {
+            return false;
+        }
+        NFA nh;
+        memcpy(&nh, bc + ni.nfaOffset, sizeof(nh));
+        if ((size_t)ni.nfaOffset + nh.length > h->length) {
+            return false;
+        }
+        out->push_back({bc + ni.nfaOffset, nh.length});
+    }
+    return true;
+}
+
 hs_error_t buildDeviceRules(ReportRules *rules, const std::vector<EngineBytes> &engines, DeviceRules *out) {
     *out = DeviceRules();
     if (!engines.empty()) {
@@ -773,6 +798,44 @@ hs_error_t ReportRules::deliver(std::vector<DevMatch> *v, const u32 *lengths, si
 }
 
 } // namespace hsb
+
+extern "C" hs_error_t hs_b200_report_ids(const hs_database_t *db, unsigned int *ids, size_t cap, size_t *count) {
+    if (!db || !count || (cap && !ids)) {
+        return HS_INVALID;
+    }
+    const hsb::DbHeader *h = (const hsb::DbHeader *)db;
+    if (h->magic != hsb::DB_MAGIC) {
+        return HS_INVALID;
+    }
+    hsb::ReportRules rules;
+    hs_error_t r = hsb::loadReportRules(db, &rules);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    std::vector<hsb::EngineBytes> engines;
+    if (rules.shape != hsb::SHAPE_PURE_LITERAL && !hsb::outfixEngines(db, &engines)) {
+        return HS_INVALID;
+    }
+    hsb::DeviceRules dr;
+    r = hsb::buildDeviceRules(&rules, engines, &dr);
+    if (r != HS_SUCCESS) {
+        return r;
+    }
+    /* the combinations' own reports, which the host adds when it orders the records */
+    std::set<unsigned int> all(dr.ids.begin(), dr.ids.end());
+    for (const hsb::CombInfo &ci : rules.comb.combs) {
+        all.insert(ci.id);
+    }
+    *count = all.size();
+    if (!ids) {
+        return HS_SUCCESS;
+    }
+    if (cap < all.size()) {
+        return HS_INSUFFICIENT_SPACE;
+    }
+    std::copy(all.begin(), all.end(), ids);
+    return HS_SUCCESS;
+}
 
 extern "C" hs_error_t hs_b200_postprocess_matches(const hs_database_t *db, hs_b200_match_t *recs,
                                                   size_t n, unsigned long long *nout) {

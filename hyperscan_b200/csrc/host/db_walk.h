@@ -139,6 +139,9 @@ struct EngineBytes {
     const u8 *nfa;
     u32 len;
 };
+/* The engines of a database with outfixes (queues [0, queueCount)), in queue order; false when its queue table or
+ * an engine does not lie inside its bytecode. */
+bool outfixEngines(const hs_database_t *db, std::vector<EngineBytes> *out);
 /* Walk every report program of the engines (none for a pure-literal database) as ReportRules::deliver
  * would on meeting it, which completes rules->progReports and rules->exhaustible, and lay the rules out
  * as tables.  HS_INVALID: an engine's report lists run past its end; HS_UNKNOWN_ERROR: a program holds an

@@ -469,6 +469,38 @@ hs_error_t hs_b200_scan_rows_async(const hs_database_t *db, const void *d_chars,
                                    const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch,
                                    void *cuda_stream);
 
+/* Match masks: which report ids fire in which block, as a bit matrix of fixed size in device memory instead of
+ * match records -- the answer a filter or a tagger needs, with no record ring to overflow and nothing to order.
+ *
+ * The report ids a database can deliver, ascending and distinct: column r of a match mask is ids[r].  *count
+ * receives their number; ids may be NULL with cap 0 to query it (HS_INSUFFICIENT_SPACE: cap below *count, nothing
+ * written).  Host only (needs no CUDA device); every database shape the device scans is taken, and for a database
+ * with logical combinations the list holds the combinations' ids too. */
+hs_error_t hs_b200_report_ids(const hs_database_t *db, unsigned int *ids, size_t cap, size_t *count);
+/* The same pass as hs_b200_scan_corpus_async / hs_b200_scan_rows_async, but instead of match records it writes
+ * d_mask: nblocks rows of words_per_block 32-bit words (device memory, 4-byte aligned; NULL only when there are no
+ * blocks).  Bit r of row b (word
+ * r / 32, bit r % 32) is set iff hs_scan of block b would deliver at least one match with id ids[r] -- equivalently,
+ * iff hs_b200_fetch_matches after the ordinary pass holds a record (b, *, ids[r]).  The pass writes every word of
+ * the mask, zeroes included; words_per_block >= ceil(count / 32), with ids and count as hs_b200_report_ids gives
+ * them.  d_status (optional, a device u32): 0 when the mask is valid, non-zero when the pass must be enqueued again
+ * after hs_b200_scan_corpus_finish (candidate-list overflow: HS_INSUFFICIENT_SPACE, list grown; bad row table:
+ * HS_INVALID), so that a pipeline can test it on the device with no host wait.  The pass is enqueued on
+ * cuda_stream (NULL = the scratch's stream) and returns at once; d_mask and d_status stay valid until it completes.
+ * A mask pass writes no records: after it, hs_b200_scan_corpus_finish reports 0 records (or the overflow above),
+ * hs_b200_fetch_matches delivers none, hs_b200_order_matches_async writes a count of 0 (HS_B200_ORDER_RING_OVERFLOW
+ * after an overflow) and hs_b200_export_records_async a count of 0.  Refused at once, as the ordinary calls refuse
+ * them: HS_INVALID for NULL or misaligned arguments, a scratch that holds no image of `db`, words_per_block too
+ * small and a database with logical combinations (their reports depend on the order within a block);
+ * HS_DB_MODE_ERROR for a database not in block mode; HS_ARCH_ERROR for a scratch with a peer exchange registered. */
+hs_error_t hs_b200_scan_corpus_mask_async(const hs_database_t *db, const hs_b200_corpus_t *corpus,
+                                          hs_scratch_t *scratch, void *d_mask, size_t words_per_block,
+                                          void *d_status, void *cuda_stream);
+hs_error_t hs_b200_scan_rows_mask_async(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
+                                        const unsigned long long *d_offsets, size_t nrows,
+                                        hs_scratch_t *scratch, void *d_mask, size_t words_per_block,
+                                        void *d_status, void *cuda_stream);
+
 /* Stream sets: `nstreams` streams of one HS_MODE_STREAM literal database whose
  * state (7 look-behind bytes + count, 64-bit offset: 16 bytes per stream) stays
  * in HBM between calls.  hs_b200_streams_scan() gives every stream one write
