@@ -115,6 +115,8 @@ def lib():
         L.hs_b200_streams_close.argtypes = [vp]
         L.hs_b200_streams_scan_async.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint, vp, vp]
         L.hs_b200_streams_reset_async.argtypes = [vp, vp, C.c_size_t, vp]
+        L.hs_b200_streams_scan_rows_async.argtypes = [vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp, vp]
+        L.hs_b200_streams_read_state.argtypes = [vp, vp, vp]
         L.hs_b200_streams_state_bytes.argtypes = [vp]
         L.hs_b200_streams_state_bytes.restype = C.c_size_t
         L.hs_open_stream.argtypes = [vp, C.c_uint, C.POINTER(vp)]
@@ -724,6 +726,35 @@ class StreamSet:
             d_len, uni = _dev_ptr(lengths), 0
         _check(lib().hs_b200_streams_scan_async(self.ptr, _dev_ptr(writes), int(pitch), d_len, uni, scratch.ptr,
                                                 C.c_void_p(stream or 0)), "streams_scan_async")
+
+    def scan_rows_async(self, chars, offsets, stream_ids, scratch, stream=None):
+        """hs_b200_streams_scan_rows_async: one pass over rows already in device memory, as traffic arrives --
+        `chars` a uint8 CUDA tensor, `offsets` an int64 CUDA tensor of nrows + 1 entries, row r =
+        chars[offsets[r]:offsets[r + 1]], written to stream `stream_ids[r]` (an int32 / uint32 CUDA tensor of nrows
+        entries; numpy arrays under the SIMT emulator) -- in row order.  Enqueued on `stream` (a cudaStream_t
+        address; None = the scratch's stream); returns at once.  The records (block = row, to = stream offset) are
+        served by scan_corpus_finish, fetch_matches and order_matches_async(self.db, ...)."""
+        for x, dts in ((chars, ("uint8",)), (offsets, ("int64", "uint64")), (stream_ids, ("int32", "uint32"))):
+            name = str(x.dtype).replace("torch.", "")
+            if name not in dts:
+                raise ValueError("expected %s, got %s" % (dts[0], name))
+        nrows = (offsets.numel() if hasattr(offsets, "numel") else offsets.size) - 1
+        nids = stream_ids.numel() if hasattr(stream_ids, "numel") else stream_ids.size
+        if nrows < 0 or nids != nrows:
+            raise ValueError("offsets needs nrows + 1 entries and stream_ids nrows")
+        nbytes = chars.numel() if hasattr(chars, "numel") else chars.size
+        _check(lib().hs_b200_streams_scan_rows_async(self.ptr, _dev_ptr(chars) if nbytes else None, nbytes,
+                                                     _dev_ptr(offsets), _dev_ptr(stream_ids) if nrows else None,
+                                                     nrows, scratch.ptr, C.c_void_p(stream or 0)),
+               "streams_scan_rows_async")
+
+    def state(self):
+        """hs_b200_streams_read_state: (look-behind, nstreams x 8 uint8; offsets, nstreams uint64), once every pass
+        enqueued on the set has run"""
+        lb = np.zeros((self.n, 8), dtype=np.uint8)
+        off = np.zeros(self.n, dtype=np.uint64)
+        _check(lib().hs_b200_streams_read_state(self.ptr, lb.ctypes.data, off.ctypes.data), "streams_read_state")
+        return lb, off
 
     def reset_async(self, indices, stream):
         """hs_b200_streams_reset_async: end the flows of the streams listed in `indices` (a device array of

@@ -36,6 +36,7 @@
 #include "kernels.h"
 #include "order_kernels.h"
 #include "rows_kernels.h"
+#include "stream_rows_kernels.h"
 
 using namespace hsb;
 
@@ -872,7 +873,8 @@ struct hs_scratch {
     /* temporaries of hs_b200_order_*_async (order_kernels.h), grown on demand */
     u8 *d_order;
     size_t orderBytes;
-    /* of hs_b200_scan_rows_async: the staging corpus, and the plan's temporaries (rows_kernels.h), grown on demand */
+    /* of hs_b200_scan_rows_async and hs_b200_streams_scan_rows_async: the staging corpus, and the plan's temporaries
+     * (rows_kernels.h, stream_rows_kernels.h), grown on demand */
     hs_b200_corpus *rowsCorpus;
     u8 *d_rows;
     size_t rowsBytes;
@@ -1428,11 +1430,14 @@ struct StreamPass {
  * For a stream-set pass (sp), the look-behind is written in front of every write first,
  * and the streams advance -- or the set is marked -- before the counters are read back.
  * For a row scan (rows), the row plan fills c's block table and packs the rows into it first.
+ * For a stream-set pass over rows (srows), the rows are grouped by stream and packed into c first, and the records
+ * are rewritten to rows and stream offsets and the streams advance -- or the set is marked -- after the scan.
  * For a mask pass (mask), the caller's mask is zeroed before the scan, which sets bits instead of writing records,
  * and *status (if given) receives the pass's verdict after it. */
 hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
                        cudaStream_t stream, const Upload *up = nullptr, const StreamPass *sp = nullptr,
-                       const RowsParams *rows = nullptr, const MaskOut *mask = nullptr, u32 *status = nullptr) {
+                       const RowsParams *rows = nullptr, const MaskOut *mask = nullptr, u32 *status = nullptr,
+                       const StreamRowsParams *srows = nullptr) {
     if (s->nPeers && (im->rules.shape == SHAPE_LITERALS_OUTFIX || im->rules.shape == SHAPE_OUTFIXES)) {
         /* the engine kernel stores no records into the peers' exchange buffers, and the count it
          * publishes would cover them: an exchange of both halves' records, or of several engines',
@@ -1457,6 +1462,12 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
     if (rows) {
         unsigned launched = 0;
         CUDA_TRY(launchRowPlan(*rows, s->smCount, stream, &launched));
+        g_launches += launched;
+    }
+    if (srows) {
+        unsigned launched = 0;
+        CUDA_TRY(cudaMemsetAsync(srows->head, 0, sizeof(StreamRowsHead), stream));
+        CUDA_TRY(launchStreamRowsPlan(*srows, s->smCount, stream, &launched));
         g_launches += launched;
     }
     CUDA_TRY(cudaEventRecord(s->evStart, stream));
@@ -1486,6 +1497,11 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
                                      c->streamPitch, sp->histReq, s->d_counters, s->outCap, sp->mark, *sp->epoch,
                                      stream));
         g_launches++;
+    }
+    if (srows) {
+        unsigned launched = 0;
+        CUDA_TRY(launchStreamRowsCommit(*srows, s->smCount, stream, &launched));
+        g_launches += launched;
     }
     s->streamEpoch = sp ? sp->epoch : nullptr;
     if (status) {
@@ -2448,8 +2464,9 @@ hs_error_t hs_b200_order_records_async(const hs_database_t *db, hs_scratch_t *sc
 
 /* ---- row scans: a column of rows in device memory -------------------------------------------------------------- */
 
-/* The staging corpus of a row scan (`bound` bytes packed, nrows blocks) and the row plan's temporaries */
-static hs_error_t reserveRows(hs_scratch *s, u64 bound, size_t nrows) {
+/* The staging corpus of a row scan (`bound` bytes packed, nrows blocks) and `need` bytes of temporaries for its
+ * plan */
+static hs_error_t reserveRows(hs_scratch *s, u64 bound, size_t nrows, size_t need) {
     if (!s->rowsCorpus) {
         s->rowsCorpus = new (std::nothrow) hs_b200_corpus();
         if (!s->rowsCorpus) {
@@ -2467,8 +2484,6 @@ static hs_error_t reserveRows(hs_scratch *s, u64 bound, size_t nrows) {
         /* the front pad of a new allocation is zeroed on the legacy stream: done before any pass reads it */
         CUDA_TRY(cudaDeviceSynchronize());
     }
-    const size_t ntiles = (nrows + ROWS_TILE - 1) / ROWS_TILE;
-    const size_t need = 256 + HSB_ROUNDUP(ntiles * sizeof(u64), 256) + ntiles * sizeof(u32);
     if (need > s->rowsBytes) {
         cudaFree(s->d_rows); /* (synchronises with any pass still using it) */
         s->d_rows = nullptr;
@@ -2599,7 +2614,8 @@ static hs_error_t rowsPass(const hs_database_t *db, const void *d_chars, size_t 
     if (nrows == 0) {
         r = mask ? emptyMaskPass(scratch, st, m, 0, (u32 *)d_status) : emptyPass(scratch, st);
     } else {
-        r = reserveRows(scratch, bound, nrows);
+        const size_t ntiles = (nrows + ROWS_TILE - 1) / ROWS_TILE;
+        r = reserveRows(scratch, bound, nrows, 256 + HSB_ROUNDUP(ntiles * sizeof(u64), 256) + ntiles * sizeof(u32));
     }
     hs_b200_corpus *c = scratch->rowsCorpus;
     if (r == HS_SUCCESS && nrows) {
@@ -3371,6 +3387,22 @@ hs_error_t hs_b200_streams_close(hs_b200_stream_set_t *s) {
 
 size_t hs_b200_streams_state_bytes(const hs_b200_stream_set_t *s) { return s ? s->nstreams * 16 : 0; }
 
+hs_error_t hs_b200_streams_read_state(const hs_b200_stream_set_t *s, unsigned char *look_behind,
+                                      unsigned long long *offsets) {
+    if (!s) {
+        return HS_INVALID;
+    }
+    DeviceGuard guard(s->device);
+    CUDA_TRY(cudaDeviceSynchronize());
+    if (look_behind) {
+        CUDA_TRY(cudaMemcpy(look_behind, s->d_hist, s->nstreams * 8, cudaMemcpyDeviceToHost));
+    }
+    if (offsets) {
+        CUDA_TRY(cudaMemcpy(offsets, s->d_offset, s->nstreams * 8, cudaMemcpyDeviceToHost));
+    }
+    return HS_SUCCESS;
+}
+
 static StreamPass streamPass(hs_b200_stream_set_t *set, const u32 *srcLen) {
     StreamPass sp;
     sp.hist = set->d_hist;
@@ -3564,6 +3596,109 @@ hs_error_t hs_b200_streams_reset_async(hs_b200_stream_set_t *set, const unsigned
     }
     g_launches += n != 0;
     return HS_SUCCESS;
+}
+
+/* A stream-set pass over no rows: nothing to scan, but it takes the set's verdict like every other pass, so that
+ * behind a pass that overflowed or was bad in this epoch it commits nothing either and finish reports that epoch's
+ * outcome (HS_INSUFFICIENT_SPACE, HS_INVALID) */
+static hs_error_t emptyStreamPass(hs_scratch *s, hs_b200_stream_set *set, cudaStream_t st) {
+    CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), st));
+    CUDA_TRY(cudaEventRecord(s->evStart, st));
+    CUDA_TRY(cudaEventRecord(s->evStop, st));
+    CUDA_TRY(launchStreamVerdict(s->d_counters, s->outCap, set->d_mark, set->epoch, st));
+    g_launches++;
+    CUDA_TRY(cudaMemcpyAsync(s->h_counters, s->d_counters, CTR_COUNT * sizeof(u32), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaEventRecord(s->evDone, st));
+    s->pending = true;
+    return HS_SUCCESS;
+}
+
+hs_error_t hs_b200_streams_scan_rows_async(hs_b200_stream_set_t *set, const void *d_chars, size_t chars_bytes,
+                                           const unsigned long long *d_offsets, const unsigned int *d_stream_ids,
+                                           size_t nrows, hs_scratch_t *scratch, void *cuda_stream) {
+    if (!set || !d_offsets || (uintptr_t)d_offsets % 8 || (!d_chars && chars_bytes) || (!d_stream_ids && nrows) ||
+        (uintptr_t)d_stream_ids % 4 || nrows > 0xfffffff0u || !validScratch(scratch) || scratch->device != set->device) {
+        return HS_INVALID;
+    }
+    DevImage *im = heldImage(scratch, set->db);
+    if (!im) {
+        return HS_INVALID;
+    }
+    if (scratch->nPeers) {
+        return HS_ARCH_ERROR; /* the exchanged records would be the scan's, not the rewritten ones */
+    }
+    if (markInUse(scratch)) {
+        return HS_SCRATCH_IN_USE;
+    }
+    DeviceGuard guard(set->device);
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
+    /* a group's block takes its rows' bytes, at most 7 look-behind bytes and at most 15 of pad (16 for an empty
+     * group), and the table's unused entries are empty blocks 16 bytes apart behind the last one */
+    const u64 bound = (u64)chars_bytes + 32 * (u64)nrows;
+    const size_t n = nrows, tiles = (n + ROWS_TILE - 1) / ROWS_TILE;
+    size_t at = 0;
+    auto carve = [&](size_t bytes) {
+        const size_t o = at;
+        at = HSB_ROUNDUP(at + bytes, 256);
+        return o;
+    };
+    const size_t oHead = carve(sizeof(StreamRowsHead)), oDigits = carve(256 * tiles * 4), oTileA = carve(tiles * 8),
+                 oTileB = carve(tiles * 8), oPairs0 = carve(n * 8), oPairs1 = carve(n * 8), oPos = carve(n * 8),
+                 oGroup = carve(n * 4), oFirst = carve((n + 1) * 4), oGPos = carve((n + 1) * 8),
+                 oStream = carve(n * 4), oHl = carve(n * 4), oBase = carve(n * 8);
+    hs_error_t r = nrows ? reserveRows(scratch, bound, nrows, at) : emptyStreamPass(scratch, set, st);
+    hs_b200_corpus *c = scratch->rowsCorpus;
+    if (r == HS_SUCCESS && nrows) {
+        c->nblocks = nrows;
+        c->bytes = bound;
+        c->readableEnd = HSB_ROUNDUP(bound, 16) + 16;
+        c->payload = chars_bytes;
+        c->uniformPitch = 0;
+        c->uniformLen = 0;
+        u8 *b = scratch->d_rows;
+        StreamRowsParams p;
+        p.chars = (const u8 *)d_chars;
+        p.charsBytes = chars_bytes;
+        p.offsets = (const u64 *)d_offsets;
+        p.ids = d_stream_ids;
+        p.nrows = (u32)nrows;
+        p.nstreams = (u32)set->nstreams;
+        p.passes = (bitWidth(set->nstreams - 1) + 7) / 8;
+        p.lookBehind = set->d_hist;
+        p.streamOffset = set->d_offset;
+        p.histReq = set->histReq;
+        p.mark = set->d_mark;
+        p.epoch = set->epoch;
+        p.corpus = c->d_data;
+        p.zeroEnd = HSB_ROUNDUP(bound, 16) + 32;
+        p.blockOff = c->d_off;
+        p.blockLen = c->d_len;
+        p.out = scratch->d_out;
+        p.outCap = scratch->outCap;
+        p.counters = scratch->d_counters;
+        p.head = (StreamRowsHead *)(b + oHead);
+        p.tileDigits = (u32 *)(b + oDigits);
+        p.tileA = (u64 *)(b + oTileA);
+        p.tileB = (u64 *)(b + oTileB);
+        p.pairs[0] = (uint2 *)(b + oPairs0);
+        p.pairs[1] = (uint2 *)(b + oPairs1);
+        p.posOf = (u64 *)(b + oPos);
+        p.groupOf = (u32 *)(b + oGroup);
+        p.gFirst = (u32 *)(b + oFirst);
+        p.gPos = (u64 *)(b + oGPos);
+        p.gStream = (u32 *)(b + oStream);
+        p.gHl = (u32 *)(b + oHl);
+        p.gBase = (u64 *)(b + oBase);
+        r = enqueueScan(scratch, im, c, st, nullptr, nullptr, nullptr, nullptr, nullptr, &p);
+    }
+    /* the pass belongs to the set's epoch: finish moves the set on when it sees the pass marked, and the ordering
+     * takes the records for a stream database's */
+    scratch->streamEpoch = &set->epoch;
+    scratch->lastCorpus = c;
+    scratch->lastBlocks = nrows;
+    scratch->lastMaxLen = 0;
+    unmarkInUse(scratch);
+    return r;
 }
 
 } /* extern "C" */

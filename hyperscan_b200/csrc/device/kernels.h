@@ -202,6 +202,27 @@ struct StreamMark {
 };
 enum { STREAM_MARKED = 1, STREAM_BAD_LENGTH = 2 };
 
+/* The verdict of a stream-set pass after its scan: may it commit?  It may not when the set is marked in this epoch,
+ * the pass is bad, the scan failed or the record ring or candidate list overflowed; then `first` (one thread of the
+ * launch) marks the set, remembers the largest record count since the mark and raises the pass's count above the
+ * ring.  Every thread reaches the same verdict, because only a "no" is written (a mark of an earlier epoch is one
+ * the host has seen: it counts as none). */
+__device__ __forceinline__ bool streamPassCommits(u32 *counters, u32 outCap, StreamMark *mark, u32 epoch, bool first) {
+    const u32 count = counters[CTR_MATCHES];
+    const bool marked = mark->marked == epoch + 1, bad = mark->bad == epoch + 1;
+    if (marked || bad || counters[CTR_ERROR] || count > outCap) {
+        if (first) {
+            const u32 need = max(max(marked ? mark->need : 0u, count), outCap + 1);
+            mark->need = need;
+            mark->marked = epoch + 1;
+            counters[CTR_MATCHES] = need;
+            counters[CTR_STREAM] = STREAM_MARKED | (bad ? (u32)STREAM_BAD_LENGTH : 0u);
+        }
+        return false;
+    }
+    return true;
+}
+
 /* stream-set helpers, each given the set's epoch at enqueue time: write every stream's look-behind in front of
  * its write (and, given srcLens, take the caller's device lengths into lens, a length above pitch - 16
  * becoming 0 and marking the pass bad) / roll history and offsets forward after a scan, only if the pass may
@@ -387,6 +408,61 @@ struct RowSegParams {
     u32 *segFirst;
 };
 cudaError_t launchRowSegments(const RowSegParams &p, int smCount, cudaStream_t stream, unsigned *launches);
+
+/* ---- stream-set passes over rows (stream_rows_kernels.h): rows tagged with their stream -> one block per stream ---- */
+
+/* zeroed by the host before every pass */
+struct StreamRowsHead {
+    u32 bad;          /* the batch is bad: a stream id at or above nstreams, a bad row, a stream's block past 32 bits */
+    u32 groups;       /* D: the distinct streams of the batch */
+    u32 kept;         /* records the rewrite kept */
+    u32 applied;      /* the rewrite ran (the pass may commit) */
+    u64 packedEnd;    /* end of the last group's block */
+    u32 digits[4 * 256]; /* per radix pass of the stream ids: the count of every digit value */
+};
+
+struct StreamRowsParams {
+    /* row r = chars[offsets[r], offsets[r + 1]), written to stream ids[r] */
+    const u8 *chars;
+    u64 charsBytes;
+    const u64 *offsets;
+    const u32 *ids;
+    u32 nrows;
+    u32 nstreams;
+    u32 passes;         /* 8-bit radix passes the stream ids need */
+    /* the set: 8 bytes of look-behind per stream (7 bytes + their count), 64-bit offsets, the mark */
+    u8 *lookBehind;
+    u64 *streamOffset;
+    u32 histReq;
+    StreamMark *mark;
+    u32 epoch;
+    /* the packed corpus (bytes [0, zeroEnd) are written) and its block table, one block per group */
+    u8 *corpus;
+    u64 zeroEnd;
+    u64 *blockOff;
+    u32 *blockLen;
+    /* the pass's record ring (2 * outCap records: the second half is free once the confirm kernel has run) */
+    DevMatch *out;
+    u32 outCap;
+    u32 *counters;
+    /* temporaries: tiles of ROWS_TILE entries */
+    StreamRowsHead *head;
+    u32 *tileDigits;    /* [256][tiles] */
+    u64 *tileA, *tileB; /* [tiles] */
+    uint2 *pairs[2];    /* [nrows] (stream, row): the sort's two buffers */
+    u64 *posOf;         /* per sorted position: the bytes of the sorted rows before it */
+    u32 *groupOf;       /* per sorted position: its group */
+    u32 *gFirst;        /* per group (+ 1): its first sorted position */
+    u64 *gPos;          /* per group (+ 1): posOf of its first row */
+    u32 *gStream, *gHl; /* per group: its stream, and the look-behind bytes at the front of its block */
+    u64 *gBase;         /* per group: the stream offset of its block's first byte */
+};
+/* Enqueue the grouping and the packing (after the counters are cleared, before the scan; the head zeroed) */
+cudaError_t launchStreamRowsPlan(const StreamRowsParams &p, int smCount, cudaStream_t stream, unsigned *launches);
+/* Enqueue the rewrite of the records and the advance of the streams (after the scan) */
+cudaError_t launchStreamRowsCommit(const StreamRowsParams &p, int smCount, cudaStream_t stream, unsigned *launches);
+/* The verdict of a pass over no rows (streamPassCommits on the cleared counters) */
+cudaError_t launchStreamVerdict(u32 *counters, u32 outCap, StreamMark *mark, u32 epoch, cudaStream_t stream);
 
 /* accel primitives (src/nfa/shufti.c, truffle.c, vermicelli.h): first
  * position in [0,len) whose byte is in the class, or len. */

@@ -1763,18 +1763,7 @@ __global__ void streamAdvanceKernel(const u8 *corpus, u8 *hist, u64 *offsets, co
                                     u32 nstreams, u32 pitch, u32 histReq, u32 *counters, u32 outCap,
                                     StreamMark *mark, u32 epoch) {
     const u32 b = blockIdx.x * blockDim.x + threadIdx.x;
-    /* every thread reaches the same verdict: only thread 0 writes, and only what makes it "no" (a mark of an
-     * earlier epoch is one the host has seen: it counts as none) */
-    const u32 count = counters[CTR_MATCHES];
-    const bool marked = mark->marked == epoch + 1, bad = mark->bad == epoch + 1;
-    if (marked || bad || counters[CTR_ERROR] || count > outCap) {
-        if (b == 0) {
-            const u32 need = max(max(marked ? mark->need : 0u, count), outCap + 1);
-            mark->need = need;
-            mark->marked = epoch + 1;
-            counters[CTR_MATCHES] = need;
-            counters[CTR_STREAM] = STREAM_MARKED | (bad ? (u32)STREAM_BAD_LENGTH : 0u);
-        }
+    if (!streamPassCommits(counters, outCap, mark, epoch, b == 0)) {
         return;
     }
     if (b >= nstreams) {

@@ -549,6 +549,33 @@ hs_error_t hs_b200_streams_scan_collect(hs_b200_stream_set_t *set, const char *d
 hs_error_t hs_b200_streams_scan_async(hs_b200_stream_set_t *set, void *d_writes, size_t pitch,
                                       const unsigned int *d_lengths, unsigned int uniform_length,
                                       hs_scratch_t *scratch, void *cuda_stream);
+/* A pass over a batch of writes as traffic arrives: rows in device memory, each tagged with its stream, in
+ * arrival order.  Row r is d_chars[d_offsets[r], d_offsets[r + 1]) (the layout of hs_b200_scan_rows_async: nrows + 1
+ * offsets in device memory, 8-byte aligned, d_offsets[0] may be above 0, no row needs an alignment) and is written
+ * to stream d_stream_ids[r] (nrows ids in device memory).  The pass is equivalent to hs_scan_stream of row r on
+ * stream d_stream_ids[r] for r = 0 .. nrows - 1 in order: a stream may receive any number of rows anywhere in the
+ * batch, a match may span its rows, an empty row is a write of nothing, and the streams the batch does not name
+ * are neither read nor written.  Enqueued on cuda_stream (NULL = the scratch's stream) with no host wait; the
+ * device groups the rows by stream and packs them into staging memory of the scratch (grown in the call).  Nothing
+ * outside [d_chars, d_chars + chars_bytes), the offsets and the ids is read, and none of them is written; they stay
+ * valid until the pass completes.  d_chars may be NULL when chars_bytes is 0, d_stream_ids when nrows is 0.
+ * The records go into the scratch's ring with block = the row that holds the match's last byte and to = the stream
+ * offset of the match's end; ordered by (block, to, id) they are the callbacks of the loop above, in order.
+ * hs_b200_scan_corpus_finish, hs_b200_fetch_matches, hs_b200_export_records_async and
+ * hs_b200_order_matches_async serve the pass, with nrows blocks.  Commit, mark and epoch are those of
+ * hs_b200_streams_scan_async, and passes of both kinds and hs_b200_streams_reset_async mix freely on one set, on
+ * one CUDA stream.  A bad batch fails the pass as a bad length does there (no records, the streams stay, the
+ * ordering reports HS_B200_ORDER_RING_OVERFLOW, finish returns HS_INVALID): offsets that decrease or end past
+ * chars_bytes, a stream id at or above the set's stream count, or one stream receiving 4 GiB minus its
+ * look-behind or more in the batch.  A batch of no rows scans nothing and delivers no records, but takes the set's
+ * verdict like any pass: behind a pass that overflowed or was bad in the same epoch, its ordering reports
+ * HS_B200_ORDER_RING_OVERFLOW and finish returns that outcome (HS_INSUFFICIENT_SPACE, HS_INVALID).
+ * HS_INVALID at once: NULL arguments, misaligned offsets or ids, nrows above 0xfffffff0, a scratch on another
+ * device than the set or holding no image of the set's database; HS_ARCH_ERROR for a scratch with a peer
+ * exchange registered. */
+hs_error_t hs_b200_streams_scan_rows_async(hs_b200_stream_set_t *set, const void *d_chars, size_t chars_bytes,
+                                           const unsigned long long *d_offsets, const unsigned int *d_stream_ids,
+                                           size_t nrows, hs_scratch_t *scratch, void *cuda_stream);
 /* End the flows of the `count` streams listed in d_streams (device memory; NULL = every stream): their
  * look-behind becomes empty and their offset 0, in stream order on cuda_stream.  Indices at or above
  * nstreams are ignored.  Nothing is delivered: a pure-literal stream database has no end-of-data reports.
@@ -559,6 +586,11 @@ hs_error_t hs_b200_streams_scan_async(hs_b200_stream_set_t *set, void *d_writes,
 hs_error_t hs_b200_streams_reset_async(hs_b200_stream_set_t *set, const unsigned int *d_streams, size_t count,
                                        void *cuda_stream);
 size_t hs_b200_streams_state_bytes(const hs_b200_stream_set_t *set);
+/* The set's state, copied to host memory once every pass and reset enqueued on it has run (the call synchronises
+ * the device): 8 bytes per stream into look_behind (the look-behind bytes, oldest first, and their count in byte 7)
+ * and the 64-bit stream offsets into offsets, nstreams of each; either may be NULL.  For tests and diagnostics. */
+hs_error_t hs_b200_streams_read_state(const hs_b200_stream_set_t *set, unsigned char *look_behind,
+                                      unsigned long long *offsets);
 hs_error_t hs_b200_streams_close(hs_b200_stream_set_t *set);
 
 /* Introspection used by tests and bench.py. */
