@@ -11,7 +11,10 @@ CSRC = os.path.join(ROOT, "hyperscan_b200", "csrc")
 # HSB_EMU_SANITIZE=1: AddressSanitizer build (run pytest with LD_PRELOAD=libasan.so and
 # ASAN_OPTIONS=detect_leaks=0:detect_stack_use_after_return=0) -- a memcheck for host and kernel logic
 SANITIZE = os.environ.get("HSB_EMU_SANITIZE") == "1"
-OUT_DIR = os.path.join(HERE, "_build_asan" if SANITIZE else "_build")
+# HSB_EMU_COVERAGE=1: gcov build (--coverage -O0); each test run adds its counts to the .gcda files beside the
+# objects, which kernel_coverage.py reads
+COVERAGE = os.environ.get("HSB_EMU_COVERAGE") == "1"
+OUT_DIR = os.path.join(HERE, "_build_asan" if SANITIZE else "_build_cov" if COVERAGE else "_build")
 OUT = os.path.join(OUT_DIR, "libhs_b200_simt_emu.so")
 HOST = ["host/api_host.cpp", "host/rose_build.cpp", "host/hwlm_build.cpp", "host/db_walk.cpp",
         "host/pair_table.cpp", "host/dfa_build.cpp", "host/limex_build.cpp", "host/regex_nfa.cpp"]
@@ -34,6 +37,8 @@ def build(verbose=False):
     common = ["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-fno-strict-aliasing", "-Wno-unused-value"]
     if SANITIZE:
         common += ["-fsanitize=address", "-fno-omit-frame-pointer"]
+    if COVERAGE:
+        common = [f for f in common if f != "-O1"] + ["--coverage", "-O0"]
     jobs = [(os.path.join(CSRC, s), common) for s in HOST]
     jobs += [(os.path.join(CSRC, s), common + ["-x", "c++", "-DHSB_HOST_EMU", "-I", HERE]) for s in DEVICE]
     jobs += [(os.path.join(HERE, "simt_emu.cpp"), common)]
@@ -48,7 +53,8 @@ def build(verbose=False):
     for full, pr in procs:
         if pr.wait() != 0:
             raise RuntimeError("emulator build failed: " + " ".join(full))
-    subprocess.run(["g++", "-shared"] + (["-fsanitize=address"] if SANITIZE else []) + ["-o", OUT] + objs, check=True)
+    link = (["-fsanitize=address"] if SANITIZE else []) + (["--coverage"] if COVERAGE else [])
+    subprocess.run(["g++", "-shared"] + link + ["-o", OUT] + objs, check=True)
     return OUT
 
 
