@@ -116,6 +116,9 @@ def lib():
         L.hs_b200_streams_scan_async.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint, vp, vp]
         L.hs_b200_streams_reset_async.argtypes = [vp, vp, C.c_size_t, vp]
         L.hs_b200_streams_scan_rows_async.argtypes = [vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp, vp]
+        L.hs_b200_streams_scan_mask_async.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint, vp, vp, C.c_size_t, vp, vp]
+        L.hs_b200_streams_scan_rows_mask_async.argtypes = [vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp, vp, C.c_size_t,
+                                                           vp, vp]
         L.hs_b200_streams_read_state.argtypes = [vp, vp, vp]
         L.hs_b200_streams_state_bytes.argtypes = [vp]
         L.hs_b200_streams_state_bytes.restype = C.c_size_t
@@ -734,6 +737,15 @@ class StreamSet:
         entries; numpy arrays under the SIMT emulator) -- in row order.  Enqueued on `stream` (a cudaStream_t
         address; None = the scratch's stream); returns at once.  The records (block = row, to = stream offset) are
         served by scan_corpus_finish, fetch_matches and order_matches_async(self.db, ...)."""
+        nrows, nbytes = self._batch(chars, offsets, stream_ids)
+        _check(lib().hs_b200_streams_scan_rows_async(self.ptr, _dev_ptr(chars) if nbytes else None, nbytes,
+                                                     _dev_ptr(offsets), _dev_ptr(stream_ids) if nrows else None,
+                                                     nrows, scratch.ptr, C.c_void_p(stream or 0)),
+               "streams_scan_rows_async")
+
+    @staticmethod
+    def _batch(chars, offsets, stream_ids):
+        """(nrows, chars' bytes) of a batch, its dtypes and sizes checked"""
         for x, dts in ((chars, ("uint8",)), (offsets, ("int64", "uint64")), (stream_ids, ("int32", "uint32"))):
             name = str(x.dtype).replace("torch.", "")
             if name not in dts:
@@ -742,11 +754,32 @@ class StreamSet:
         nids = stream_ids.numel() if hasattr(stream_ids, "numel") else stream_ids.size
         if nrows < 0 or nids != nrows:
             raise ValueError("offsets needs nrows + 1 entries and stream_ids nrows")
-        nbytes = chars.numel() if hasattr(chars, "numel") else chars.size
-        _check(lib().hs_b200_streams_scan_rows_async(self.ptr, _dev_ptr(chars) if nbytes else None, nbytes,
-                                                     _dev_ptr(offsets), _dev_ptr(stream_ids) if nrows else None,
-                                                     nrows, scratch.ptr, C.c_void_p(stream or 0)),
-               "streams_scan_rows_async")
+        return nrows, chars.numel() if hasattr(chars, "numel") else chars.size
+
+    def scan_mask_async(self, writes, pitch, lengths, scratch, mask, words_per_block=None, status=None, stream=None):
+        """hs_b200_streams_scan_mask_async: the pass of scan_async, writing the match mask `mask` (nstreams x
+        words_per_block 32-bit words, row = stream; as scan_corpus_mask_async) and, given `status` (one 32-bit
+        element), 0 when the pass committed, 1 when it did not.  No records; scan_corpus_finish serves the pass."""
+        if isinstance(lengths, (int, np.integer)):
+            d_len, uni = None, int(lengths)
+        else:
+            d_len, uni = _dev_ptr(lengths), 0
+        wpb = _words_per_block(mask, self.n, words_per_block)
+        _check(lib().hs_b200_streams_scan_mask_async(self.ptr, _dev_ptr(writes), int(pitch), d_len, uni, scratch.ptr,
+                                                     _dev_ptr(mask), wpb, _dev_ptr(status), C.c_void_p(stream or 0)),
+               "streams_scan_mask_async")
+
+    def scan_rows_mask_async(self, chars, offsets, stream_ids, scratch, mask, words_per_block=None, status=None,
+                             stream=None):
+        """hs_b200_streams_scan_rows_mask_async: the pass of scan_rows_async, writing the match mask `mask` (nrows x
+        words_per_block 32-bit words, row = the batch row that holds the match's last byte) and its status, as
+        scan_mask_async."""
+        nrows, nbytes = self._batch(chars, offsets, stream_ids)
+        wpb = _words_per_block(mask, nrows, words_per_block)
+        _check(lib().hs_b200_streams_scan_rows_mask_async(self.ptr, _dev_ptr(chars) if nbytes else None, nbytes,
+                                                          _dev_ptr(offsets), _dev_ptr(stream_ids) if nrows else None,
+                                                          nrows, scratch.ptr, _dev_ptr(mask), wpb, _dev_ptr(status),
+                                                          C.c_void_p(stream or 0)), "streams_scan_rows_mask_async")
 
     def state(self):
         """hs_b200_streams_read_state: (look-behind, nstreams x 8 uint8; offsets, nstreams uint64), once every pass

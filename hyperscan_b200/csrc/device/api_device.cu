@@ -1431,9 +1431,11 @@ struct StreamPass {
  * and the streams advance -- or the set is marked -- before the counters are read back.
  * For a row scan (rows), the row plan fills c's block table and packs the rows into it first.
  * For a stream-set pass over rows (srows), the rows are grouped by stream and packed into c first, and the records
- * are rewritten to rows and stream offsets and the streams advance -- or the set is marked -- after the scan.
+ * are rewritten to rows and stream offsets and the streams advance -- or the set is marked -- after the scan; a mask
+ * pass over rows has no records to rewrite (its confirm kernel maps every match to its row) and only advances.
  * For a mask pass (mask), the caller's mask is zeroed before the scan, which sets bits instead of writing records,
- * and *status (if given) receives the pass's verdict after it. */
+ * and *status (if given) receives the pass's verdict last, after a stream set's advance: a pass the set did not
+ * commit has its record count raised above the ring by then (streamPassCommits). */
 hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
                        cudaStream_t stream, const Upload *up = nullptr, const StreamPass *sp = nullptr,
                        const RowsParams *rows = nullptr, const MaskOut *mask = nullptr, u32 *status = nullptr,
@@ -1500,7 +1502,7 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
     }
     if (srows) {
         unsigned launched = 0;
-        CUDA_TRY(launchStreamRowsCommit(*srows, s->smCount, stream, &launched));
+        CUDA_TRY(launchStreamRowsCommit(*srows, mask != nullptr, s->smCount, stream, &launched));
         g_launches += launched;
     }
     s->streamEpoch = sp ? sp->epoch : nullptr;
@@ -2515,6 +2517,7 @@ static hs_error_t maskArgs(const DevImage *im, size_t nblocks, void *d_mask, siz
     m->progStart = t.progStart;
     m->reps = t.reps;
     m->nProg = t.nProg;
+    m->rows = StreamRowsMap(); /* (a stream-set pass over rows sets it) */
     return HS_SUCCESS;
 }
 
@@ -3547,12 +3550,16 @@ hs_error_t hs_b200_streams_scan_collect(hs_b200_stream_set_t *set, const char *d
     });
 }
 
-hs_error_t hs_b200_streams_scan_async(hs_b200_stream_set_t *set, void *d_writes, size_t pitch,
-                                      const unsigned int *d_lengths, unsigned int uniform_length,
-                                      hs_scratch_t *scratch, void *cuda_stream) {
+/* hs_b200_streams_scan_mask_async when mask is set, else hs_b200_streams_scan_async */
+static hs_error_t streamsPass(hs_b200_stream_set_t *set, void *d_writes, size_t pitch, const unsigned int *d_lengths,
+                              unsigned int uniform_length, hs_scratch_t *scratch, void *cuda_stream, bool mask,
+                              void *d_mask, size_t words_per_block, void *d_status) {
     if (!set || !d_writes || (uintptr_t)d_writes % 16 || pitch < 32 || pitch % 16 || pitch > 0xfffffff0u ||
         (!d_lengths && uniform_length > pitch - 16) || !validScratch(scratch) || scratch->device != set->device) {
         return HS_INVALID;
+    }
+    if (mask && scratch->nPeers) {
+        return HS_ARCH_ERROR;
     }
     if (markInUse(scratch)) {
         return HS_SCRATCH_IN_USE;
@@ -3560,6 +3567,14 @@ hs_error_t hs_b200_streams_scan_async(hs_b200_stream_set_t *set, void *d_writes,
     DeviceGuard guard(set->device);
     DevImage *im = nullptr;
     hs_error_t r = findImage(scratch, set->db, &im);
+    MaskOut m;
+    if (r == HS_SUCCESS && mask) {
+        r = maskArgs(im, set->nstreams, d_mask, words_per_block, d_status, &m);
+        if (r != HS_SUCCESS) {
+            unmarkInUse(scratch);
+            return r;
+        }
+    }
     if (r == HS_SUCCESS) {
         cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : scratch->stream;
         /* no uniform length and no device lengths: no stream has a write, which the scan reads from the
@@ -3573,7 +3588,9 @@ hs_error_t hs_b200_streams_scan_async(hs_b200_stream_set_t *set, void *d_writes,
         hs_b200_corpus *c = streamCorpus(set, (u8 *)d_writes, (u32)pitch, d_lengths ? 0 : uniform_length, bytes);
         const StreamPass sp = streamPass(set, d_lengths);
         if (r == HS_SUCCESS) {
-            r = enqueueScan(scratch, im, c, st, nullptr, &sp);
+            /* a mask pass: the confirm kernel finds the stream as the block and drops the look-behind's ends, as it
+             * does for records, and the status is written after the advance has taken the set's verdict */
+            r = enqueueScan(scratch, im, c, st, nullptr, &sp, nullptr, mask ? &m : nullptr, (u32 *)d_status);
         }
         scratch->lastCorpus = c;
         scratch->lastBlocks = set->nstreams;
@@ -3581,6 +3598,21 @@ hs_error_t hs_b200_streams_scan_async(hs_b200_stream_set_t *set, void *d_writes,
     }
     unmarkInUse(scratch);
     return r;
+}
+
+hs_error_t hs_b200_streams_scan_async(hs_b200_stream_set_t *set, void *d_writes, size_t pitch,
+                                      const unsigned int *d_lengths, unsigned int uniform_length,
+                                      hs_scratch_t *scratch, void *cuda_stream) {
+    return streamsPass(set, d_writes, pitch, d_lengths, uniform_length, scratch, cuda_stream, false, nullptr, 0,
+                       nullptr);
+}
+
+hs_error_t hs_b200_streams_scan_mask_async(hs_b200_stream_set_t *set, void *d_writes, size_t pitch,
+                                           const unsigned int *d_lengths, unsigned int uniform_length,
+                                           hs_scratch_t *scratch, void *d_mask, size_t words_per_block,
+                                           void *d_status, void *cuda_stream) {
+    return streamsPass(set, d_writes, pitch, d_lengths, uniform_length, scratch, cuda_stream, true, d_mask,
+                       words_per_block, d_status);
 }
 
 hs_error_t hs_b200_streams_reset_async(hs_b200_stream_set_t *set, const unsigned int *d_streams, size_t count,
@@ -3601,21 +3633,27 @@ hs_error_t hs_b200_streams_reset_async(hs_b200_stream_set_t *set, const unsigned
 /* A stream-set pass over no rows: nothing to scan, but it takes the set's verdict like every other pass, so that
  * behind a pass that overflowed or was bad in this epoch it commits nothing either and finish reports that epoch's
  * outcome (HS_INSUFFICIENT_SPACE, HS_INVALID) */
-static hs_error_t emptyStreamPass(hs_scratch *s, hs_b200_stream_set *set, cudaStream_t st) {
+static hs_error_t emptyStreamPass(hs_scratch *s, hs_b200_stream_set *set, cudaStream_t st, u32 *status) {
     CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), st));
     CUDA_TRY(cudaEventRecord(s->evStart, st));
     CUDA_TRY(cudaEventRecord(s->evStop, st));
     CUDA_TRY(launchStreamVerdict(s->d_counters, s->outCap, set->d_mark, set->epoch, st));
     g_launches++;
+    if (status) { /* a mask pass over no rows: a mask of no words, and the verdict's status */
+        CUDA_TRY(launchMaskStatus(s->d_counters, s->outCap, status, st));
+        g_launches++;
+    }
     CUDA_TRY(cudaMemcpyAsync(s->h_counters, s->d_counters, CTR_COUNT * sizeof(u32), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaEventRecord(s->evDone, st));
     s->pending = true;
     return HS_SUCCESS;
 }
 
-hs_error_t hs_b200_streams_scan_rows_async(hs_b200_stream_set_t *set, const void *d_chars, size_t chars_bytes,
-                                           const unsigned long long *d_offsets, const unsigned int *d_stream_ids,
-                                           size_t nrows, hs_scratch_t *scratch, void *cuda_stream) {
+/* hs_b200_streams_scan_rows_mask_async when mask is set, else hs_b200_streams_scan_rows_async */
+static hs_error_t streamsRowsPass(hs_b200_stream_set_t *set, const void *d_chars, size_t chars_bytes,
+                                  const unsigned long long *d_offsets, const unsigned int *d_stream_ids, size_t nrows,
+                                  hs_scratch_t *scratch, void *cuda_stream, bool mask, void *d_mask,
+                                  size_t words_per_block, void *d_status) {
     if (!set || !d_offsets || (uintptr_t)d_offsets % 8 || (!d_chars && chars_bytes) || (!d_stream_ids && nrows) ||
         (uintptr_t)d_stream_ids % 4 || nrows > 0xfffffff0u || !validScratch(scratch) || scratch->device != set->device) {
         return HS_INVALID;
@@ -3626,6 +3664,13 @@ hs_error_t hs_b200_streams_scan_rows_async(hs_b200_stream_set_t *set, const void
     }
     if (scratch->nPeers) {
         return HS_ARCH_ERROR; /* the exchanged records would be the scan's, not the rewritten ones */
+    }
+    MaskOut m;
+    if (mask) {
+        const hs_error_t r = maskArgs(im, nrows, d_mask, words_per_block, d_status, &m);
+        if (r != HS_SUCCESS) {
+            return r;
+        }
     }
     if (markInUse(scratch)) {
         return HS_SCRATCH_IN_USE;
@@ -3646,7 +3691,8 @@ hs_error_t hs_b200_streams_scan_rows_async(hs_b200_stream_set_t *set, const void
                  oTileB = carve(tiles * 8), oPairs0 = carve(n * 8), oPairs1 = carve(n * 8), oPos = carve(n * 8),
                  oGroup = carve(n * 4), oFirst = carve((n + 1) * 4), oGPos = carve((n + 1) * 8),
                  oStream = carve(n * 4), oHl = carve(n * 4), oBase = carve(n * 8);
-    hs_error_t r = nrows ? reserveRows(scratch, bound, nrows, at) : emptyStreamPass(scratch, set, st);
+    hs_error_t r = nrows ? reserveRows(scratch, bound, nrows, at)
+                         : emptyStreamPass(scratch, set, st, mask ? (u32 *)d_status : nullptr);
     hs_b200_corpus *c = scratch->rowsCorpus;
     if (r == HS_SUCCESS && nrows) {
         c->nblocks = nrows;
@@ -3689,7 +3735,10 @@ hs_error_t hs_b200_streams_scan_rows_async(hs_b200_stream_set_t *set, const void
         p.gStream = (u32 *)(b + oStream);
         p.gHl = (u32 *)(b + oHl);
         p.gBase = (u64 *)(b + oBase);
-        r = enqueueScan(scratch, im, c, st, nullptr, nullptr, nullptr, nullptr, nullptr, &p);
+        if (mask) { /* the confirm kernel maps each match to its row through the pass's tables */
+            m.rows = streamRowsMap(p);
+        }
+        r = enqueueScan(scratch, im, c, st, nullptr, nullptr, nullptr, mask ? &m : nullptr, (u32 *)d_status, &p);
     }
     /* the pass belongs to the set's epoch: finish moves the set on when it sees the pass marked, and the ordering
      * takes the records for a stream database's */
@@ -3699,6 +3748,21 @@ hs_error_t hs_b200_streams_scan_rows_async(hs_b200_stream_set_t *set, const void
     scratch->lastMaxLen = 0;
     unmarkInUse(scratch);
     return r;
+}
+
+hs_error_t hs_b200_streams_scan_rows_async(hs_b200_stream_set_t *set, const void *d_chars, size_t chars_bytes,
+                                           const unsigned long long *d_offsets, const unsigned int *d_stream_ids,
+                                           size_t nrows, hs_scratch_t *scratch, void *cuda_stream) {
+    return streamsRowsPass(set, d_chars, chars_bytes, d_offsets, d_stream_ids, nrows, scratch, cuda_stream, false,
+                           nullptr, 0, nullptr);
+}
+
+hs_error_t hs_b200_streams_scan_rows_mask_async(hs_b200_stream_set_t *set, const void *d_chars, size_t chars_bytes,
+                                                const unsigned long long *d_offsets, const unsigned int *d_stream_ids,
+                                                size_t nrows, hs_scratch_t *scratch, void *d_mask,
+                                                size_t words_per_block, void *d_status, void *cuda_stream) {
+    return streamsRowsPass(set, d_chars, chars_bytes, d_offsets, d_stream_ids, nrows, scratch, cuda_stream, true,
+                           d_mask, words_per_block, d_status);
 }
 
 } /* extern "C" */

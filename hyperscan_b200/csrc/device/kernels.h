@@ -85,10 +85,37 @@ struct OrderRep {
     u32 pad;
 };
 
+/* A stream-set pass over rows (StreamRowsParams): the tables that map a match in a group's block back to the row
+ * of the batch that holds its last byte (srRewriteKernel for records, the confirm kernel for a mask). */
+struct StreamRowsMap {
+    const uint2 *sorted; /* (stream, row) pairs in group order */
+    const u64 *posOf;    /* per sorted position: the bytes of the sorted rows before it */
+    const u64 *gPos;     /* per group: posOf of its first row */
+    const u32 *gFirst;   /* per group (+ 1): its first sorted position */
+    const u32 *gHl;      /* per group: the look-behind bytes at the front of its block */
+};
+
+/* The sorted position of the row of group g that holds sorted-row byte `at` (posOf's count): the last of the
+ * group's rows that starts at or before it, so that an empty row holds no byte. */
+__device__ __forceinline__ u32 streamRowAt(const u32 *gFirst, const u64 *posOf, u32 g, u64 at) {
+    u32 a = gFirst[g], b = gFirst[g + 1];
+    while (b - a > 1) {
+        const u32 mid = a + ((b - a) >> 1);
+        if (posOf[mid] <= at) {
+            a = mid;
+        } else {
+            b = mid;
+        }
+    }
+    return a;
+}
+
 /* A match-mask pass (hs_b200_scan_corpus_mask_async / hs_b200_scan_rows_mask_async): where a record would be
  * written, the match sets bit r % 32 of bits[block * words + r / 32] instead, r = the rank of its report id in
  * ids[0, nIds) (DeviceRules.ids).  An engine's record (a report program) first becomes the reports its program
- * raises, through the program tables the ordering uses (resolve.h). */
+ * raises, through the program tables the ordering uses (resolve.h).  In a stream-set mask pass over rows
+ * (hs_b200_streams_scan_rows_mask_async) a block is a group of the batch: rows.sorted is set, and the bit goes to
+ * the row that holds the match's last byte (resolve.h maskRowReport). */
 struct MaskOut {
     u32 *bits;       /* null: the pass writes records */
     u32 words;       /* per block */
@@ -97,6 +124,7 @@ struct MaskOut {
     const u32 *progOff, *progStart;
     const OrderRep *reps;
     u32 nProg;
+    StreamRowsMap rows; /* rows.sorted null: a block is a mask row */
 };
 
 struct ScanParams {
@@ -459,8 +487,12 @@ struct StreamRowsParams {
 };
 /* Enqueue the grouping and the packing (after the counters are cleared, before the scan; the head zeroed) */
 cudaError_t launchStreamRowsPlan(const StreamRowsParams &p, int smCount, cudaStream_t stream, unsigned *launches);
-/* Enqueue the rewrite of the records and the advance of the streams (after the scan) */
-cudaError_t launchStreamRowsCommit(const StreamRowsParams &p, int smCount, cudaStream_t stream, unsigned *launches);
+/* Enqueue the rewrite of the records and the advance of the streams (after the scan); a mask pass has no records
+ * and only advances */
+cudaError_t launchStreamRowsCommit(const StreamRowsParams &p, bool mask, int smCount, cudaStream_t stream,
+                                   unsigned *launches);
+/* The row map of a pass (StreamRowsMap), for its mask */
+StreamRowsMap streamRowsMap(const StreamRowsParams &p);
 /* The verdict of a pass over no rows (streamPassCommits on the cleared counters) */
 cudaError_t launchStreamVerdict(u32 *counters, u32 outCap, StreamMark *mark, u32 epoch, cudaStream_t stream);
 

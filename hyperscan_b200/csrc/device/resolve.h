@@ -69,6 +69,18 @@ __device__ __forceinline__ void maskReport(const MaskOut &m, u32 id, u32 block) 
     }
 }
 
+/* A stream-set mask pass over rows: a match of report id `id` that ends at `to` of group g's block.  An end inside
+ * the look-behind was delivered by an earlier pass; any other sets its bit in the row that holds its last byte, the
+ * row srRewriteKernel gives the same match's record. */
+__device__ __forceinline__ void maskRowReport(const MaskOut &m, u32 id, u32 g, u64 to) {
+    const StreamRowsMap &rm = m.rows;
+    const u32 hl = rm.gHl[g];
+    if (to <= hl) {
+        return;
+    }
+    maskReport(m, id, rm.sorted[streamRowAt(rm.gFirst, rm.posOf, g, rm.gPos[g] + (to - 1 - hl))].y);
+}
+
 } // namespace
 
 } // namespace hsb

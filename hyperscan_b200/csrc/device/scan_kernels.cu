@@ -158,7 +158,13 @@ __device__ bool findBlock(const ScanParams &p, u64 g, BlockRef *out) {
     return true;
 }
 
-__device__ __forceinline__ void emitMatch(const ScanParams &p, u32 id, u32 block, u64 to) {
+/* ROWS: the confirm kernel of a stream-set mask pass over rows (confirmRowsMaskKernel), whose blocks are the
+ * batch's groups; every other pass is ROWS = false */
+template <bool ROWS> __device__ __forceinline__ void emitMatch(const ScanParams &p, u32 id, u32 block, u64 to) {
+    if (ROWS) {
+        maskRowReport(p.mask, id, block, to);
+        return;
+    }
     if (p.mask.bits) {
         maskReport(p.mask, id, block); /* (no logical-key record: a database with combinations is refused) */
         return;
@@ -285,7 +291,7 @@ template <class T> __device__ __forceinline__ T loadInstr(const u8 *pc) {
  * REPORT_EXHAUST) and dedupe (DEDUPE*) are order-dependent and are applied
  * when the records are ordered for delivery (host, DESIGN.md section 5); here
  * they pass. */
-__device__ void runProgram(const ScanParams &p, const BlockRef &blk, u32 prog, u64 to) {
+template <bool ROWS> __device__ void runProgram(const ScanParams &p, const BlockRef &blk, u32 prog, u64 to) {
     const u8 *pc = p.bc + prog;
 #define NEXT(T) pc += HSB_ROUNDUP(sizeof(T), INSTR_ALIGN)
     for (int guard = 0; guard < 4096; guard++) {
@@ -362,25 +368,25 @@ __device__ void runProgram(const ScanParams &p, const BlockRef &blk, u32 prog, u
             break;
         case OP_REPORT: {
             const InstrReport in = loadInstr<InstrReport>(pc);
-            emitMatch(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
+            emitMatch<ROWS>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
             NEXT(InstrReport);
             break;
         }
         case OP_REPORT_EXHAUST: {
             const InstrReportExhaust in = loadInstr<InstrReportExhaust>(pc);
-            emitMatch(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
+            emitMatch<ROWS>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
             NEXT(InstrReportExhaust);
             break;
         }
         case OP_DEDUPE_AND_REPORT: {
             const InstrDedupeAndReport in = loadInstr<InstrDedupeAndReport>(pc);
-            emitMatch(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
+            emitMatch<ROWS>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
             NEXT(InstrDedupeAndReport);
             break;
         }
         case OP_FINAL_REPORT: {
             const InstrFinalReport in = loadInstr<InstrFinalReport>(pc);
-            emitMatch(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
+            emitMatch<ROWS>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
             return;
         }
         case OP_SQUASH_GROUPS: /* group squashing only prunes work */
@@ -396,7 +402,7 @@ __device__ void runProgram(const ScanParams &p, const BlockRef &blk, u32 prog, u
             /* a logical-key record (id = lkey, bit 63 of `to` set): the combinations are
              * evaluated on the host when the records are ordered (postprocessCombinations) */
             const InstrSetLogical in = loadInstr<InstrSetLogical>(pc);
-            emitMatch(p, in.lkey, blk.index, (blk.toBase + to + in.offset_adjust) | (1ull << 63));
+            emitMatch<ROWS>(p, in.lkey, blk.index, (blk.toBase + to + in.offset_adjust) | (1ull << 63));
             NEXT(InstrSetLogical);
             break;
         }
@@ -423,7 +429,7 @@ __device__ void runProgram(const ScanParams &p, const BlockRef &blk, u32 prog, u
  * confWithBit (src/fdr/fdr_confirm_runtime.h:43-102) minus the callback
  * feedback: bytes before the block start never decide (every accepted
  * literal lies inside the block, item 3 of SURVEY.md A.1). */
-__device__ void confirmFdr(const ScanParams &p, u32 bucket, u64 g, u64 confVal, u32 *nconf) {
+template <bool ROWS> __device__ void confirmFdr(const ScanParams &p, u32 bucket, u64 g, u64 confVal, u32 *nconf) {
     const u8 *confBase = p.bc + p.confOff;
     const u32 cf = ld32(confBase + 4 * bucket);
     if (!cf) {
@@ -455,7 +461,7 @@ __device__ void confirmFdr(const ScanParams &p, u32 bucket, u64 g, u64 confVal, 
                 const u64 end = (u64)(p.corpus + g - blk.base);
                 if ((tail & 0xff) <= end + 1 && end >= blk.hist) { /* ends inside the write */
                     (*nconf)++;
-                    runProgram(p, blk, ld32(li + 24), end + 1);
+                    runProgram<ROWS>(p, blk, ld32(li + 24), end + 1);
                 }
             }
         }
@@ -468,7 +474,7 @@ __device__ void confirmFdr(const ScanParams &p, u32 bucket, u64 g, u64 confVal, 
 
 /* Noodle second stage (src/hwlm/noodle_engine.c:114-141): the msk_len bytes
  * ending at g, first byte in the low lane, under msk must equal cmp. */
-__device__ void confirmNoodle(const ScanParams &p, u64 g, u64 confVal, u32 *nconf) {
+template <bool ROWS> __device__ void confirmNoodle(const ScanParams &p, u64 g, u64 confVal, u32 *nconf) {
     const u8 *n = p.bc + p.engineOff; /* struct noodTable */
     const u32 mskLen = ld8(n + 24);
     const u64 msk = ld64(n + 8), cmp = ld64(n + 16);
@@ -485,7 +491,7 @@ __device__ void confirmNoodle(const ScanParams &p, u64 g, u64 confVal, u32 *ncon
         return;
     }
     (*nconf)++;
-    runProgram(p, blk, ld32(n + 0), end + 1);
+    runProgram<ROWS>(p, blk, ld32(n + 0), end + 1);
 }
 
 /* ---- first stage ----------------------------------------------------------- */
@@ -1612,7 +1618,7 @@ cudaError_t launchGram(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t s
 
 /* Second kernel of every scan: one thread per candidate of the list the scan
  * kernel filled -- hash confirm, block lookup, literal program, record. */
-__global__ void __launch_bounds__(256) confirmKernel(const HSB_GRID_CONSTANT ScanParams p) {
+template <bool ROWS> __device__ __forceinline__ void confirmList(const ScanParams &p) {
     const u32 total = p.counters[CTR_CANDQ];
     const u32 n = total < p.outCap ? total : p.outCap;
     if (total > p.outCap && blockIdx.x == 0 && threadIdx.x == 0) {
@@ -1632,19 +1638,27 @@ __global__ void __launch_bounds__(256) confirmKernel(const HSB_GRID_CONSTANT Sca
         const u64 confVal = confValAt(p, g);
         if (p.confirmKind == CK_NOODLE) {
             if (buckets & 1) {
-                confirmNoodle(p, g, confVal, &nconf);
+                confirmNoodle<ROWS>(p, g, confVal, &nconf);
             }
         } else {
             while (buckets) {
                 const u32 bucket = __ffs(buckets) - 1;
                 buckets &= buckets - 1;
-                confirmFdr(p, bucket, g, confVal, &nconf);
+                confirmFdr<ROWS>(p, bucket, g, confVal, &nconf);
             }
         }
     }
     if (nconf) {
         atomicAdd(p.counters + CTR_CONFIRMED, nconf);
     }
+}
+
+__global__ void __launch_bounds__(256) confirmKernel(const HSB_GRID_CONSTANT ScanParams p) { confirmList<false>(p); }
+
+/* the confirm kernel of a stream-set mask pass over rows (p.mask.rows.sorted set): each match sets the bit of the
+ * batch row that holds its last byte, not of its block (a group) */
+__global__ void __launch_bounds__(256) confirmRowsMaskKernel(const HSB_GRID_CONSTANT ScanParams p) {
+    confirmList<true>(p);
 }
 
 cudaError_t launchWide(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream) {
@@ -1833,6 +1847,10 @@ cudaError_t launchStreamReset(u8 *hist, u64 *offsets, const u32 *idx, u32 count,
 }
 
 cudaError_t launchConfirm(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream) {
+    if (p.mask.rows.sorted) {
+        HSB_LAUNCH(confirmRowsMaskKernel, cfg.grid * 2, 256, 0, stream, p);
+        return cudaGetLastError();
+    }
     HSB_LAUNCH(confirmKernel, cfg.grid * 2, 256, 0, stream, p);
     return cudaGetLastError();
 }

@@ -24,8 +24,10 @@
  *             with the neighbouring rows).  Nothing outside [chars, chars + charsBytes) is read.
  *   rewrite   (after the scan, when the pass may commit) a record that ends in the look-behind goes (an earlier pass
  *             delivered it); the others get block = the row holding their last byte (a binary search over the
- *             group's rows: an empty row holds no byte) and to = their stream offset.  The kept records are
- *             gathered in the ring's second half, then copied back with their count.
+ *             group's rows, streamRowAt: an empty row holds no byte) and to = their stream offset.  The kept
+ *             records are gathered in the ring's second half, then copied back with their count.  A mask pass
+ *             (hs_b200_streams_scan_rows_mask_async) writes no records and skips this step: its confirm kernel
+ *             drops the same ends and maps each match to its row with the same search as it sets the bit.
  *   advance   streamPassCommits' verdict; per group, the last histReq bytes of its block become the stream's
  *             look-behind and its rows' bytes are added to the stream's offset.
  *
@@ -435,18 +437,7 @@ __global__ void __launch_bounds__(ROWS_THREADS) srRewriteKernel(const StreamRows
         if (m.to <= hl) {
             continue;
         }
-        /* the last row of the group that starts at or before the match's last byte */
-        const u64 at = p.gPos[g] + (m.to - 1 - hl);
-        u32 a = p.gFirst[g], b = p.gFirst[g + 1];
-        while (b - a > 1) {
-            const u32 mid = a + ((b - a) >> 1);
-            if (p.posOf[mid] <= at) {
-                a = mid;
-            } else {
-                b = mid;
-            }
-        }
-        m.block = sorted[a].y;
+        m.block = sorted[streamRowAt(p.gFirst, p.posOf, g, p.gPos[g] + (m.to - 1 - hl))].y;
         m.to += p.gBase[g];
         p.out[p.outCap + atomicAdd(&p.head->kept, 1u)] = m;
     }
@@ -534,18 +525,32 @@ cudaError_t launchStreamRowsPlan(const StreamRowsParams &p, int smCount, cudaStr
     return cudaGetLastError();
 }
 
-cudaError_t launchStreamRowsCommit(const StreamRowsParams &p, int smCount, cudaStream_t stream, unsigned *launches) {
+cudaError_t launchStreamRowsCommit(const StreamRowsParams &p, bool mask, int smCount, cudaStream_t stream,
+                                   unsigned *launches) {
     *launches = 0;
     if (!p.nrows) {
         return cudaSuccess;
     }
-    const u64 grid = std::min<u64>(((u64)p.outCap + ROWS_THREADS - 1) / ROWS_THREADS, (u64)smCount * 8);
-    HSB_LAUNCH(srRewriteKernel, (unsigned)grid, ROWS_THREADS, 0, stream, p);
-    HSB_LAUNCH(srCompactKernel, (unsigned)grid, ROWS_THREADS, 0, stream, p);
+    if (!mask) { /* a mask pass set its rows' bits in the scan: it has no records to rewrite */
+        const u64 grid = std::min<u64>(((u64)p.outCap + ROWS_THREADS - 1) / ROWS_THREADS, (u64)smCount * 8);
+        HSB_LAUNCH(srRewriteKernel, (unsigned)grid, ROWS_THREADS, 0, stream, p);
+        HSB_LAUNCH(srCompactKernel, (unsigned)grid, ROWS_THREADS, 0, stream, p);
+        *launches = 2;
+    }
     HSB_LAUNCH(srAdvanceKernel, (unsigned)(((u64)p.nrows + ROWS_THREADS - 1) / ROWS_THREADS), ROWS_THREADS, 0, stream,
                p);
-    *launches = 3;
+    *launches += 1;
     return cudaGetLastError();
+}
+
+StreamRowsMap streamRowsMap(const StreamRowsParams &p) {
+    StreamRowsMap m;
+    m.sorted = p.pairs[p.passes & 1]; /* srSorted */
+    m.posOf = p.posOf;
+    m.gPos = p.gPos;
+    m.gFirst = p.gFirst;
+    m.gHl = p.gHl;
+    return m;
 }
 
 } // namespace hsb

@@ -576,6 +576,33 @@ hs_error_t hs_b200_streams_scan_async(hs_b200_stream_set_t *set, void *d_writes,
 hs_error_t hs_b200_streams_scan_rows_async(hs_b200_stream_set_t *set, const void *d_chars, size_t chars_bytes,
                                            const unsigned long long *d_offsets, const unsigned int *d_stream_ids,
                                            size_t nrows, hs_scratch_t *scratch, void *cuda_stream);
+/* Stream-set passes into a match mask: the same passes as hs_b200_streams_scan_async and
+ * hs_b200_streams_scan_rows_async, but instead of match records they write d_mask, as hs_b200_scan_corpus_mask_async
+ * does (words_per_block >= ceil(count / 32) with count from hs_b200_report_ids, device memory, 4-byte aligned).  A
+ * mask row is the block the ordinary pass's records carry: nstreams rows for the pitched pass (row = stream index),
+ * nrows rows for the pass over rows (row = the batch row that holds the match's last byte).  Bit r of row b is set
+ * iff the ordinary pass, ordered by hs_b200_order_matches_async, delivers a match with block b and id ids[r]; every
+ * word is written, spare words included.  Otherwise the pass is the ordinary one: the look-behind and offsets
+ * advance as they would, commit, mark and epoch are those of hs_b200_streams_scan_async, and mask passes, record
+ * passes and hs_b200_streams_reset_async mix freely on one set and one CUDA stream.  For a flow tagger the answer
+ * of a tick is then of fixed size, needs no ordering, and a dense tick cannot overflow the record ring and mark the
+ * set.  (Masks of successive passes may be ORed by the caller to cover a flow's lifetime.)
+ * d_status (optional, a device u32) is 0 when the pass committed and 1 when it did not: a candidate-list overflow
+ * (finish: HS_INSUFFICIENT_SPACE, list grown), a bad length or batch (finish: HS_INVALID), or a set marked earlier
+ * in the epoch (finish returns that epoch's outcome).  hs_b200_scan_corpus_finish returns what it returns for the
+ * ordinary pass, and the caller enqueues the passes and resets again from the first one that did not commit.  No
+ * records are written: finish reports 0 records (or the overflow), and fetch, export and both orderings serve 0.
+ * Refused at once: what the ordinary calls refuse, with the same codes, and HS_INVALID for words_per_block too
+ * small, a NULL d_mask when the pass has mask rows and a misaligned d_mask or d_status; HS_ARCH_ERROR for a
+ * scratch with a peer exchange registered. */
+hs_error_t hs_b200_streams_scan_mask_async(hs_b200_stream_set_t *set, void *d_writes, size_t pitch,
+                                           const unsigned int *d_lengths, unsigned int uniform_length,
+                                           hs_scratch_t *scratch, void *d_mask, size_t words_per_block,
+                                           void *d_status, void *cuda_stream);
+hs_error_t hs_b200_streams_scan_rows_mask_async(hs_b200_stream_set_t *set, const void *d_chars, size_t chars_bytes,
+                                                const unsigned long long *d_offsets, const unsigned int *d_stream_ids,
+                                                size_t nrows, hs_scratch_t *scratch, void *d_mask,
+                                                size_t words_per_block, void *d_status, void *cuda_stream);
 /* End the flows of the `count` streams listed in d_streams (device memory; NULL = every stream): their
  * look-behind becomes empty and their offset 0, in stream order on cuda_stream.  Indices at or above
  * nstreams are ignored.  Nothing is delivered: a pure-literal stream database has no end-of-data reports.
