@@ -157,6 +157,8 @@ def lib():
         L.hs_b200_report_ids.argtypes = [vp, vp, C.c_size_t, C.POINTER(C.c_size_t)]
         L.hs_b200_scan_corpus_mask_async.argtypes = [vp, vp, vp, vp, C.c_size_t, vp, vp]
         L.hs_b200_scan_rows_mask_async.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, vp, C.c_size_t, vp, vp]
+        L.hs_b200_scan_corpus_first_async.argtypes = [vp, vp, vp, vp, vp, vp]
+        L.hs_b200_scan_rows_first_async.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, vp, vp, vp]
         L.hs_b200_db_info.argtypes = [vp, C.POINTER(DbInfo)]
         L.hs_b200_set_build_option.argtypes = [cp, C.c_int]
         L.hs_b200_set_runtime_option.argtypes = [cp, C.c_int]
@@ -571,6 +573,26 @@ def scan_rows_mask_async(db, chars, offsets, scratch, mask, words_per_block=None
     _check(lib().hs_b200_scan_rows_mask_async(db.ptr, _dev_ptr(chars) if nbytes else None, nbytes,
                                               _dev_ptr(offsets), nrows, scratch.ptr, _dev_ptr(mask), wpb,
                                               _dev_ptr(status), C.c_void_p(stream or 0)), "scan_rows_mask_async")
+
+
+def scan_corpus_first_async(db, corpus, scratch, first, status=None, stream=None):
+    """hs_b200_scan_corpus_first_async: one pass over the corpus that writes the first-match table `first` (a CUDA
+    tensor of nblocks 64-bit entries, e.g. torch.empty(nblocks, dtype=torch.int64); numpy under the SIMT emulator):
+    entry b is (to << 32) | id of block b's first delivered match, all ones when it has none.  Given `status` (one
+    32-bit element), its status.  Returns at once; hs_b200_scan_corpus_finish serves the pass."""
+    _check(lib().hs_b200_scan_corpus_first_async(db.ptr, corpus.ptr, scratch.ptr, _dev_ptr(first), _dev_ptr(status),
+                                                 C.c_void_p(stream or 0)), "scan_corpus_first_async")
+
+
+def scan_rows_first_async(db, chars, offsets, scratch, first, status=None, stream=None):
+    """hs_b200_scan_rows_first_async: the same for the rows of a column in device memory (as scan_rows_async)."""
+    nrows = (offsets.numel() if hasattr(offsets, "numel") else offsets.size) - 1
+    if nrows < 0:
+        raise ValueError("offsets needs nrows + 1 entries")
+    nbytes = chars.numel() if hasattr(chars, "numel") else chars.size
+    _check(lib().hs_b200_scan_rows_first_async(db.ptr, _dev_ptr(chars) if nbytes else None, nbytes,
+                                               _dev_ptr(offsets), nrows, scratch.ptr, _dev_ptr(first),
+                                               _dev_ptr(status), C.c_void_p(stream or 0)), "scan_rows_first_async")
 
 
 def scan_corpus(db, corpus, scratch, fetch=True):

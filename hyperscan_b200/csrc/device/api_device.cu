@@ -1326,7 +1326,7 @@ cudaError_t launchEngine(DfaParams dp, const hs_b200_corpus *c, DevMatch *out, u
 }
 
 /* Launch over tiles [t0, t1) of the corpus on `stream`; t0 == 0 is the first range of a
- * scan, whose counters were all cleared just before.  mask != null: a mask pass. */
+ * scan, whose counters were all cleared just before.  mask != null: a mask or first-match pass. */
 hs_error_t launchRange(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
                        const ScanPlan &pl, u32 t0, u32 t1, cudaStream_t stream, const MaskOut *mask) {
     if (t1 <= t0) {
@@ -1435,7 +1435,14 @@ struct StreamPass {
  * pass over rows has no records to rewrite (its confirm kernel maps every match to its row) and only advances.
  * For a mask pass (mask), the caller's mask is zeroed before the scan, which sets bits instead of writing records,
  * and *status (if given) receives the pass's verdict last, after a stream set's advance: a pass the set did not
- * commit has its record count raised above the ring by then (streamPassCommits). */
+ * commit has its record count raised above the ring by then (streamPassCommits).  A first-match pass (mask->first)
+ * is the same sequence with its table filled with ones instead. */
+/* the first kernel of a mask or first-match pass: every word of the caller's output written before the scan */
+static cudaError_t clearOutput(const MaskOut &m, size_t nblocks, int smCount, cudaStream_t stream) {
+    return m.first ? launchMaskClear(reinterpret_cast<u32 *>(m.first), 2 * (u64)nblocks, smCount, stream, true)
+                   : launchMaskClear(m.bits, (u64)nblocks * m.words, smCount, stream);
+}
+
 hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *c,
                        cudaStream_t stream, const Upload *up = nullptr, const StreamPass *sp = nullptr,
                        const RowsParams *rows = nullptr, const MaskOut *mask = nullptr, u32 *status = nullptr,
@@ -1453,7 +1460,7 @@ hs_error_t enqueueScan(hs_scratch *s, const DevImage *im, const hs_b200_corpus *
     }
     CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, CTR_COUNT * sizeof(u32), stream));
     if (mask) {
-        CUDA_TRY(launchMaskClear(mask->bits, (u64)c->nblocks * mask->words, s->smCount, stream));
+        CUDA_TRY(clearOutput(*mask, c->nblocks, s->smCount, stream));
         g_launches++;
     }
     if (sp) {
@@ -2122,11 +2129,11 @@ static hs_error_t emptyPass(hs_scratch *s, cudaStream_t st) {
 }
 
 static hs_error_t corpusPass(const hs_database_t *db, const hs_b200_corpus_t *corpus, hs_scratch_t *scratch,
-                             void *cuda_stream, bool mask, void *d_mask, size_t words_per_block, void *d_status);
+                             void *cuda_stream, int out, void *d_out, size_t words_per_block, void *d_status);
 
 hs_error_t hs_b200_scan_corpus_async(const hs_database_t *db, const hs_b200_corpus_t *corpus,
                                      hs_scratch_t *scratch, void *cuda_stream) {
-    return corpusPass(db, corpus, scratch, cuda_stream, false, nullptr, 0, nullptr);
+    return corpusPass(db, corpus, scratch, cuda_stream, OUT_RECORDS, nullptr, 0, nullptr);
 }
 
 hs_error_t hs_b200_scan_corpus_finish(hs_scratch_t *scratch, unsigned long long *nrecords,
@@ -2496,21 +2503,25 @@ static hs_error_t reserveRows(hs_scratch *s, u64 bound, size_t nrows, size_t nee
     return HS_SUCCESS;
 }
 
-/* The checks of a mask pass over nblocks blocks (after those of its ordinary form), and its MaskOut: the caller's
- * buffer (NULL only without blocks, as an empty torch tensor's) and the image's tables, uploaded with it
- * (uploadOrderTables). */
-static hs_error_t maskArgs(const DevImage *im, size_t nblocks, void *d_mask, size_t words_per_block, void *d_status,
-                           MaskOut *m) {
+/* The checks of a mask pass (out = OUT_MASK) or a first-match pass (OUT_FIRST) over nblocks blocks (after those of
+ * its ordinary form), and its MaskOut: the caller's buffer (NULL only without blocks, as an empty torch tensor's;
+ * words_per_block 32-bit words per block for a mask, one 8-byte entry for a first-match table) and the image's
+ * tables, uploaded with it (uploadOrderTables). */
+static hs_error_t maskArgs(const DevImage *im, int out, size_t nblocks, void *d_out, size_t words_per_block,
+                           void *d_status, MaskOut *m) {
     if (im->orderStatus != HS_SUCCESS) {
         return im->orderStatus; /* an engine program the tables cannot hold */
     }
     const OrderParams &t = im->orderTables;
-    if ((!d_mask && nblocks) || (uintptr_t)d_mask % 4 || (uintptr_t)d_status % 4 || words_per_block < (t.nIds + 31) / 32 ||
-        words_per_block > 0xffffffffu) {
+    const bool first = out == OUT_FIRST;
+    if ((!d_out && nblocks) || (uintptr_t)d_out % (first ? 8 : 4) || (uintptr_t)d_status % 4 ||
+        (!first && (words_per_block < (t.nIds + 31) / 32 || words_per_block > 0xffffffffu))) {
         return HS_INVALID;
     }
-    m->bits = (u32 *)d_mask;
-    m->words = (u32)words_per_block;
+    m->bits = first ? nullptr : (u32 *)d_out;
+    m->first = first ? (unsigned long long *)d_out : nullptr;
+    m->slack = (u32)-im->rules.minAdjust;
+    m->words = first ? 0 : (u32)words_per_block;
     m->nIds = t.nIds;
     m->ids = t.ids;
     m->progOff = t.progOff;
@@ -2521,19 +2532,21 @@ static hs_error_t maskArgs(const DevImage *im, size_t nblocks, void *d_mask, siz
     return HS_SUCCESS;
 }
 
-/* A mask pass over no bytes: no records, every word of the mask zero, status 0 */
+/* A mask or first-match pass over no bytes: no records, every word of the mask zero (every entry of the table all
+ * ones), status 0 */
 static hs_error_t emptyMaskPass(hs_scratch *s, cudaStream_t st, const MaskOut &m, size_t nblocks, u32 *status) {
     hs_error_t r = emptyPass(s, st);
-    if (r == HS_SUCCESS && (launchMaskClear(m.bits, (u64)nblocks * m.words, s->smCount, st) != cudaSuccess ||
+    if (r == HS_SUCCESS && (clearOutput(m, nblocks, s->smCount, st) != cudaSuccess ||
                             (status && launchMaskStatus(s->d_counters, s->outCap, status, st) != cudaSuccess))) {
         r = HS_UNKNOWN_ERROR;
     }
     return r;
 }
 
-/* hs_b200_scan_corpus_mask_async / hs_b200_scan_rows_mask_async when mask is set, else their ordinary forms */
+/* hs_b200_scan_corpus_mask_async / hs_b200_scan_rows_mask_async (out = OUT_MASK), their first-match forms
+ * (OUT_FIRST, words_per_block unused) or their ordinary forms (OUT_RECORDS) */
 static hs_error_t corpusPass(const hs_database_t *db, const hs_b200_corpus_t *corpus, hs_scratch_t *scratch,
-                             void *cuda_stream, bool mask, void *d_mask, size_t words_per_block, void *d_status) {
+                             void *cuda_stream, int out, void *d_out, size_t words_per_block, void *d_status) {
     if (!scratch || !corpus) {
         return HS_INVALID;
     }
@@ -2543,6 +2556,7 @@ static hs_error_t corpusPass(const hs_database_t *db, const hs_b200_corpus_t *co
     }
     MaskOut m;
     DevImage *im = nullptr;
+    const bool mask = out != OUT_RECORDS;
     if (mask) {
         if (dbRose(db)->ckeyCount) {
             return HS_INVALID; /* a combination's reports depend on the order within a block */
@@ -2554,7 +2568,7 @@ static hs_error_t corpusPass(const hs_database_t *db, const hs_b200_corpus_t *co
         if (scratch->nPeers) {
             return HS_ARCH_ERROR;
         }
-        r = maskArgs(im, corpus->nblocks, d_mask, words_per_block, d_status, &m);
+        r = maskArgs(im, out, corpus->nblocks, d_out, words_per_block, d_status, &m);
         if (r != HS_SUCCESS) {
             return r;
         }
@@ -2581,7 +2595,7 @@ static hs_error_t corpusPass(const hs_database_t *db, const hs_b200_corpus_t *co
 
 static hs_error_t rowsPass(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
                            const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch, void *cuda_stream,
-                           bool mask, void *d_mask, size_t words_per_block, void *d_status) {
+                           int out, void *d_out, size_t words_per_block, void *d_status) {
     if (!db || !scratch || !d_offsets || (uintptr_t)d_offsets % 8 || (!d_chars && chars_bytes) ||
         nrows > 0xfffffff0u) {
         return HS_INVALID;
@@ -2601,8 +2615,9 @@ static hs_error_t rowsPass(const hs_database_t *db, const void *d_chars, size_t 
         return HS_ARCH_ERROR;
     }
     MaskOut m;
+    const bool mask = out != OUT_RECORDS;
     if (mask) {
-        r = maskArgs(im, nrows, d_mask, words_per_block, d_status, &m);
+        r = maskArgs(im, out, nrows, d_out, words_per_block, d_status, &m);
         if (r != HS_SUCCESS) {
             return r;
         }
@@ -2655,20 +2670,32 @@ static hs_error_t rowsPass(const hs_database_t *db, const void *d_chars, size_t 
 hs_error_t hs_b200_scan_rows_async(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
                                    const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch,
                                    void *cuda_stream) {
-    return rowsPass(db, d_chars, chars_bytes, d_offsets, nrows, scratch, cuda_stream, false, nullptr, 0, nullptr);
+    return rowsPass(db, d_chars, chars_bytes, d_offsets, nrows, scratch, cuda_stream, OUT_RECORDS, nullptr, 0,
+                    nullptr);
 }
 
 hs_error_t hs_b200_scan_corpus_mask_async(const hs_database_t *db, const hs_b200_corpus_t *corpus,
                                           hs_scratch_t *scratch, void *d_mask, size_t words_per_block,
                                           void *d_status, void *cuda_stream) {
-    return corpusPass(db, corpus, scratch, cuda_stream, true, d_mask, words_per_block, d_status);
+    return corpusPass(db, corpus, scratch, cuda_stream, OUT_MASK, d_mask, words_per_block, d_status);
 }
 
 hs_error_t hs_b200_scan_rows_mask_async(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
                                         const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch,
                                         void *d_mask, size_t words_per_block, void *d_status, void *cuda_stream) {
-    return rowsPass(db, d_chars, chars_bytes, d_offsets, nrows, scratch, cuda_stream, true, d_mask, words_per_block,
+    return rowsPass(db, d_chars, chars_bytes, d_offsets, nrows, scratch, cuda_stream, OUT_MASK, d_mask, words_per_block,
                     d_status);
+}
+
+hs_error_t hs_b200_scan_corpus_first_async(const hs_database_t *db, const hs_b200_corpus_t *corpus,
+                                           hs_scratch_t *scratch, void *d_first, void *d_status, void *cuda_stream) {
+    return corpusPass(db, corpus, scratch, cuda_stream, OUT_FIRST, d_first, 0, d_status);
+}
+
+hs_error_t hs_b200_scan_rows_first_async(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
+                                         const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch,
+                                         void *d_first, void *d_status, void *cuda_stream) {
+    return rowsPass(db, d_chars, chars_bytes, d_offsets, nrows, scratch, cuda_stream, OUT_FIRST, d_first, 0, d_status);
 }
 
 /* ---- DFA engines in block mode ------------------------------------------------------
@@ -3569,7 +3596,7 @@ static hs_error_t streamsPass(hs_b200_stream_set_t *set, void *d_writes, size_t 
     hs_error_t r = findImage(scratch, set->db, &im);
     MaskOut m;
     if (r == HS_SUCCESS && mask) {
-        r = maskArgs(im, set->nstreams, d_mask, words_per_block, d_status, &m);
+        r = maskArgs(im, OUT_MASK, set->nstreams, d_mask, words_per_block, d_status, &m);
         if (r != HS_SUCCESS) {
             unmarkInUse(scratch);
             return r;
@@ -3667,7 +3694,7 @@ static hs_error_t streamsRowsPass(hs_b200_stream_set_t *set, const void *d_chars
     }
     MaskOut m;
     if (mask) {
-        const hs_error_t r = maskArgs(im, nrows, d_mask, words_per_block, d_status, &m);
+        const hs_error_t r = maskArgs(im, OUT_MASK, nrows, d_mask, words_per_block, d_status, &m);
         if (r != HS_SUCCESS) {
             return r;
         }

@@ -50,12 +50,27 @@ __device__ __forceinline__ void maskEngineRecord(const DfaParams &p, u32 prog, u
                    [&](const OrderRep &rp) { maskReport(p.mask, rp.onmatch, block); });
 }
 
-/* MASK: the walk of a mask pass (dfaStagedKernel) */
-template <bool MASK>
+/* A first-match pass: the reports of program `prog` whose bounds admit `to` lower the block's entry, at the offset
+ * the ordering gives them (to + offset_adjust); 1 when there was one */
+__device__ __forceinline__ u32 firstEngineRecord(const DfaParams &p, u32 prog, u32 block, u64 to) {
+    return programReports(p.mask.progStart, p.mask.reps, indexOf(p.mask.progOff, p.mask.nProg, prog), to,
+                          [&](const OrderRep &rp) {
+                              firstReport(p.mask, rp.onmatch, block, (u64)((long long)to + rp.adjust));
+                          }) != 0;
+}
+
+/* OUT: what the walk writes (OutKind; dfaStagedKernel).  A first-match walk keeps no slots: its `cursor` is 1 once
+ * the walk has raised a report; from then on the walk checks, byte by byte, whether anything it finds later could
+ * still come first (resolve.h firstPast: a report program's offset_adjust may put a later byte's report at the same
+ * `to` as this one, with a smaller id). */
+template <int OUT>
 __device__ __forceinline__ u32 emitDfaMatch(const DfaParams &p, u32 cursor, u32 id, u32 block, u64 to) {
-    if (MASK) {
+    if (OUT == OUT_MASK) {
         maskEngineRecord(p, id, block, to);
         return cursor;
+    }
+    if (OUT == OUT_FIRST) {
+        return cursor | firstEngineRecord(p, id, block, to);
     }
     if ((cursor & (DFA_SLOTS - 1)) == 0) {
         cursor = atomicAdd(p.counters + CTR_MATCHES, (u32)DFA_SLOTS);
@@ -71,11 +86,11 @@ __device__ __forceinline__ u32 emitDfaMatch(const DfaParams &p, u32 cursor, u32 
 }
 
 /* struct report_list {u32 count; ReportID report[]} at offset `off` of the engine at `nfa` */
-template <bool MASK>
+template <int OUT>
 __device__ u32 emitReportList(const DfaParams &p, const u8 *nfa, u32 cursor, u32 off, u32 block, u64 to) {
     const u32 n = g32(nfa + off);
     for (u32 i = 0; i < n; i++) {
-        cursor = emitDfaMatch<MASK>(p, cursor, g32(nfa + off + 4 + 4 * i), block, to);
+        cursor = emitDfaMatch<OUT>(p, cursor, g32(nfa + off + 4 + 4 * i), block, to);
     }
     return cursor;
 }
@@ -245,7 +260,7 @@ template <int W> struct StOps<WideSt<W>> {
 };
 
 /* LimEx report list: ReportID[] terminated by MO_INVALID_IDX (limexRunReports, limex_runtime.h:90-103) */
-template <bool MASK>
+template <int OUT>
 __device__ HSB_NOINLINE u32 emitLimexReports(const DfaParams &p, const u8 *nfa, u32 cursor, u32 listOff, u32 block,
                                              u64 to) {
     const u8 *lx = nfa + sizeof(NFA);
@@ -254,14 +269,14 @@ __device__ HSB_NOINLINE u32 emitLimexReports(const DfaParams &p, const u8 *nfa, 
         if (id == MO_INVALID_IDX) {
             break;
         }
-        cursor = emitDfaMatch<MASK>(p, cursor, id, block, to);
+        cursor = emitDfaMatch<OUT>(p, cursor, id, block, to);
     }
     return cursor;
 }
 
 /* accepts of the states in `found` through an NFAAccept table (PROCESS_ACCEPTS_IMPL_FN,
  * limex_common_impl.h:116-163; the squash of PROCESS_ACCEPTS_FN is dead code there) */
-template <class ST, bool MASK>
+template <class ST, int OUT>
 __device__ HSB_NOINLINE u32 emitLimexAccepts(const DfaParams &p, const u8 *nfa, u32 cursor, ST found, ST mask,
                                              u32 tableOff, u32 block, u64 to) {
     const u8 *lx = nfa + sizeof(NFA);
@@ -270,9 +285,9 @@ __device__ HSB_NOINLINE u32 emitLimexAccepts(const DfaParams &p, const u8 *nfa, 
         const u8 *a = lx + tableOff + idx * (u32)sizeof(NFAAccept);
         const u32 reports = g32(a + offsetof(NFAAccept, reports));
         if (__ldg(a + offsetof(NFAAccept, single_report))) {
-            cursor = emitDfaMatch<MASK>(p, cursor, reports, block, to);
+            cursor = emitDfaMatch<OUT>(p, cursor, reports, block, to);
         } else {
-            cursor = emitLimexReports<MASK>(p, nfa, cursor, reports, block, to);
+            cursor = emitLimexReports<OUT>(p, nfa, cursor, reports, block, to);
         }
     });
     return cursor;
@@ -436,19 +451,20 @@ struct DfaConsts {
 /* reports of a state that was just entered at offset `to` (doComplexReport, mcclellan.c:43-91;
  * fireReports, sheng_impl.h:116-155).  what = the one report of a single-report engine, else
  * the offset of the state's aux record.  Returns the lane's record cursor. */
-template <bool MASK>
+template <int OUT>
 __device__ HSB_NOINLINE u32 emitAccept(const DfaParams &p, const u8 *nfa, u32 cursor, u32 single, u32 what, u32 block,
                                        u64 to) {
     if (single) {
-        return emitDfaMatch<MASK>(p, cursor, what, block, to);
+        return emitDfaMatch<OUT>(p, cursor, what, block, to);
     }
-    return emitReportList<MASK>(p, nfa, cursor, g32(nfa + what), block, to);
+    return emitReportList<OUT>(p, nfa, cursor, g32(nfa + what), block, to);
 }
 
-/* SEG: the segment mode (p.segs, p.segMode; DESIGN.md section 10f), fused or not.  MASK: a mask pass (p.mask), whose
- * accepts set bits instead of writing records: instantiations of their own, so that the record walks stay as they
- * are */
-template <int ENGINE, int SMEM_TABLE, int CH, int ILP, bool FUSED, bool SEG = false, bool MASK = false>
+/* SEG: the segment mode (p.segs, p.segMode; DESIGN.md section 10f), fused or not.  OUT: what the accepts write
+ * (OutKind): records, the bits of a mask pass (p.mask.bits) or the entries of a first-match pass (p.mask.first), whose
+ * walks also stop once nothing they can find would come first (DESIGN.md section 10i).  The mask and first-match
+ * walks are instantiations of their own, so that the record walks stay as they are. */
+template <int ENGINE, int SMEM_TABLE, int CH, int ILP, bool FUSED, bool SEG = false, int OUT = OUT_RECORDS>
 __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(const HSB_GRID_CONSTANT DfaParams p) {
     HSB_DYNAMIC_SMEM(smem);
     typedef DfaTile<CH> Tile;
@@ -638,7 +654,9 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
         lxShiftCount = min(g32(eng + offsetof(LxNfa, shiftCount)), 8u);
         lxShiftAmounts = (u64)g32(eng + offsetof(LxNfa, shiftAmount)) | ((u64)g32(eng + offsetof(LxNfa, shiftAmount) + 4) << 32);
     }
-    u32 cursor = 0; /* this lane's next record slot (emitDfaMatch) */
+    u32 cursor = 0; /* this lane's next record slot (emitDfaMatch); a first-match walk: it has reported */
+    constexpr bool FIRST = OUT == OUT_FIRST;
+    static_assert(!FIRST || ILP == 1, "a first-match walk is one chain per lane");
     const bool segEmit = !SEG || p.segMode == SEG_EMIT; /* the segment passes before SEG_EMIT write no records */
     /* one input byte: byte j of data word w, at block offset pos.  DFAs: returns true when the
      * state entered accepts.  LimEx (LOOP_NOACCEL_FN, limex_runtime_impl.h:209-243): the states
@@ -663,7 +681,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
             Ops::forEach(Ops::band(s, tShift[8]), [&](const u32 bit) {
                 const u32 rep = reinterpret_cast<const u32 *>(smem + T::REP)[bit];
                 if (rep != MO_INVALID_IDX && pos != 0 && segEmit) {
-                    cursor = emitLimexReports<MASK>(p, nfa, cursor, rep, blk, pos);
+                    cursor = emitLimexReports<OUT>(p, nfa, cursor, rep, blk, pos);
                 }
                 local = Ops::bor(local, Ops::loadChunks(reinterpret_cast<const uint4 *>(smem + T::LOCAL), T::STATES, bit));
                 if (squashes) {
@@ -690,7 +708,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                 const ST *e = lxRows + 4 * bit;
                 const u32 rep = Ops::low32(e[3]);
                 if (rep != MO_INVALID_IDX && pos != 0 && segEmit) {
-                    cursor = emitLimexReports<MASK>(p, nfa, cursor, rep, blk, pos);
+                    cursor = emitLimexReports<OUT>(p, nfa, cursor, rep, blk, pos);
                 }
                 lim = Ops::bor(lim, e[0]);
                 local = Ops::bor(local, e[1]);
@@ -726,15 +744,18 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
     };
     /* reports of a block's last state that fire at end of data (nfaExec*_B), the block `len` bytes long */
     auto blockEnd = [&](const ST &s, const u32 blk, const u32 len) {
+        if (FIRST && firstPast(p.mask, blk, len)) {
+            return; /* its reports, at raw offset len, cannot come first */
+        }
         if constexpr (LIMEX) {
             /* STREAM_FN's closing accept check (only if the block had bytes to stream),
              * then nfaExecLimEx*_testEOD (limex_common_impl.h:192-218) */
             if (len && Ops::any(Ops::band(s, lxAccept))) {
-                cursor = emitLimexAccepts<ST, MASK>(p, nfa, cursor, Ops::band(s, lxAccept), lxAccept,
+                cursor = emitLimexAccepts<ST, OUT>(p, nfa, cursor, Ops::band(s, lxAccept), lxAccept,
                                               g32(eng + offsetof(LxNfa, acceptOffset)), blk, len);
             }
             if (Ops::any(Ops::band(s, lxAcceptEod))) {
-                cursor = emitLimexAccepts<ST, MASK>(p, nfa, cursor, Ops::band(s, lxAcceptEod), lxAcceptEod,
+                cursor = emitLimexAccepts<ST, OUT>(p, nfa, cursor, Ops::band(s, lxAcceptEod), lxAcceptEod,
                                               g32(eng + offsetof(LxNfa, acceptEodOffset)), blk, len);
             }
         } else {
@@ -742,7 +763,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                                                    : (u32)offsetof(MStateAux, accept_eod);
             const u32 eod = g32(nfa + k.auxOffset + k.auxSize * (Ops::low32(s) & k.stateMask) + eodOff);
             if (eod) {
-                cursor = emitReportList<MASK>(p, nfa, cursor, eod, blk, len);
+                cursor = emitReportList<OUT>(p, nfa, cursor, eod, blk, len);
             }
         }
     };
@@ -845,8 +866,14 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                 const u32 n = walks ? to - from : 0;
                 bool met = false, live = n != 0 && !dead(s);
                 u32 walked = 0; /* bytes of a re-walk, up to the 16-byte piece where the two walks met */
+                if (FIRST) {
+                    cursor = 0;
+                }
                 for (u32 r = 0;; r++) {
                     const u32 done = r * CH;
+                    if (FIRST && segEmit && live && firstPast(p.mask, sg.block, from + done)) {
+                        live = false; /* (the passes before SEG_EMIT need their end states) */
+                    }
                     const bool want = live && done < n;
                     if (!__any_sync(0xffffffffu, want)) {
                         break;
@@ -875,11 +902,11 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                     if (WIDE) {
                         /* one byte at a time: the wide models' steps (see above) */
 #pragma unroll 1
-                        for (u32 c = 0; c < m && live; c++) {
+                        for (u32 c = 0; c < m && live && !(FIRST && cursor && firstPast(p.mask, sg.block, at + c)); c++) {
                             const u32 x = myRow[c];
                             walked++;
                             if (step(x, 0, s, at + c, sg.block) && segEmit) {
-                                cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s), sg.block, (u64)at + c + 1);
+                                cursor = emitAccept<OUT>(p, nfa, cursor, k.single, acceptWhat(s), sg.block, (u64)at + c + 1);
                             }
                             if (cmp) {
                                 (void)step(x, 0, alt, at + c, sg.block);
@@ -921,19 +948,21 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll
                             for (u32 jj = 0; jj < 16; jj++) {
                                 if (step(w[jj >> 2], jj & 3, s, at + cc * 16 + jj, sg.block) && segEmit) {
-                                    cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s), sg.block,
+                                    cursor = emitAccept<OUT>(p, nfa, cursor, k.single, acceptWhat(s), sg.block,
                                                         (u64)at + cc * 16 + jj + 1);
                                 }
                             }
-                            live = !dead(s);
+                            live = !dead(s) && !(FIRST && cursor && firstPast(p.mask, sg.block, at + cc * 16 + 16));
                         }
                         if (live && cc * 16 < m) { /* the walk's last, partial piece */
                             const uint4 x = *reinterpret_cast<const uint4 *>(myRow + cc * 16);
                             const u32 w[4] = {x.x, x.y, x.z, x.w};
 #pragma unroll 1
-                            for (u32 jj = 0; jj < m - cc * 16; jj++) {
+                            for (u32 jj = 0;
+                                 jj < m - cc * 16 && !(FIRST && cursor && firstPast(p.mask, sg.block, at + cc * 16 + jj));
+                                 jj++) {
                                 if (step(w[jj >> 2] >> (8 * (jj & 3)), 0, s, at + cc * 16 + jj, sg.block) && segEmit) {
-                                    cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s), sg.block,
+                                    cursor = emitAccept<OUT>(p, nfa, cursor, k.single, acceptWhat(s), sg.block,
                                                         (u64)at + cc * 16 + jj + 1);
                                 }
                             }
@@ -980,7 +1009,9 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
             atomicAdd(p.segStats + SEGSTAT_WALKS, rewalks);
             atomicAdd(p.segStats + SEGSTAT_BYTES, rebytes);
         }
-        padReserved(p, cursor);
+        if (!FIRST) {
+            padReserved(p, cursor);
+        }
         return;
     }
 
@@ -1006,8 +1037,14 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
             s[u] = LIMEX ? lxStart : Ops::fromU32(k.start);
             live[u] = len[u] != 0;
         }
+        if (FIRST) {
+            cursor = 0;
+        }
         for (u32 r = 0;; r++) {
             const u32 done = r * CH;
+            if (FIRST && live[0] && firstPast(p.mask, b[0], done)) {
+                live[0] = false; /* nothing from the block's next byte on can come first */
+            }
             bool more = false;
 #pragma unroll
             for (int u = 0; u < ILP; u++) {
@@ -1071,7 +1108,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll
                         for (int u = 0; u < ILP; u++) {
                             if (step(w[u][j >> 2], j & 3, s[u], done + c * 16 + j, b[u])) {
-                                cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + c * 16 + j + 1);
+                                cursor = emitAccept<OUT>(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + c * 16 + j + 1);
                             }
                         }
                     }
@@ -1092,7 +1129,7 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                      * reason was "no instruction" -- so their bytes go through ONE copy of the step */
                     if (live[u]) {
 #pragma unroll 1
-                        for (u32 j = cc * 16; j < n[u]; j++) {
+                        for (u32 j = cc * 16; j < n[u] && !(FIRST && cursor && firstPast(p.mask, b[u], done + j)); j++) {
                             (void)step(row[j], 0, s[u], done + j, b[u]);
                         }
                         live[u] = !dead(s[u]);
@@ -1105,19 +1142,19 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
 #pragma unroll
                         for (u32 j = 0; j < 16; j++) {
                             if (step(w[j >> 2], j & 3, s[u], done + cc * 16 + j, b[u])) {
-                                cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
+                                cursor = emitAccept<OUT>(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
                             }
                         }
-                        live[u] = !dead(s[u]);
+                        live[u] = !dead(s[u]) && !(FIRST && cursor && firstPast(p.mask, b[u], done + cc * 16 + 16));
                     }
                     if (live[u] && cc * 16 < n[u]) { /* the block's last, partial piece */
                         const uint4 x = *reinterpret_cast<const uint4 *>(row + cc * 16);
                         const u32 w[4] = {x.x, x.y, x.z, x.w};
                         const u32 m = n[u] - cc * 16;
 #pragma unroll 1
-                        for (u32 j = 0; j < m; j++) {
+                        for (u32 j = 0; j < m && !(FIRST && cursor && firstPast(p.mask, b[u], done + cc * 16 + j)); j++) {
                             if (step(w[j >> 2] >> (8 * (j & 3)), 0, s[u], done + cc * 16 + j, b[u])) {
-                                cursor = emitAccept<MASK>(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
+                                cursor = emitAccept<OUT>(p, nfa, cursor, k.single, acceptWhat(s[u]), b[u], (u64)done + cc * 16 + j + 1);
                             }
                         }
                         live[u] = !dead(s[u]);
@@ -1126,19 +1163,24 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
             }
             __syncwarp();
         }
-        /* nfaExec*_B: reports of the final state that fire at end of data */
+        /* nfaExec*_B: reports of the final state that fire at end of data -- in a first-match pass, only while the
+         * block's entry is not before the end (a walk that stopped early has such an entry: its state is not the end
+         * state, and it needs none) */
 #pragma unroll
         for (int u = 0; u < ILP; u++) {
+            if (FIRST && b[u] < p.nblocks && firstPast(p.mask, b[u], len[u])) {
+                continue;
+            }
             if (LIMEX) {
                 if (b[u] < p.nblocks) {
                     /* STREAM_FN's closing accept check (only if the block had bytes to stream),
                      * then nfaExecLimEx*_testEOD (limex_common_impl.h:192-218) */
                     if (len[u] && Ops::any(Ops::band(s[u], lxAccept))) {
-                        cursor = emitLimexAccepts<ST, MASK>(p, nfa, cursor, Ops::band(s[u], lxAccept), lxAccept,
+                        cursor = emitLimexAccepts<ST, OUT>(p, nfa, cursor, Ops::band(s[u], lxAccept), lxAccept,
                                                       g32(eng + offsetof(LxNfa, acceptOffset)), b[u], len[u]);
                     }
                     if (Ops::any(Ops::band(s[u], lxAcceptEod))) {
-                        cursor = emitLimexAccepts<ST, MASK>(p, nfa, cursor, Ops::band(s[u], lxAcceptEod), lxAcceptEod,
+                        cursor = emitLimexAccepts<ST, OUT>(p, nfa, cursor, Ops::band(s[u], lxAcceptEod), lxAcceptEod,
                                                       g32(eng + offsetof(LxNfa, acceptEodOffset)), b[u], len[u]);
                     }
                 }
@@ -1147,12 +1189,14 @@ __global__ void __launch_bounds__(StagedThreads<ENGINE>::N, 1) dfaStagedKernel(c
                                                        : (u32)offsetof(MStateAux, accept_eod);
                 const u32 eod = g32(nfa + k.auxOffset + k.auxSize * (Ops::low32(s[u]) & k.stateMask) + eodOff);
                 if (eod) {
-                    cursor = emitReportList<MASK>(p, nfa, cursor, eod, b[u], len[u]);
+                    cursor = emitReportList<OUT>(p, nfa, cursor, eod, b[u], len[u]);
                 }
             }
         }
     }
-    padReserved(p, cursor);
+    if (!FIRST) {
+        padReserved(p, cursor);
+    }
 }
 
 template <int ENGINE, int SMEM_TABLE>
@@ -1163,8 +1207,9 @@ cudaError_t launchStaged(const DfaParams &p, int smCount, size_t tableBytes, cud
     const int threads = StagedThreads<ENGINE>::N;
     /* (the wide models, a fused launch and a segmented one walk one block or segment per lane) */
     const bool fused = p.engines != nullptr, seg = p.segs != nullptr;
-    const bool mask = p.mask.bits != nullptr; /* (a mask pass walks one block or segment per lane) */
-    const bool two = !fused && !seg && !mask && p.ilp == 2 && ENGINE < ENG_LIMEX128;
+    /* (a mask or first-match pass walks one block or segment per lane) */
+    const int out = p.mask.bits ? OUT_MASK : p.mask.first ? OUT_FIRST : OUT_RECORDS;
+    const bool two = !fused && !seg && out == OUT_RECORDS && p.ilp == 2 && ENGINE < ENG_LIMEX128;
     const size_t tiles = (size_t)(threads / 32) * (two ? 2 * DfaTile<64>::WARP_BYTES : DfaTile<128>::WARP_BYTES);
     const u64 units = !seg ? p.nblocks : p.segMode == SEG_SETTLE ? p.ncuts : p.nsegs;
     const u64 groups = (units + (two ? 63 : 31)) / (two ? 64 : 32);
@@ -1172,9 +1217,12 @@ cudaError_t launchStaged(const DfaParams &p, int smCount, size_t tableBytes, cud
      * engine share the GPU: a corpus too small to fill it for one engine fills it for several) */
     const int grid = (int)std::min<u64>((u64)smCount, (groups + threads / 32 - 1) / (threads / 32));
     void (*kern)(const DfaParams) =
-        mask ? (seg     ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, true, true>
-                : fused ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, true, false, true>
-                        : dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, false, true>)
+        out == OUT_MASK    ? (seg     ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, true, OUT_MASK>
+                              : fused ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, true, false, OUT_MASK>
+                                      : dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, false, OUT_MASK>)
+        : out == OUT_FIRST ? (seg     ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, true, OUT_FIRST>
+                              : fused ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, true, false, OUT_FIRST>
+                                      : dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, false, OUT_FIRST>)
              : seg     ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, false, true>
              : fused   ? dfaStagedKernel<ENGINE, SMEM_TABLE, 128, 1, true>
              : two     ? dfaStagedKernel<ENGINE, SMEM_TABLE, 64, 2, false>
@@ -1211,8 +1259,8 @@ cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t
     if (!p.nblocks) {
         return cudaSuccess;
     }
-    if (p.toTag && !p.mask.bits && (!p.segs || p.segMode == SEG_EMIT)) { /* (the passes before SEG_EMIT and a mask
-                                                                           * pass write no records) */
+    if (p.toTag && !p.mask.bits && !p.mask.first && (!p.segs || p.segMode == SEG_EMIT)) {
+        /* (the passes before SEG_EMIT, a mask pass and a first-match pass write no records) */
         HSB_LAUNCH(alignSharedRing, 1, 1, 0, stream, p);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) {

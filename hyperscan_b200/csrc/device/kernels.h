@@ -115,9 +115,13 @@ __device__ __forceinline__ u32 streamRowAt(const u32 *gFirst, const u64 *posOf, 
  * ids[0, nIds) (DeviceRules.ids).  An engine's record (a report program) first becomes the reports its program
  * raises, through the program tables the ordering uses (resolve.h).  In a stream-set mask pass over rows
  * (hs_b200_streams_scan_rows_mask_async) a block is a group of the batch: rows.sorted is set, and the bit goes to
- * the row that holds the match's last byte (resolve.h maskRowReport). */
+ * the row that holds the match's last byte (resolve.h maskRowReport).
+ * A first-match pass (hs_b200_scan_corpus_first_async / hs_b200_scan_rows_first_async) is described by the same
+ * structure with `first` set instead of `bits`: where a record would be written, the match lowers first[block] to
+ * (to << 32) | id (resolve.h firstReport), and the engine walks stop once nothing they find can be lower. */
+enum OutKind { OUT_RECORDS = 0, OUT_MASK = 1, OUT_FIRST = 2 };
 struct MaskOut {
-    u32 *bits;       /* null: the pass writes records */
+    u32 *bits;       /* null: the pass writes records, or the first-match table */
     u32 words;       /* per block */
     u32 nIds;
     const u32 *ids;
@@ -125,6 +129,9 @@ struct MaskOut {
     const OrderRep *reps;
     u32 nProg;
     StreamRowsMap rows; /* rows.sorted null: a block is a mask row */
+    unsigned long long *first; /* a first-match pass: one entry per block, ~0 = none */
+    u32 slack;       /* a first-match pass: how far before its raw end offset a report may lie (minus the smallest
+                      * offset_adjust of the database's report programs, literal and engine) */
 };
 
 struct ScanParams {
@@ -181,7 +188,8 @@ struct ScanParams {
     u32 peerCap;
     u32 blockBase;           /* added to block indices in exchanged records */
     DevMatch *peers[MAX_PEERS];
-    MaskOut mask;            /* mask.bits != null: a mask pass (the confirm kernel sets bits, writes no records) */
+    MaskOut mask;            /* mask.bits != null: a mask pass (the confirm kernel sets bits, writes no records);
+                              * mask.first != null: a first-match pass (confirmFirstKernel) */
 };
 
 struct LaunchCfg {
@@ -209,10 +217,11 @@ cudaError_t launchConfirm(const LaunchCfg &cfg, const ScanParams &p, cudaStream_
  * region in every peer's exchange buffer (runs after the scan on its stream). */
 cudaError_t launchPublishCount(const ScanParams &p, cudaStream_t stream);
 
-/* The two ends of a mask pass: zero the n words of the caller's mask (after the counters are cleared, before the
- * scan), and write its status from the pass's counters (after the scan): 0 when the mask is valid, 1 when
- * hs_b200_scan_corpus_finish will not return HS_SUCCESS (an error, a bad row table or a candidate-list overflow). */
-cudaError_t launchMaskClear(u32 *bits, u64 n, int smCount, cudaStream_t stream);
+/* The two ends of a mask or first-match pass: fill the n words of the caller's mask with 0 (a first-match table
+ * with all ones: ones = true) after the counters are cleared, before the scan, and write its status from the pass's
+ * counters (after the scan): 0 when the output is valid, 1 when hs_b200_scan_corpus_finish will not return
+ * HS_SUCCESS (an error, a bad row table or a candidate-list overflow). */
+cudaError_t launchMaskClear(u32 *bits, u64 n, int smCount, cudaStream_t stream, bool ones = false);
 cudaError_t launchMaskStatus(const u32 *counters, u32 outCap, u32 *status, cudaStream_t stream);
 
 /* A stream set's pass state in device memory.  A pass whose record ring or candidate list overflowed, or
@@ -328,7 +337,8 @@ struct DfaParams {
     unsigned long long *segStats; /* SEGSTAT_COUNT counters, accumulated */
     u32 *segOpen;    /* per engine of the launch, per block: the first segment whose start is not settled (SEG_CHECK;
                       * all ones = none), cleared by the caller */
-    MaskOut mask;    /* mask.bits != null: a mask pass (the accepts set bits, no slot is reserved or written) */
+    MaskOut mask;    /* mask.bits != null: a mask pass (the accepts set bits, no slot is reserved or written);
+                      * mask.first != null: a first-match pass (the accepts lower the block's entry) */
 };
 cudaError_t launchDfa(const DfaParams &p, int smCount, int maxSmem, cudaStream_t stream);
 

@@ -69,6 +69,34 @@ __device__ __forceinline__ void maskReport(const MaskOut &m, u32 id, u32 block) 
     }
 }
 
+/* A first-match pass: lower block `block`'s entry to (to << 32) | id, the delivery order's key within a block (every
+ * id counts, as in the ordering, known to the id table or not).  The entry is read first, so that a match that
+ * cannot win costs a load, not an atomic: entries only go down during the pass, so a stale read can only send a
+ * match to the atomic. */
+__device__ __forceinline__ void firstReport(const MaskOut &m, u32 id, u32 block, u64 to) {
+    unsigned long long *e = m.first + block;
+    const unsigned long long key = (to << 32) | id;
+    if (*(volatile unsigned long long *)e > key) {
+#ifdef HSB_HOST_EMU /* the SIMT emulator of tests/emu runs one thread at a time between its barriers */
+        *e = key;
+#else
+        atomicMin(e, key);
+#endif
+    }
+}
+
+/* the `to` of block `block`'s entry so far (~0 >> 32 = none): a match that ends later cannot win */
+__device__ __forceinline__ u32 firstTo(const MaskOut &m, u32 block) {
+    return (u32)(*(volatile unsigned long long *)(m.first + block) >> 32);
+}
+
+/* A first-match pass: no report raised at a raw end offset `pos` or later can come first in block `block` -- its
+ * offset (pos + offset_adjust >= pos - slack) lies past the entry's.  A tie on `to` is not past: a smaller id may win
+ * it. */
+__device__ __forceinline__ bool firstPast(const MaskOut &m, u32 block, u64 pos) {
+    return (u64)firstTo(m, block) + m.slack < pos;
+}
+
 /* A stream-set mask pass over rows: a match of report id `id` that ends at `to` of group g's block.  An end inside
  * the look-behind was delivered by an earlier pass; any other sets its bit in the row that holds its last byte, the
  * row srRewriteKernel gives the same match's record. */

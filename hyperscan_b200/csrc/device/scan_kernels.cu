@@ -158,11 +158,17 @@ __device__ bool findBlock(const ScanParams &p, u64 g, BlockRef *out) {
     return true;
 }
 
-/* ROWS: the confirm kernel of a stream-set mask pass over rows (confirmRowsMaskKernel), whose blocks are the
- * batch's groups; every other pass is ROWS = false */
-template <bool ROWS> __device__ __forceinline__ void emitMatch(const ScanParams &p, u32 id, u32 block, u64 to) {
-    if (ROWS) {
+/* The confirm paths: CONF_PLAIN writes records, or sets the bits of a mask pass (p.mask.bits); CONF_ROWS_MASK is the
+ * confirm kernel of a stream-set mask pass over rows (confirmRowsMaskKernel), whose blocks are the batch's groups;
+ * CONF_FIRST is the confirm kernel of a first-match pass (confirmFirstKernel) */
+enum { CONF_PLAIN = 0, CONF_ROWS_MASK = 1, CONF_FIRST = 2 };
+template <int CONF> __device__ __forceinline__ void emitMatch(const ScanParams &p, u32 id, u32 block, u64 to) {
+    if (CONF == CONF_ROWS_MASK) {
         maskRowReport(p.mask, id, block, to);
+        return;
+    }
+    if (CONF == CONF_FIRST) {
+        firstReport(p.mask, id, block, to); /* (no logical-key record: a database with combinations is refused) */
         return;
     }
     if (p.mask.bits) {
@@ -291,7 +297,7 @@ template <class T> __device__ __forceinline__ T loadInstr(const u8 *pc) {
  * REPORT_EXHAUST) and dedupe (DEDUPE*) are order-dependent and are applied
  * when the records are ordered for delivery (host, DESIGN.md section 5); here
  * they pass. */
-template <bool ROWS> __device__ void runProgram(const ScanParams &p, const BlockRef &blk, u32 prog, u64 to) {
+template <int CONF> __device__ void runProgram(const ScanParams &p, const BlockRef &blk, u32 prog, u64 to) {
     const u8 *pc = p.bc + prog;
 #define NEXT(T) pc += HSB_ROUNDUP(sizeof(T), INSTR_ALIGN)
     for (int guard = 0; guard < 4096; guard++) {
@@ -368,25 +374,25 @@ template <bool ROWS> __device__ void runProgram(const ScanParams &p, const Block
             break;
         case OP_REPORT: {
             const InstrReport in = loadInstr<InstrReport>(pc);
-            emitMatch<ROWS>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
+            emitMatch<CONF>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
             NEXT(InstrReport);
             break;
         }
         case OP_REPORT_EXHAUST: {
             const InstrReportExhaust in = loadInstr<InstrReportExhaust>(pc);
-            emitMatch<ROWS>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
+            emitMatch<CONF>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
             NEXT(InstrReportExhaust);
             break;
         }
         case OP_DEDUPE_AND_REPORT: {
             const InstrDedupeAndReport in = loadInstr<InstrDedupeAndReport>(pc);
-            emitMatch<ROWS>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
+            emitMatch<CONF>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
             NEXT(InstrDedupeAndReport);
             break;
         }
         case OP_FINAL_REPORT: {
             const InstrFinalReport in = loadInstr<InstrFinalReport>(pc);
-            emitMatch<ROWS>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
+            emitMatch<CONF>(p, in.onmatch, blk.index, blk.toBase + to + in.offset_adjust);
             return;
         }
         case OP_SQUASH_GROUPS: /* group squashing only prunes work */
@@ -402,7 +408,7 @@ template <bool ROWS> __device__ void runProgram(const ScanParams &p, const Block
             /* a logical-key record (id = lkey, bit 63 of `to` set): the combinations are
              * evaluated on the host when the records are ordered (postprocessCombinations) */
             const InstrSetLogical in = loadInstr<InstrSetLogical>(pc);
-            emitMatch<ROWS>(p, in.lkey, blk.index, (blk.toBase + to + in.offset_adjust) | (1ull << 63));
+            emitMatch<CONF>(p, in.lkey, blk.index, (blk.toBase + to + in.offset_adjust) | (1ull << 63));
             NEXT(InstrSetLogical);
             break;
         }
@@ -429,7 +435,7 @@ template <bool ROWS> __device__ void runProgram(const ScanParams &p, const Block
  * confWithBit (src/fdr/fdr_confirm_runtime.h:43-102) minus the callback
  * feedback: bytes before the block start never decide (every accepted
  * literal lies inside the block, item 3 of SURVEY.md A.1). */
-template <bool ROWS> __device__ void confirmFdr(const ScanParams &p, u32 bucket, u64 g, u64 confVal, u32 *nconf) {
+template <int CONF> __device__ void confirmFdr(const ScanParams &p, u32 bucket, u64 g, u64 confVal, u32 *nconf) {
     const u8 *confBase = p.bc + p.confOff;
     const u32 cf = ld32(confBase + 4 * bucket);
     if (!cf) {
@@ -459,9 +465,12 @@ template <bool ROWS> __device__ void confirmFdr(const ScanParams &p, u32 bucket,
             }
             if (inBlock) {
                 const u64 end = (u64)(p.corpus + g - blk.base);
+                if (CONF == CONF_FIRST && firstPast(p.mask, blk.index, end + 1)) {
+                    break; /* no report of a literal ending here can come before the block's entry */
+                }
                 if ((tail & 0xff) <= end + 1 && end >= blk.hist) { /* ends inside the write */
                     (*nconf)++;
-                    runProgram<ROWS>(p, blk, ld32(li + 24), end + 1);
+                    runProgram<CONF>(p, blk, ld32(li + 24), end + 1);
                 }
             }
         }
@@ -474,7 +483,7 @@ template <bool ROWS> __device__ void confirmFdr(const ScanParams &p, u32 bucket,
 
 /* Noodle second stage (src/hwlm/noodle_engine.c:114-141): the msk_len bytes
  * ending at g, first byte in the low lane, under msk must equal cmp. */
-template <bool ROWS> __device__ void confirmNoodle(const ScanParams &p, u64 g, u64 confVal, u32 *nconf) {
+template <int CONF> __device__ void confirmNoodle(const ScanParams &p, u64 g, u64 confVal, u32 *nconf) {
     const u8 *n = p.bc + p.engineOff; /* struct noodTable */
     const u32 mskLen = ld8(n + 24);
     const u64 msk = ld64(n + 8), cmp = ld64(n + 16);
@@ -490,8 +499,11 @@ template <bool ROWS> __device__ void confirmNoodle(const ScanParams &p, u64 g, u
     if (mskLen > end + 1 || end < blk.hist) {
         return;
     }
+    if (CONF == CONF_FIRST && firstPast(p.mask, blk.index, end + 1)) {
+        return; /* no report of the literal can come before the block's entry */
+    }
     (*nconf)++;
-    runProgram<ROWS>(p, blk, ld32(n + 0), end + 1);
+    runProgram<CONF>(p, blk, ld32(n + 0), end + 1);
 }
 
 /* ---- first stage ----------------------------------------------------------- */
@@ -1618,7 +1630,7 @@ cudaError_t launchGram(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t s
 
 /* Second kernel of every scan: one thread per candidate of the list the scan
  * kernel filled -- hash confirm, block lookup, literal program, record. */
-template <bool ROWS> __device__ __forceinline__ void confirmList(const ScanParams &p) {
+template <int CONF> __device__ __forceinline__ void confirmList(const ScanParams &p) {
     const u32 total = p.counters[CTR_CANDQ];
     const u32 n = total < p.outCap ? total : p.outCap;
     if (total > p.outCap && blockIdx.x == 0 && threadIdx.x == 0) {
@@ -1638,13 +1650,13 @@ template <bool ROWS> __device__ __forceinline__ void confirmList(const ScanParam
         const u64 confVal = confValAt(p, g);
         if (p.confirmKind == CK_NOODLE) {
             if (buckets & 1) {
-                confirmNoodle<ROWS>(p, g, confVal, &nconf);
+                confirmNoodle<CONF>(p, g, confVal, &nconf);
             }
         } else {
             while (buckets) {
                 const u32 bucket = __ffs(buckets) - 1;
                 buckets &= buckets - 1;
-                confirmFdr<ROWS>(p, bucket, g, confVal, &nconf);
+                confirmFdr<CONF>(p, bucket, g, confVal, &nconf);
             }
         }
     }
@@ -1653,12 +1665,20 @@ template <bool ROWS> __device__ __forceinline__ void confirmList(const ScanParam
     }
 }
 
-__global__ void __launch_bounds__(256) confirmKernel(const HSB_GRID_CONSTANT ScanParams p) { confirmList<false>(p); }
+__global__ void __launch_bounds__(256) confirmKernel(const HSB_GRID_CONSTANT ScanParams p) {
+    confirmList<CONF_PLAIN>(p);
+}
 
 /* the confirm kernel of a stream-set mask pass over rows (p.mask.rows.sorted set): each match sets the bit of the
  * batch row that holds its last byte, not of its block (a group) */
 __global__ void __launch_bounds__(256) confirmRowsMaskKernel(const HSB_GRID_CONSTANT ScanParams p) {
-    confirmList<true>(p);
+    confirmList<CONF_ROWS_MASK>(p);
+}
+
+/* the confirm kernel of a first-match pass (p.mask.first set): each match lowers its block's entry, and a candidate
+ * that ends after the entry is dropped before its program runs */
+__global__ void __launch_bounds__(256) confirmFirstKernel(const HSB_GRID_CONSTANT ScanParams p) {
+    confirmList<CONF_FIRST>(p);
 }
 
 cudaError_t launchWide(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream) {
@@ -1715,9 +1735,9 @@ __global__ void publishCountKernel(const ScanParams p) {
 } // namespace
 
 namespace {
-__global__ void maskClearKernel(u32 *bits, u64 n) {
+template <u32 FILL> __global__ void maskClearKernel(u32 *bits, u64 n) {
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
-        bits[i] = 0;
+        bits[i] = FILL;
     }
 }
 
@@ -1727,12 +1747,16 @@ __global__ void maskStatusKernel(const u32 *counters, u32 outCap, u32 *status) {
 }
 } // namespace
 
-cudaError_t launchMaskClear(u32 *bits, u64 n, int smCount, cudaStream_t stream) {
+cudaError_t launchMaskClear(u32 *bits, u64 n, int smCount, cudaStream_t stream, bool ones) {
     if (!n) {
         return cudaSuccess;
     }
     const u64 blocks = std::min<u64>((n + 255) / 256, (u64)std::max(1, smCount) * 8);
-    HSB_LAUNCH(maskClearKernel, (unsigned)blocks, 256, 0, stream, bits, n);
+    if (ones) {
+        HSB_LAUNCH(maskClearKernel<0xffffffffu>, (unsigned)blocks, 256, 0, stream, bits, n);
+    } else {
+        HSB_LAUNCH(maskClearKernel<0u>, (unsigned)blocks, 256, 0, stream, bits, n);
+    }
     return cudaGetLastError();
 }
 
@@ -1849,6 +1873,10 @@ cudaError_t launchStreamReset(u8 *hist, u64 *offsets, const u32 *idx, u32 count,
 cudaError_t launchConfirm(const LaunchCfg &cfg, const ScanParams &p, cudaStream_t stream) {
     if (p.mask.rows.sorted) {
         HSB_LAUNCH(confirmRowsMaskKernel, cfg.grid * 2, 256, 0, stream, p);
+        return cudaGetLastError();
+    }
+    if (p.mask.first) {
+        HSB_LAUNCH(confirmFirstKernel, cfg.grid * 2, 256, 0, stream, p);
         return cudaGetLastError();
     }
     HSB_LAUNCH(confirmKernel, cfg.grid * 2, 256, 0, stream, p);

@@ -34,6 +34,7 @@ bool collectProgramReports(ReportRules *rr, u32 prog, std::vector<ProgReport> *r
         if (!logical) {
             rr->reportIds.insert(onmatch);
         }
+        rr->minAdjust = std::min(rr->minAdjust, adjust);
         if (!reports) {
             return;
         }

@@ -96,6 +96,10 @@ struct ReportRules {
     std::unordered_map<u32, std::vector<ProgReport>> progReports;
     /* the report ids the programs walked so far can raise (logical keys excluded) */
     std::set<u32> reportIds;
+    /* the smallest offset_adjust of the programs walked so far (at most 0): after loadReportRules (every literal
+     * program) and buildDeviceRules (every engine program), no report lies more than -minAdjust bytes before the
+     * raw end offset of the match that raised it */
+    s32 minAdjust = 0;
 
     /* Without dedupe keys, exhaustion keys, combinations or engine records, the raw record count is the
      * delivered count. */

@@ -500,6 +500,25 @@ hs_error_t hs_b200_scan_rows_mask_async(const hs_database_t *db, const void *d_c
                                         const unsigned long long *d_offsets, size_t nrows,
                                         hs_scratch_t *scratch, void *d_mask, size_t words_per_block,
                                         void *d_status, void *cuda_stream);
+/* First-match passes: the passes of hs_b200_scan_corpus_async / hs_b200_scan_rows_async, but instead of match records
+ * they write one entry per block (per row) to d_first (nblocks or nrows unsigned long longs, device memory, 8-byte
+ * aligned; NULL only when there are no blocks).  Entry b is ((to << 32) | id) of the first match that
+ * hs_b200_fetch_matches would deliver for block b after the ordinary pass, in its (block, to, id) order -- the match
+ * hs_scan of block b passes to a callback that returns non-zero on its first call -- or ~0ULL when block b delivers
+ * nothing.  `to` is relative to the block (the row).  Every entry is written.  The entry is exact under dedupe,
+ * HS_FLAG_SINGLEMATCH, min_offset / max_offset and min_length: a match competes only after the checks that decide
+ * its delivery.  The engine walks stop once nothing they can still find would come first, so a block with many
+ * matches costs about as much as one whose first match is as early.  d_status (optional, a device u32) is 0 when the
+ * table is valid and 1 when hs_b200_scan_corpus_finish asks for the pass again (a candidate-list overflow:
+ * HS_INSUFFICIENT_SPACE, list grown; a bad row table: HS_INVALID).  No records are written: finish reports 0
+ * records, and fetch, export and both orderings serve 0.  Refused at once, as the mask passes refuse: HS_INVALID for
+ * NULL or misaligned arguments, a scratch that holds no image of `db` and a database with logical combinations;
+ * HS_DB_MODE_ERROR for a database not in block mode; HS_ARCH_ERROR for a scratch with a peer exchange registered. */
+hs_error_t hs_b200_scan_corpus_first_async(const hs_database_t *db, const hs_b200_corpus_t *corpus,
+                                           hs_scratch_t *scratch, void *d_first, void *d_status, void *cuda_stream);
+hs_error_t hs_b200_scan_rows_first_async(const hs_database_t *db, const void *d_chars, size_t chars_bytes,
+                                         const unsigned long long *d_offsets, size_t nrows, hs_scratch_t *scratch,
+                                         void *d_first, void *d_status, void *cuda_stream);
 
 /* Stream sets: `nstreams` streams of one HS_MODE_STREAM literal database whose
  * state (7 look-behind bytes + count, 64-bit offset: 16 bytes per stream) stays
